@@ -62,7 +62,9 @@ typedef struct ltr_config {
                                      0 = ((m00 x + m01 y) + m02 z) + m03 (PCL <= 1.9), 1 = ((m03 + m00 x) + m01 y) + m02 z (PCL >= 1.10 SSE2) */
     int32_t keyframe_batch;       /* keyframes projected per kernel launch (0 = default) */
     int32_t fast_path;            /* 0 = reference arithmetic for every (point, keyframe) pair; 1 = exactness-preserving fast rejection path;
-                                     2 = 1 + tile-level occlusion/range culling for the scan-minus-map variants (default) */
+                                     2 = 1 + tile-level occlusion/range culling for the scan-minus-map variants (default).
+                                     With 1 or 2, ltr_parse_projected claims map tiles near to far from each launch's keyframes
+                                     (fewer running-minimum atomics; the result does not depend on the order). */
 } ltr_config;
 
 /* Fills cfg with the reference defaults (vfov 50, hfov 360, identity extrinsic, order 0). */

@@ -345,8 +345,22 @@ static void launch_fast(ltr_ctx* ctx, const DevCloud& map, const DevPoses& poses
         const int64_t total = (int64_t)nb * g.rows * g.cols;
         ctx->launches++;
         deferred_resolve_kernel<<<grid_for(total, 256, ctx->sm_count * 16), 256, 0, ctx->stream>>>(view(map), poses.d, k0, nb, ctx->d_ext, ctx->ext_identity ? 1 : 0,
-            ctx->cfg.transform_order, (uint32_t)(g.rows * g.cols), da, win);
+            ctx->cfg.transform_order, (uint32_t)(g.rows * g.cols), da, win, ctx->d_counters);
     }
+}
+
+// Near-to-far claim order of the deferred mode (DeferredArgs::order): per tile, a lower bound of its distance from `o` (a reference
+// origin of the launch's keyframes) quantised to 1/16 m and saturated at 4096 m in key bits 32..47, the tile index in bits 0..31.
+// Sorting bits 32..47 (two 8-bit radix passes) keeps equal distances in map order.  The order only changes how fast `best` fills.
+constexpr float kOrderSteps = 16.0f;   // per metre
+__global__ void __launch_bounds__(256) tile_order_key_kernel(const float4* __restrict__ tiles, long long ntiles, float ox, float oy, float oz,
+                                                             uint64_t* __restrict__ keys) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= ntiles) return;
+    const float4 s = tiles[t];
+    const float dx = s.x - ox, dy = s.y - oy, dz = s.z - oz;
+    const float q = fminf(fmaxf((sqrtf(dx * dx + dy * dy + dz * dz) - s.w) * kOrderSteps, 0.0f), 65535.0f);   // NaN -> 0
+    keys[t] = ((uint64_t)(uint32_t)q << 32) | (uint64_t)t;
 }
 
 // scratch of the deferred true-minimum mode for launches of up to B keyframes: best image + overflow list + its counter
@@ -569,11 +583,25 @@ static int parse_projected_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_poses poses_h
     if (K > 0 && mapc.n > 0) {
         const int B = std::max(1, std::min(std::min(ctx->cfg.keyframe_batch, use_fast ? kFastMaxBatch : 400), K));
         if (use_deferred) LTR_TRY(deferred_alloc(ctx, B, npx, &p_def, &da));
-        void *p_win = nullptr, *p_amin = nullptr;
-        ScratchGuard g_win(ctx, &p_win), g_amin(ctx, &p_amin);
+        void *p_win = nullptr, *p_amin = nullptr, *p_tiles = nullptr, *p_keys = nullptr;
+        ScratchGuard g_win(ctx, &p_win), g_amin(ctx, &p_amin), g_tiles(ctx, &p_tiles), g_keys(ctx, &p_keys);
         LTR_TRY(dev_alloc(ctx, &p_win, (size_t)B * npx * sizeof(uint64_t)));
-        if (use_fast) LTR_TRY(dev_alloc(ctx, &p_amin, (size_t)B * npx * sizeof(uint32_t)));
+        if (use_fast && !use_deferred) LTR_TRY(dev_alloc(ctx, &p_amin, (size_t)B * npx * sizeof(uint32_t)));   // the deferred mode keeps `best` instead
         uint32_t* amin = (uint32_t*)p_amin;
+        // deferred mode: the tiles are claimed near to far from each launch's keyframes (DeferredArgs::order); their bounding spheres
+        // are computed once per call
+        const bool use_order = use_deferred && mapc.n >= kTilePts;
+        const long long ntiles = (mapc.n + kTilePts - 1) / kTilePts;
+        uint64_t* keys = nullptr;
+        if (use_order) {
+            LTR_TRY(dev_alloc(ctx, &p_tiles, (size_t)ntiles * sizeof(float4)));
+            LTR_TRY(dev_alloc(ctx, &p_keys, (size_t)ntiles * 2 * sizeof(uint64_t)));
+            keys = (uint64_t*)p_keys;
+            tile_sphere_kernel<<<(unsigned)((ntiles * 32 + 255) / 256), 256, 0, ctx->stream>>>(view(mapc), (float4*)p_tiles, ntiles);
+            LTR_LAUNCH_CHECK(ctx);
+        }
+        CullArgs no_cull;
+        std::memset(&no_cull, 0, sizeof(no_cull));
         LTR_TRY(dev_alloc(ctx, &p_list, (size_t)K * npx * sizeof(uint32_t)));
         const int nchunk = (int)((npx + kParseChunk - 1) / kParseChunk);
         LTR_TRY(dev_alloc(ctx, &p_cnt, ((size_t)K + (size_t)B * nchunk) * sizeof(unsigned int)));
@@ -585,13 +613,24 @@ static int parse_projected_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_poses poses_h
             const int nb = std::min(B, K - k0);
             prof_begin(ctx);
             launch_units.push_back(nb);
-            if (use_fast) {
+            if (use_deferred) {
+                if (use_order) {
+                    // reference origin of the launch: the mean sensor origin of its keyframes (KfFast::chi)
+                    double o[3] = {0.0, 0.0, 0.0};
+                    for (int k = 0; k < nb; ++k)
+                        for (int d = 0; d < 3; ++d) o[d] += (double)posc.h_fast[(size_t)(kf_begin + k0 + k) * 16 + 9 + d] / nb;
+                    tile_order_key_kernel<<<(unsigned)((ntiles + 255) / 256), 256, 0, ctx->stream>>>((const float4*)p_tiles, ntiles, (float)o[0], (float)o[1],
+                                                                                                      (float)o[2], keys);
+                    LTR_LAUNCH_CHECK(ctx);
+                    uint64_t* sorted = nullptr;
+                    LTR_TRY(radix_sort_pairs(ctx, keys, keys + ntiles, nullptr, nullptr, ntiles, 32, 48, &sorted, nullptr));
+                    da.order = (const unsigned long long*)sorted;
+                }
+                launch_fast<false, true>(ctx, mapc, posc, kf_begin + k0, nb, g, fc, nullptr, nullptr, 0.0f, win, nullptr, no_cull, da);
+            } else if (use_fast) {
                 fill_u32_kernel<<<grid_for(nb * npx, 256, ctx->sm_count * 8), 256, 0, ctx->stream>>>(amin, 0x7f800000u, nb * npx);
                 LTR_LAUNCH_CHECK(ctx);
-                CullArgs no_cull;
-                std::memset(&no_cull, 0, sizeof(no_cull));
-                if (use_deferred) launch_fast<false, true>(ctx, mapc, posc, kf_begin + k0, nb, g, fc, nullptr, amin, 0.0f, win, amin, no_cull, da);
-                else launch_fast<false>(ctx, mapc, posc, kf_begin + k0, nb, g, fc, nullptr, amin, 0.0f, win, amin, no_cull);
+                launch_fast<false>(ctx, mapc, posc, kf_begin + k0, nb, g, fc, nullptr, amin, 0.0f, win, amin, no_cull);
             } else {
                 const unsigned mb = (unsigned)((mapc.n + 255) / 256);
                 map_project_kernel<false><<<mb, 256, (size_t)nb * 12 * sizeof(double), ctx->stream>>>(view(mapc), posc.d, kf_begin + k0, nb, ctx->d_ext,
@@ -607,6 +646,8 @@ static int parse_projected_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_poses poses_h
         }
         g_win.release();
         g_amin.release();
+        g_tiles.release();
+        g_keys.release();
         std::vector<unsigned int> cnt((size_t)K);
         unsigned int h_over = 0;
         LTR_CUDA(ctx, cudaMemcpyAsync(cnt.data(), p_cnt, (size_t)K * sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));

@@ -263,12 +263,16 @@ struct KfBatch { float kf[kFastMaxBatch][16]; };
 // deferred_resolve_kernel then evaluates exactly the final best of every pixel and the list entries (a few per cent of a pixel
 // count instead of tens of per cent of all pairs).  A full list sets `overflow_count` beyond the capacity; the host then repeats the
 // call with the immediate mode.
+// With `order`, the warps claim the tiles near to far from the keyframes of the launch, so that `best` holds near surfaces before
+// the far tiles arrive: a pixel's running minimum drops fewer times, so fewer pairs issue the returning atomic.  The order cannot
+// change a result: the argument above holds for any order in which the pairs arrive (DESIGN.md 4.1).
 struct DeferredArgs {
     unsigned long long* best;      // [keyframes in launch][npx], initialised to ~0
     unsigned long long* list;      // overflow entries: q_pack(index, pixel, keyframe)
     unsigned int* count;           // entries appended by the current launch (may exceed capacity)
     unsigned int* overflow;        // set to 1 when that happened (sticky over the launches of a call)
     unsigned int capacity;
+    const unsigned long long* order;   // tile claim order (low 32 bits: tile index), or nullptr: map order
 };
 
 template <bool kCandidatesOnly, bool kElDirect, bool kDeferred = false>
@@ -299,8 +303,8 @@ __global__ void __launch_bounds__(kFastThreads, kFastCtasPerSm) map_project_fast
     unsigned tile_u = 0;
     if (lane == 0) tile_u = atomicAdd(work_counter, 1u);
     tile_u = __shfl_sync(0xffffffffu, tile_u, 0);
-    const long long tile = (long long)tile_u;
-    if (tile >= total_tiles) break;
+    if ((long long)tile_u >= total_tiles) break;
+    const long long tile = (kDeferred && da.order) ? (long long)(uint32_t)da.order[tile_u] : (long long)tile_u;
     const int64_t base = (int64_t)tile * (32 * kFastPts) + lane;
     float px_[kFastPts], py_[kFastPts], pz_[kFastPts];
 #pragma unroll
@@ -322,8 +326,8 @@ __global__ void __launch_bounds__(kFastThreads, kFastCtasPerSm) map_project_fast
         if ((cull_mask >> k) & 1u) continue;         // warp-uniform (ballot)
         const float* __restrict__ kf = kb.kf[k];
         const bool kf_ok = kf[15] != 0.0f;
-        const uint32_t* __restrict__ test_k = test_img + (size_t)k * npx;    // this keyframe's images
-        uint32_t* __restrict__ amin_k = approx_min + (size_t)k * npx;
+        const uint32_t* __restrict__ test_k = kDeferred ? nullptr : test_img + (size_t)k * npx;    // this keyframe's images
+        uint32_t* __restrict__ amin_k = kDeferred ? nullptr : approx_min + (size_t)k * npx;
         unsigned long long* __restrict__ best_k = kDeferred ? da.best + (size_t)k * npx : nullptr;
         // Phase 1, branch-free: project the thread's points and ISSUE all their image gathers, so that the (mostly L2) latencies of
         // the four loads overlap instead of being paid one after the other behind a branch each.
@@ -366,6 +370,7 @@ __global__ void __launch_bounds__(kFastThreads, kFastCtasPerSm) map_project_fast
                 if (lead_[j]) {
                     const uint32_t mi = (uint32_t)(base + j * 32 < map.n ? base + j * 32 : map.n - 1);
                     old_[j] = atomicMin(&best_k[pxl_[j]], ((unsigned long long)__float_as_uint(fr) << 32) | mi);
+                    ++n_atomics;
                 }
             }
 #pragma unroll
@@ -444,7 +449,8 @@ __global__ void __launch_bounds__(kFastThreads, kFastCtasPerSm) map_project_fast
         exact_full_pair<kCandidatesOnly>(map, s_qb[lane], poses, kf0, ext, ext_identity, order, g, scan_rimg, thres, win, fc.empty_scan_shortcut, &n_atomics);
         ++n_b;
     }
-    // statistics: [0] pairs through the exact-range path, [1] atomics on the winner image, [2] pairs through the full exact path, [3] culled pairs
+    // statistics: [0] pairs through the exact-range path (deferred mode: deferred_resolve_kernel adds the list entries), [1] atomics on
+    // the winner image (deferred mode: plus those on `best`), [2] pairs through the full exact path, [3] culled pairs
     for (int o = 16; o > 0; o >>= 1) {
         n_a += __shfl_down_sync(0xffffffffu, n_a, o); n_b += __shfl_down_sync(0xffffffffu, n_b, o); n_atomics += __shfl_down_sync(0xffffffffu, n_atomics, o);
     }
@@ -457,10 +463,14 @@ __global__ void __launch_bounds__(kFastThreads, kFastCtasPerSm) map_project_fast
 // Deferred true-minimum mode, second half: the exact (range, index) key of the final best pair of every pixel and of every list entry
 // goes into the winner image with the same 64-bit atomicMin as everywhere else.
 __global__ void __launch_bounds__(256) deferred_resolve_kernel(PtrView map, const double* __restrict__ poses, int kf0, int nb, const double* __restrict__ ext,
-                                                               int ext_identity, int order, uint32_t npx, DeferredArgs da, uint64_t* __restrict__ win) {
+                                                               int ext_identity, int order, uint32_t npx, DeferredArgs da, uint64_t* __restrict__ win,
+                                                               unsigned long long* __restrict__ counters) {
     const int64_t total = (int64_t)nb * npx;
     const unsigned n_list = min(*da.count, da.capacity);
-    if (blockIdx.x == 0 && threadIdx.x == 0 && *da.count > da.capacity) *da.overflow = 1u;
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        if (*da.count > da.capacity) *da.overflow = 1u;
+        if (counters) atomicAdd(&counters[0], (unsigned long long)*da.count);   // list appends: pairs through the exact-range path
+    }
     for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total + n_list; t += (int64_t)gridDim.x * blockDim.x) {
         unsigned long long e;
         if (t < total) {

@@ -331,7 +331,7 @@ constexpr size_t kRsScatterSmemKeys = (size_t)kRsTile * sizeof(uint64_t);       
 
 // Sorts (keys0, vals0) on the key bits [bit_lo, bit_hi) using (keys1, vals1) as the other half of the ping-pong; *keys_sorted /
 // *vals_sorted point at the result.  vals0 == nullptr: keys only.
-static int radix_sort_pairs(ltr_ctx* ctx, uint64_t* keys0, uint64_t* keys1, uint32_t* vals0, uint32_t* vals1, int64_t n, int bit_lo, int bit_hi,
+int radix_sort_pairs(ltr_ctx* ctx, uint64_t* keys0, uint64_t* keys1, uint32_t* vals0, uint32_t* vals1, int64_t n, int bit_lo, int bit_hi,
                             uint64_t** keys_sorted, uint32_t** vals_sorted) {
     *keys_sorted = keys0;
     if (vals_sorted) *vals_sorted = vals0;
