@@ -156,11 +156,13 @@ int ltr_parse_projected(ltr_ctx* ctx, ltr_cloud map, ltr_poses poses, int32_t kf
  * partition{Low,High}DynamicPointsOfScanByKnn (Session.cpp:537-642): every point of keyframe k (poses index
  * pose_offset + k) is moved to the global frame (as written in the reference: base2lidar first, then the pose),
  * its k nearest SQUARED distances to `target` are averaged ((float)sum_double / float(k)) and compared with thr;
- * |avg| < thr -> coexist else diff; both partitions are moved back with global2local.  Either output may be NULL. */
+ * |avg| < thr -> coexist else diff; both partitions are moved back with global2local.  Either output may be NULL.
+ * With any query point, a target of k or more points with a non-finite coordinate fails with LTR_ERR_UNSUPPORTED. */
 int ltr_knn_diff(ltr_ctx* ctx, ltr_scanset scans, ltr_poses poses, int32_t pose_offset, ltr_cloud target, int32_t k, float thr,
                  ltr_scanset* out_coexist, ltr_scanset* out_diff);
 /* Same decision rule for a flat cloud already in the target's frame (no transforms):
- * Session::removeWeakNDMapPointsHavingStrongNDInNear (Session.cpp:452-484). near = |avg| < thr, far = the rest. */
+ * Session::removeWeakNDMapPointsHavingStrongNDInNear (Session.cpp:452-484). near = |avg| < thr, far = the rest.
+ * With any query point, a target of k or more points with a non-finite coordinate fails with LTR_ERR_UNSUPPORTED. */
 int ltr_knn_split_cloud(ltr_ctx* ctx, ltr_cloud query, ltr_cloud target, int32_t k, float thr, ltr_cloud* out_near, ltr_cloud* out_far);
 
 /* ---- multi-GPU exchange points (NCCL, on the context's stream; libnccl is dlopen'ed at first use) ----------------

@@ -196,7 +196,11 @@ struct GridBuf {
 
 static int build_grid(ltr_ctx* ctx, const DevCloud& target, int k, float thr, GridBuf* gb) {
     float mn[3], mx[3];
-    LTR_TRY(minmax_xyz(ctx, target, mn, mx));
+    uint32_t nonfinite = 0;
+    LTR_TRY(minmax_xyz(ctx, target, mn, mx, &nonfinite));
+    // an infinite or NaN extent would keep the cell loop below from ever terminating.  Targets of the path are voxelised maps,
+    // which the voxeliser has already checked, so nothing reproduces PCL's skipping of invalid points here.
+    if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite target coordinates (%u points)", nonfinite);
     const double reach = std::sqrt((double)k * (double)thr) * 1.001 + 1e-6;
     double cell = reach;
     // bound the dense grid to 2^29 cells by growing the cell (exactness only needs cell >= reach)
@@ -313,14 +317,14 @@ int ltr_knn_split_cloud(ltr_ctx* ctx, ltr_cloud query_h, ltr_cloud target_h, int
     if (tp->n < 1) return fail(ctx, LTR_ERR_UNSUPPORTED, "empty target (PCL's nearestKSearch asserts on an empty tree)");
     const bool small = tp->n < k;
     const DevCloud q = *qp, target = *tp;
-    LTR_TRY(cloud_new(ctx, q.n, out_near));
-    LTR_TRY(cloud_new(ctx, q.n, out_far));
-    if (q.n == 0) return LTR_OK;
     GridBuf gb;
     ScratchGuard g_grid(ctx, &gb.block);
     PtrView small_view{nullptr, nullptr, nullptr, nullptr, 0};
     if (small) small_view = view(target);
-    else LTR_TRY(build_grid(ctx, target, k, thr, &gb));
+    else if (q.n > 0) LTR_TRY(build_grid(ctx, target, k, thr, &gb));   // before the outputs exist, so that a rejected target leaks nothing
+    LTR_TRY(cloud_new(ctx, q.n, out_near));
+    LTR_TRY(cloud_new(ctx, q.n, out_far));
+    if (q.n == 0) return LTR_OK;
     void* p = nullptr;
     ScratchGuard g_p(ctx, &p);
     LTR_TRY(dev_alloc(ctx, &p, (size_t)q.n));

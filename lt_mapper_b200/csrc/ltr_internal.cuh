@@ -169,7 +169,8 @@ int stable_partition_by_flag(ltr_ctx* ctx, const DevCloud& in, const uint8_t* fl
                              DevCloud* out_unflagged, DevCloud* out_flagged);   // outputs must be pre-allocated with cap >= in.n
 int count_flags(ltr_ctx* ctx, const uint8_t* flags, int64_t n, int64_t* count);
 int exclusive_scan_u32(ltr_ctx* ctx, const uint32_t* in, uint32_t* out, int64_t n);  // out[n] elements; returns via out
-int minmax_xyz(ltr_ctx* ctx, const DevCloud& c, float mn[3], float mx[3]);
+// *nonfinite (if non-null): number of points with a non-finite x, y or z (NaN coordinates do not show in mn / mx)
+int minmax_xyz(ltr_ctx* ctx, const DevCloud& c, float mn[3], float mx[3], uint32_t* nonfinite = nullptr);
 // stable LSD radix sort of (keys0, vals0) on the key bits [bit_lo, bit_hi), 8 bits per pass, ping-ponging with (keys1, vals1);
 // *keys_sorted / *vals_sorted point at whichever buffer holds the result.  vals0 == vals1 == nullptr: keys only.
 int radix_sort_pairs(ltr_ctx* ctx, uint64_t* keys0, uint64_t* keys1, uint32_t* vals0, uint32_t* vals1, int64_t n, int bit_lo, int bit_hi,

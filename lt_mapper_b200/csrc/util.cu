@@ -375,40 +375,49 @@ static inline float ord2f(uint32_t o) {
     float f; memcpy(&f, &u, 4); return f;
 }
 
-__global__ void __launch_bounds__(256) minmax_kernel(PtrView c, uint32_t* __restrict__ out /* 6: min xyz, max xyz (ordered encoding) */) {
+// nonfinite (may be null): incremented by the number of points with a non-finite x, y or z.  fminf / fmaxf skip NaN, so the
+// extrema alone do not reveal them (an all-NaN cloud leaves the initial encodings, which decode to NaN).
+__global__ void __launch_bounds__(256) minmax_kernel(PtrView c, uint32_t* __restrict__ out /* 6: min xyz, max xyz (ordered encoding) */,
+                                                     uint32_t* __restrict__ nonfinite) {
     float mn[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, mx[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
+    uint32_t bad = 0;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < c.n; i += (int64_t)gridDim.x * blockDim.x) {
         const float x = c.x[i], y = c.y[i], z = c.z[i];
         mn[0] = fminf(mn[0], x); mn[1] = fminf(mn[1], y); mn[2] = fminf(mn[2], z);
         mx[0] = fmaxf(mx[0], x); mx[1] = fmaxf(mx[1], y); mx[2] = fmaxf(mx[2], z);
+        bad += (isfinite(x) && isfinite(y) && isfinite(z)) ? 0u : 1u;
     }
     for (int d = 0; d < 3; ++d)
         for (int o = 16; o > 0; o >>= 1) {
             mn[d] = fminf(mn[d], __shfl_down_sync(0xffffffffu, mn[d], o));
             mx[d] = fmaxf(mx[d], __shfl_down_sync(0xffffffffu, mx[d], o));
         }
-    if ((threadIdx.x & 31) == 0)
+    for (int o = 16; o > 0; o >>= 1) bad += __shfl_down_sync(0xffffffffu, bad, o);
+    if ((threadIdx.x & 31) == 0) {
         for (int d = 0; d < 3; ++d) { atomicMin(&out[d], f2ord(mn[d])); atomicMax(&out[3 + d], f2ord(mx[d])); }
+        if (nonfinite && bad) atomicAdd(nonfinite, bad);
+    }
 }
 
-static int minmax_view(ltr_ctx* ctx, const PtrView& v, float mn[3], float mx[3]) {
+static int minmax_view(ltr_ctx* ctx, const PtrView& v, float mn[3], float mx[3], uint32_t* nonfinite) {
     void* p = nullptr;
     ScratchGuard g_p(ctx, &p);
-    LTR_TRY(dev_alloc(ctx, &p, 6 * sizeof(uint32_t)));
-    uint32_t init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
+    LTR_TRY(dev_alloc(ctx, &p, 7 * sizeof(uint32_t)));
+    uint32_t init[7] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u, 0u};
     LTR_CUDA(ctx, cudaMemcpyAsync(p, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
     const int blocks = (int)std::min<int64_t>((v.n + 255) / 256, (int64_t)ctx->sm_count * 8);
-    minmax_kernel<<<std::max(blocks, 1), 256, 0, ctx->stream>>>(v, (uint32_t*)p);
+    minmax_kernel<<<std::max(blocks, 1), 256, 0, ctx->stream>>>(v, (uint32_t*)p, (uint32_t*)p + 6);
     LTR_LAUNCH_CHECK(ctx);
-    uint32_t res[6];
+    uint32_t res[7];
     LTR_CUDA(ctx, cudaMemcpyAsync(res, p, sizeof(res), cudaMemcpyDeviceToHost, ctx->stream));
     LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     g_p.release();
     for (int d = 0; d < 3; ++d) { mn[d] = ord2f(res[d]); mx[d] = ord2f(res[3 + d]); }
+    if (nonfinite) *nonfinite = res[6];
     return LTR_OK;
 }
 
-int minmax_xyz(ltr_ctx* ctx, const DevCloud& c, float mn[3], float mx[3]) { return minmax_view(ctx, view(c), mn, mx); }
+int minmax_xyz(ltr_ctx* ctx, const DevCloud& c, float mn[3], float mx[3], uint32_t* nonfinite) { return minmax_view(ctx, view(c), mn, mx, nonfinite); }
 
 // ------------------------------------------------------------------------------------------------
 // Voxel centroid == pcl::octree::OctreePointCloudVoxelCentroid as used by octreeDownsampling
@@ -554,7 +563,12 @@ static int voxel_view(ltr_ctx* ctx, const PtrView& v, float leaf, DevCloud* out,
     if (!(leaf > 0.0f)) return fail(ctx, LTR_ERR_INVALID, "voxel leaf must be positive");
     if (n >= (int64_t)1 << 31) return fail(ctx, LTR_ERR_UNSUPPORTED, "cloud too large for voxel centroid");
     float mn[3], mx[3];
-    if (!given_box) LTR_TRY(minmax_view(ctx, v, mn, mx));
+    if (!given_box) {
+        uint32_t nonfinite = 0;
+        LTR_TRY(minmax_view(ctx, v, mn, mx, &nonfinite));
+        // rejected before define_box, whose cast of ceil(inf or NaN) to unsigned is undefined
+        if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "%u points with non-finite coordinates", nonfinite);
+    }
     const VoxBox b = given_box ? *given_box : define_box(mn, mx, leaf);
     if (b.depth > 21) return fail(ctx, LTR_ERR_UNSUPPORTED, "octree depth %d > 21 (extent/leaf too large)", b.depth);
     void* p = nullptr;
@@ -671,7 +685,7 @@ static int voxel_distributed(ltr_ctx* ctx, int comm, const DevCloud& loc, float 
     LTR_CUDA(ctx, cudaMemcpyAsync(d_mm, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
     if (n > 0) {
         const int blocks = (int)std::min<int64_t>((n + 255) / 256, (int64_t)ctx->sm_count * 8);
-        minmax_kernel<<<std::max(blocks, 1), 256, 0, ctx->stream>>>(view(loc), d_mm);
+        minmax_kernel<<<std::max(blocks, 1), 256, 0, ctx->stream>>>(view(loc), d_mm, nullptr);
         LTR_LAUNCH_CHECK(ctx);
     }
     LTR_TRY(nccl_allreduce_u32(ctx, comm, d_mm, 3, 1));
