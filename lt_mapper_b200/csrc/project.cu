@@ -76,12 +76,23 @@ __global__ void __launch_bounds__(256) scan_rimg_fast_kernel(PtrView scans, cons
     atomicMin(&rimg[(size_t)k * g.rows * g.cols + (size_t)r * g.cols + c], __float_as_uint(range));
 }
 
-// test image of the scan-minus-map fast path (project_fast.cuh): the scan image with "no return" pixels set to -inf, which makes
-// "scan - range > thres" false for every range -- valid when no map point can be ~10000 m away (empty_scan_shortcut_ok)
-__global__ void __launch_bounds__(256) scan_test_image_kernel(const uint32_t* __restrict__ rimg, uint32_t* __restrict__ test_img, int64_t n) {
+// test image of the scan-minus-map fast path (project_fast.cuh) for nb keyframes: the scan image, with "no return" pixels set to -inf when
+// `empty_to_ninf` (that makes "scan - range > thres" false for every range -- valid when no map point can be ~10000 m away,
+// empty_scan_shortcut_ok).  With pad_g guard rows above and below and pad_c = 1 guard column (FastCfg::pad_*) the guard rows replicate the
+// rows that pixel_index clamps to, so the short elevation path gathers from it without clamping its index, and column 0 and the guard column
+// hold +inf: the pixels next to the azimuth seam, whose pairs map_project_fast_kernel sends to the full exact path.  pad_g = pad_c = 0: plain layout.
+__global__ void __launch_bounds__(256) scan_test_image_kernel(const uint32_t* __restrict__ rimg, uint32_t* __restrict__ test_img, int nb, int rows, int cols,
+                                                              int pad_g, int pad_c, int empty_to_ninf) {
+    const int W = cols + pad_c;
+    const int64_t per_kf = (int64_t)(rows + 2 * pad_g) * W, n = nb * per_kf;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        const uint32_t b = rimg[i];
-        test_img[i] = (b == kNoPointBits) ? 0xff800000u : b;
+        const int k = (int)(i / per_kf);
+        const int p = (int)(i - k * per_kf);
+        const int rp = p / W;
+        const int cp = p - rp * W;
+        const int r = min(max(rp - pad_g, 0), rows - 1), c = min(cp, cols - 1);
+        const uint32_t b = rimg[(size_t)k * rows * cols + (size_t)r * cols + c];
+        test_img[i] = (pad_c && (cp == 0 || cp == cols)) ? 0x7f800000u : (empty_to_ninf && b == kNoPointBits) ? 0xff800000u : b;
     }
 }
 
@@ -304,11 +315,12 @@ __global__ void __launch_bounds__(256) atan_sweep_kernel(int which, uint32_t las
     if (wb > old) *arg_bits = worst_arg;   // racy between equal-ish maxima; the argument is informational only
 }
 
-// persistent grid: 4 resident CTAs per SM (64 registers, ~22 KB shared memory each), never more CTAs than tiles need
+// persistent grid: up to 4 resident CTAs per SM (20 KB shared memory each; the 3-CTA variants leave the rest queued: the warps claim tiles
+// from a counter, so a late CTA only finds less work), never more CTAs than tiles need
 static inline unsigned fast_grid(const ltr_ctx* ctx, int64_t n) {
     const int64_t tiles = (n + 32 * kFastPts - 1) / (32 * kFastPts);
     const int64_t ctas = (tiles + kFastThreads / 32 - 1) / (kFastThreads / 32);
-    return (unsigned)std::max<int64_t>(1, std::min<int64_t>(ctas, (int64_t)ctx->sm_count * kFastCtasPerSm));
+    return (unsigned)std::max<int64_t>(1, std::min<int64_t>(ctas, (int64_t)ctx->sm_count * kFastCtasPerSmPad));
 }
 
 static inline size_t fast_smem_bytes() { return (size_t)(kFastThreads / 32) * 2 * kQueueCap * sizeof(uint64_t); }
@@ -337,7 +349,10 @@ static void launch_fast(ltr_ctx* ctx, const DevCloud& map, const DevPoses& poses
         cudaMemsetAsync(da.best, 0xff, (size_t)nb * g.rows * g.cols * sizeof(unsigned long long), ctx->stream);   // "no pair yet"
         cudaMemsetAsync(da.count, 0, sizeof(unsigned int), ctx->stream);
     }
-    if (fc.el_direct) map_project_fast_kernel<kCand, true, kDeferred><<<fb, kFastThreads, fast_smem_bytes(), ctx->stream>>>(view(map), kb, poses.d, k0, nb, ctx->d_ext,
+    if (kCand && !kDeferred && fc.pad_ok)   // test_img is the guard-padded test image
+        map_project_fast_kernel<kCand, true, kDeferred, kCand && !kDeferred><<<fb, kFastThreads, fast_smem_bytes(), ctx->stream>>>(view(map), kb, poses.d, k0, nb,
+            ctx->d_ext, ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, g, fc, rimg, test_img, thres, win, amin, ca, ctx->d_counters, work, da);
+    else if (fc.el_direct) map_project_fast_kernel<kCand, true, kDeferred><<<fb, kFastThreads, fast_smem_bytes(), ctx->stream>>>(view(map), kb, poses.d, k0, nb, ctx->d_ext,
         ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, g, fc, rimg, test_img, thres, win, amin, ca, ctx->d_counters, work, da);
     else map_project_fast_kernel<kCand, false, kDeferred><<<fb, kFastThreads, fast_smem_bytes(), ctx->stream>>>(view(map), kb, poses.d, k0, nb, ctx->d_ext,
         ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, g, fc, rimg, test_img, thres, win, amin, ca, ctx->d_counters, work, da);
@@ -435,19 +450,15 @@ static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, 
     // tile culling (project_cull.cuh): scan-minus-map variants only, one keyframe per lane -> launches of at most 32 keyframes
     CullArgs ca;
     std::memset(&ca, 0, sizeof(ca));
-    const bool use_cull = use_fast && cand && ctx->cfg.fast_path >= 2 && B <= 32 && map->n >= kTilePts;
+    // the sliding-window maxima cost 5 stores per pixel and keyframe: below one map point per pixel they cost more than the culling saves
+    // (the small ND / PD candidate maps), so those passes project every pair
+    const bool use_cull = use_fast && cand && ctx->cfg.fast_path >= 2 && B <= 32 && map->n >= kTilePts && map->n >= npx;
     void *p_tiles = nullptr, *p_pyr = nullptr;
     ScratchGuard g_tiles(ctx, &p_tiles), g_pyr(ctx, &p_pyr);
     if (use_cull) {
         ca.enabled = 1;
         ca.ntiles = (map->n + kTilePts - 1) / kTilePts;
-        unsigned off = 0;
-        for (int L = 1; L <= kPyrLevels; ++L) {
-            const int RL = (rows + (1 << L) - 1) >> L, CL = (cols + (1 << L) - 1) >> L;
-            ca.lvl_off[L] = off; ca.lvl_cols[L] = CL;
-            off += (unsigned)(RL * CL);
-        }
-        ca.pyr_stride = off;
+        ca.pyr_stride = (unsigned)(kPyrLevels * npx);
         LTR_TRY(dev_alloc(ctx, &p_tiles, (size_t)ca.ntiles * sizeof(float4)));
         LTR_TRY(dev_alloc(ctx, &p_pyr, (size_t)B * ca.pyr_stride * sizeof(float)));
         ca.tiles = (const float4*)p_tiles; ca.pyr = (const float*)p_pyr;
@@ -460,11 +471,14 @@ static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, 
     if (map->n > 0 && kf_end > kf_begin) {
         void *p_rimg = nullptr, *p_win = nullptr;
         ScratchGuard g_rimg(ctx, &p_rimg), g_win(ctx, &p_win);
-        LTR_TRY(dev_alloc(ctx, &p_rimg, (size_t)B * npx * sizeof(uint32_t) * (use_fast ? 3 : 1)));
+        // scan-minus-map with the short elevation path and a 360 degree field of view: the test image is guard-padded (FastCfg::pad_*) and always built
+        const bool pad = use_fast && cand && fc.pad_ok;
+        const int64_t timg_px = pad ? (int64_t)fc.pad_npx : npx;
+        LTR_TRY(dev_alloc(ctx, &p_rimg, (size_t)B * (use_fast ? 2 * npx + timg_px : npx) * sizeof(uint32_t)));
         LTR_TRY(dev_alloc(ctx, &p_win, (size_t)B * npx * sizeof(uint64_t)));
         uint32_t* rimg = (uint32_t*)p_rimg;
         uint32_t* amin = rimg + (size_t)B * npx;   // approximate running minimum (fast path only)
-        uint32_t* timg = amin + (size_t)B * npx;   // test image of the scan-minus-map variants when pixels without a return can never flag
+        uint32_t* timg = amin + (size_t)B * npx;   // test image of the scan-minus-map variants (padded, or pixels without a return can never flag)
         uint64_t* win = (uint64_t*)p_win;
         const int fill_blocks = ctx->sm_count * 8;
         fill_u64_kernel<<<grid_for(B * npx, 256, fill_blocks), 256, 0, ctx->stream>>>(win, cand ? kWinNone : kWinEmpty, B * npx);
@@ -487,12 +501,14 @@ static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, 
             }
             if (use_cull) {
                 const float empty_value = shortcut ? -__builtin_huge_valf() : __builtin_huge_valf();   // empty scan pixel: never flags / unknown
-                scan_pyramid_kernel<<<(unsigned)nb, 1024, 0, ctx->stream>>>(rimg, nb, rows, cols, empty_value, ca, (float*)p_pyr);
+                const dim3 wg((unsigned)((cols + kWinTile - 1) / kWinTile), (unsigned)((rows + kWinTile - 1) / kWinTile), (unsigned)nb);
+                scan_window_max_kernel<<<wg, 256, 0, ctx->stream>>>(rimg, rows, cols, empty_value, ca.pyr_stride, (float*)p_pyr);
                 LTR_LAUNCH_CHECK(ctx);
             }
             const uint32_t* test_img = rimg;
-            if (use_fast && cand && shortcut) {
-                scan_test_image_kernel<<<grid_for(nb * npx, 256, fill_blocks), 256, 0, ctx->stream>>>(rimg, timg, nb * npx);
+            if (use_fast && cand && (shortcut || pad)) {
+                scan_test_image_kernel<<<grid_for(nb * timg_px, 256, fill_blocks), 256, 0, ctx->stream>>>(rimg, timg, nb, rows, cols, pad ? fc.pad_g : 0,
+                                                                                                         pad ? 1 : 0, shortcut);
                 LTR_LAUNCH_CHECK(ctx);
                 test_img = timg;
             }

@@ -8,7 +8,8 @@
 // then scan(px_p) - range_p <= thres for every p in the tile: no point of the tile is a candidate (SURVEY.md A.2), so all
 // 128 (point, keyframe) pairs are skipped.  This removes the map regions that are occluded in, or beyond the reach of, a
 // keyframe's scan (~30 % of all pairs on the BASELINE scene) and never changes a result.  The rectangle maximum comes
-// from a max-pyramid of the scan image (levels 1..5, at most 3 x 3 lookups).  The 32 tests of one tile against the 32
+// from sliding-window maxima of the scan image (a 2-D sparse table, windows of 2..32 pixels): four overlapping windows cover a
+// near-square rectangle exactly.  The 32 tests of one tile against the 32
 // keyframes of a launch are evaluated by the 32 lanes of the warp in parallel (one keyframe per lane) and exchanged with
 // one ballot, so the test costs ~1 % of the work it saves.
 //
@@ -18,15 +19,14 @@
 
 namespace ltr {
 
-constexpr int kPyrLevels = 5;  // levels 1..5: blocks of 2, 4, 8, 16, 32 pixels
+constexpr int kPyrLevels = 5;  // sliding-window maxima of 2x2, 4x4, 8x8, 16x16 and 32x32 pixels
 
 struct CullArgs {
     const float4* tiles;        // per 128-point tile: sphere centre xyz, radius (inflated)
     long long ntiles;
-    const float* pyr;           // [keyframes in launch][pyr_stride]: levels 1..5 of max(scan range), empty pixel -> empty_value
-    unsigned pyr_stride;
-    unsigned lvl_off[kPyrLevels + 1];
-    int lvl_cols[kPyrLevels + 1];
+    const float* pyr;           // [keyframes in launch][kPyrLevels][rows * cols]: level L at pixel (r, c) = max of the scan range over the
+                                // 2^L x 2^L window starting there (cut at the image edge), empty pixel -> empty_value
+    unsigned pyr_stride;        // kPyrLevels * rows * cols
     int enabled;
 };
 
@@ -60,39 +60,37 @@ __global__ void __launch_bounds__(256) tile_sphere_kernel(PtrView map, float4* _
     if (lane == 0) tiles[tile] = make_float4(cx, cy, cz, sqrtf(r2) * 1.00001f + 1.0e-4f);   // inflated: f32 rounding of centre / distance
 }
 
-// max-pyramid of the scan range images of one launch; level 0 is the scan image itself (float bits, 10000.0f = empty).
-// One CTA per keyframe builds level 1 from the image and every further level from the previous one (4 reads per output).
-__global__ void __launch_bounds__(1024) scan_pyramid_kernel(const uint32_t* __restrict__ scan_rimg, int nb, int rows, int cols, float empty_value,
-                                                            CullArgs ca, float* __restrict__ pyr) {
-    const int k = blockIdx.x;
-    if (k >= nb) return;
-    const uint32_t* img = scan_rimg + (size_t)k * rows * cols;
-    float* P = pyr + (size_t)k * ca.pyr_stride;
+// Sliding-window maxima (a 2-D sparse table) of the scan range images of one launch: level L at (r, c) is the maximum of the scan range
+// over the 2^L x 2^L window starting at (r, c), cut at the image edge (10000.0f = empty -> empty_value).  One CTA per 32 x 32 output
+// pixels of one keyframe: it loads the 63 x 63 pixels those windows reach (-inf beyond the edge, which is the same as cutting the window)
+// and builds level L from level L - 1 in shared memory, max of (r, c), (r, c + h), (r + h, c), (r + h, c + h), h = 2^(L-1).
+constexpr int kWinTile = 32, kWinSpan = kWinTile + (1 << kPyrLevels) - 1;   // 63
+__global__ void __launch_bounds__(256) scan_window_max_kernel(const uint32_t* __restrict__ scan_rimg, int rows, int cols, float empty_value,
+                                                              unsigned pyr_stride, float* __restrict__ pyr) {
+    __shared__ float buf[2][kWinSpan][kWinSpan + 1];
+    const int k = blockIdx.z, r0 = blockIdx.y * kWinTile, c0 = blockIdx.x * kWinTile, npx = rows * cols;
+    const uint32_t* img = scan_rimg + (size_t)k * npx;
     const float ninf = -__int_as_float(0x7f800000);
-    int pr = rows, pc = cols;                       // dimensions of the previous level
+    for (int e = threadIdx.x; e < kWinSpan * kWinSpan; e += blockDim.x) {
+        const int y = e / kWinSpan, x = e - y * kWinSpan, r = r0 + y, c = c0 + x;
+        float v = ninf;
+        if (r < rows && c < cols) { const uint32_t b = img[r * cols + c]; v = (b == 0x461C4000u) ? empty_value : __uint_as_float(b); }
+        buf[0][y][x] = v;
+    }
+    __syncthreads();
+    float* out = pyr + (size_t)k * pyr_stride;
+    int span = kWinSpan;
     for (int L = 1; L <= kPyrLevels; ++L) {
-        const int RL = (pr + 1) >> 1, CL = (pc + 1) >> 1;
-        float* out = P + ca.lvl_off[L];
-        const float* prev = (L > 1) ? P + ca.lvl_off[L - 1] : nullptr;
-        for (int e = threadIdx.x; e < RL * CL; e += blockDim.x) {
-            const int br = e / CL, bc = e - br * CL;
-            float m = ninf;
-#pragma unroll
-            for (int dr = 0; dr < 2; ++dr)
-#pragma unroll
-                for (int dc = 0; dc < 2; ++dc) {
-                    const int r = 2 * br + dr, c = 2 * bc + dc;
-                    if (r < pr && c < pc) {
-                        float v;
-                        if (L == 1) { const uint32_t b = img[(size_t)r * cols + c]; v = (b == 0x461C4000u) ? empty_value : __uint_as_float(b); }
-                        else v = prev[r * pc + c];
-                        m = fmaxf(m, v);
-                    }
-                }
-            out[e] = m;
+        const int h = 1 << (L - 1), src = (L - 1) & 1;
+        span -= h;                                   // level L is needed over (32 + 2^5 - 2^L)^2 pixels
+        for (int e = threadIdx.x; e < span * span; e += blockDim.x) {
+            const int y = e / span, x = e - y * span;
+            const float m = fmaxf(fmaxf(buf[src][y][x], buf[src][y][x + h]), fmaxf(buf[src][y + h][x], buf[src][y + h][x + h]));
+            buf[src ^ 1][y][x] = m;
+            const int r = r0 + y, c = c0 + x;
+            if (y < kWinTile && x < kWinTile && r < rows && c < cols) out[(size_t)(L - 1) * npx + r * cols + c] = m;
         }
         __syncthreads();
-        pr = RL; pc = CL;
     }
 }
 
@@ -115,15 +113,25 @@ LTR_DEV bool tile_culled(const float* __restrict__ kf, float4 tile, const FastCf
     const int c0 = (int)c0f, c1 = (int)c1f;
     const int r0 = min(max((int)fminf(fmaxf(floorf(__fsub_rn(vrow, dr)), -1.0f), 1.0e6f), 0), g.rows - 1);  // rows clamp exactly like the pixel index does
     const int r1 = min(max((int)fminf(fmaxf(ceilf(__fadd_rn(vrow, dr)), -1.0f), 1.0e6f), 0), g.rows - 1);
-    const int e = max(c1 - c0, r1 - r0) + 1;
-    int L = 32 - __clz(e - 1) - 1;                                             // blocks of 2^L >= e / 2: at most 3 x 3 blocks
-    L = max(L, 1);
-    if (L > kPyrLevels) return false;
-    const float* P = ca.pyr + (size_t)k * ca.pyr_stride + ca.lvl_off[L];
-    const int CL = ca.lvl_cols[L];
+    // cover the rectangle with windows of side s = 2^L: s <= its shorter side where possible (no window reaches beyond it), s >= a quarter of
+    // its longer side (at most 4 x 4 windows, 2 x 2 for a near-square rectangle); a side shorter than s gets one window, which reaches
+    // beyond the rectangle -- a larger set, still sound
+    const int hgt = r1 - r0 + 1, wid = c1 - c0 + 1, lo = min(hgt, wid), hi = max(hgt, wid);
+    if (hi > 64) return false;
+    int L = max(31 - __clz(lo), 30 - __clz(hi - 1));                             // max(floor(log2(lo)), ceil(log2(hi)) - 2)
+    L = min(max(L, 1), kPyrLevels);
+    const int s = 1 << L;
+    const float* P = ca.pyr + (size_t)k * ca.pyr_stride + (size_t)(L - 1) * (g.rows * g.cols);
     float smax = -__int_as_float(0x7f800000);
-    for (int br = r0 >> L; br <= (r1 >> L); ++br)
-        for (int bc = c0 >> L; bc <= (c1 >> L); ++bc) smax = fmaxf(smax, P[br * CL + bc]);
+    for (int r = r0;; r += s) {
+        const int rr = (r + s - 1 >= r1) ? max(min(r, r1 - s + 1), r0) : r;     // the last window ends at r1 (or starts at r0 when s > hgt)
+        for (int c = c0;; c += s) {
+            const int cc = (c + s - 1 >= c1) ? max(min(c, c1 - s + 1), c0) : c;
+            smax = fmaxf(smax, P[rr * g.cols + cc]);
+            if (c + s - 1 >= c1) break;
+        }
+        if (r + s - 1 >= r1) break;
+    }
     const float rmin = __fsub_rn(__fsub_rn(__fmul_rn(d, 0.999996f), tile.w), 1.0e-4f);
     return smax <= __fsub_rn(__fadd_rn(rmin, thres), 1.0e-3f);                 // scan - range <= thres - 1 mm for every point of the tile
 }

@@ -34,6 +34,14 @@ struct FastCfg {
     float mr2_rel, mr2_abs;     // 2 * m_r_rel, 2 * m_r_abs
     float neg_row_scale;
     int el_direct;              // 1: |elevation| beyond atan(0.5) clamps to the first / last row with room to spare -> short elevation path
+    // guard-padded test image of the scan-minus-map variant with the short elevation path (scan_test_image_kernel): pad_g rows above and
+    // below replicate the first / last row, and one guard column follows the last; pixel (r, c) is at (r + pad_g) * (cols + 1) + c
+    int pad_ok;                 // 1: el_direct and a 360 degree field of view (columns in [0, cols], the seam at columns 0 / cols)
+    int pad_g;                  // rows the short path can reach beyond either edge of the image
+    int pad_npx;                // (rows + 2 pad_g) * (cols + 1): padded pixels per keyframe
+    uint32_t pad_w;             // cols + 1
+    uint32_t pad_bias;          // 0x4B400000 (cols + 2) - pad_g (cols + 1), modulo 2^32 (see map_project_fast_kernel)
+    uint32_t pad_last;          // pad_npx - 1
 };
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -89,6 +97,16 @@ __host__ inline FastCfg make_fast_cfg(int rows, int cols, float vfov, float hfov
     f.rel_m1 = f.m_r_rel - 1.0f;
     f.mr2_rel = 2.0f * f.m_r_rel; f.mr2_abs = 2.0f * f.m_r_abs;
     f.neg_row_scale = -f.row_scale;
+    // the short path's elevation is |fast_atan_half(t)| <= atan(0.5) + kElPolyErr; the rows it rounds to, with 1e-3 px for the f32 pixel arithmetic
+    const double el_max = std::atan(0.5) + kElPolyErr;
+    const int r_top = (int)std::floor(0.5 * rows - el_max * ppr_r - 1.0e-3 + 0.5);
+    const int r_bot = (int)std::floor(0.5 * rows + el_max * ppr_r + 1.0e-3 + 0.5);
+    f.pad_ok = (f.el_direct && hfov == 360.0f) ? 1 : 0;
+    f.pad_g = f.pad_ok ? std::max(std::max(-r_top, r_bot - (rows - 1)), 0) : 0;
+    f.pad_npx = (rows + 2 * f.pad_g) * (cols + 1);
+    f.pad_w = (uint32_t)(cols + 1);
+    f.pad_bias = 0x4B400000u * (uint32_t)(cols + 2) - (uint32_t)(f.pad_g * (cols + 1));   // bits of 1.5 * 2^23 + i are 0x4B400000 + i for |i| < 2^22
+    f.pad_last = (uint32_t)f.pad_npx - 1u;
     return f;
 }
 
@@ -232,8 +250,14 @@ __device__ __noinline__ void exact_full_pair(const PtrView& map, uint64_t e, con
 #include "project_cull.cuh"
 namespace ltr {
 
+// the same pointer, opaque to the compiler: indexing it costs one IMAD.WIDE instead of re-deriving the 64-bit element offset per load
+LTR_DEV const uint32_t* opaque_ptr(const uint32_t* p) { asm("mov.b64 %0, %0;" : "+l"(p)); return p; }
+
 constexpr int kFastThreads = 256;
-constexpr int kFastCtasPerSm = 3;   // 85 registers per thread: the per-keyframe and image constants stay in registers across the 4 points of a step
+constexpr int kFastCtasPerSm = 3;   // 80 registers per thread: the per-keyframe and image constants stay in registers across the 4 points of a step
+// The guard-padded variant (HD / revert / PD passes) fits 64 registers without spills and runs 4 CTAs per SM: the kernel waits on its
+// (mostly L2) image gathers rather than on instruction issue, and the fourth CTA hides more of that latency (DESIGN.md 4.1)
+constexpr int kFastCtasPerSmPad = 4;
 constexpr int kFastPts = 4;      // map points per thread (registers); lane l of a warp holds points tile * 128 + 32 j + l
 constexpr int kQueueCap = 160;   // per warp and kind: < 32 left over + 4 * 32 pushed per keyframe step
 constexpr int kFastMaxBatch = 32;   // keyframes per launch: their constants travel as a kernel parameter (constant bank)
@@ -250,9 +274,11 @@ struct KfBatch { float kf[kFastMaxBatch][16]; };
 // for the pixel.  A pair whose approximate range exceeds it by more than twice the range margin is provably farther than an
 // already-queued pair and cannot win the pixel, so it is dropped without exact arithmetic.
 //
-// Hot loop (profiles/sass_mix.py prints its SASS mix): the kernel is issue-bound, so the common "no effect" path is one straight line
-// per point -- transform (12), azimuth (16), ranges (7), elevation (10), pixel + certainty (14), one gather + compare (5) -- and
-// rare pairs reserve a queue slot with a shared-memory atomic (no ballots on the common path).
+// Hot loop (profiles/sass_mix.py prints its SASS mix): the common "no effect" path is one straight line per point -- transform,
+// azimuth, ranges, elevation, certainty, and (guard-padded variant) one IMAD + one unsigned min for the gather index: 64 instructions
+// per point, 44 of them FP32 arithmetic -- and rare pairs reserve a queue slot with a shared-memory atomic (no ballots on the common
+// path).  Measured on an H100, the kernel waits on its image gathers more than on instruction issue: cutting that line from 76 to 64
+// instructions alone did not shorten it; the fourth CTA per SM that the 64 registers of the padded variant allow did (DESIGN.md 4.1).
 // Deferred true-minimum mode (kDeferred; ND pass and visible-point extraction).  The pixel winner is the point of minimum EXACT
 // range (lowest index on ties); an approximate range is within `band/2 = m_r_abs + m_r_rel r` of the exact one.  Instead of sending
 // every running minimum through the exact arithmetic (on Morton-ordered surface patches that was 44 % of all pairs), the scan only
@@ -275,27 +301,35 @@ struct DeferredArgs {
     const unsigned long long* order;   // tile claim order (low 32 bits: tile index), or nullptr: map order
 };
 
-template <bool kCandidatesOnly, bool kElDirect, bool kDeferred = false>
-__global__ void __launch_bounds__(kFastThreads, kFastCtasPerSm) map_project_fast_kernel(PtrView map, const __grid_constant__ KfBatch kb, const double* __restrict__ poses,
+template <bool kCandidatesOnly, bool kElDirect, bool kDeferred = false, bool kPad = false>
+__global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFastCtasPerSm) map_project_fast_kernel(PtrView map, const __grid_constant__ KfBatch kb, const double* __restrict__ poses,
                                                                         int kf0, int nb, const double* __restrict__ ext, int ext_identity, int order,
                                                                         ImgShape g, const __grid_constant__ FastCfg fc, const uint32_t* __restrict__ scan_rimg,
                                                                         const uint32_t* __restrict__ test_img, float thres,
                                                                         uint64_t* __restrict__ win, uint32_t* __restrict__ approx_min,
                                                                         CullArgs ca, unsigned long long* __restrict__ counters,
                                                                         unsigned int* __restrict__ work_counter, DeferredArgs da) {
+    // kPad (scan-minus-map, short elevation path, 360 degree field of view): the test image is guard-padded (FastCfg::pad_*), so the
+    // gather needs no index clamp
+    static_assert(!kPad || (kCandidatesOnly && kElDirect && !kDeferred), "the padded test image exists for the scan-minus-map short path only");
     extern __shared__ uint64_t s_queues[];
     const int warp = threadIdx.x >> 5;
     uint64_t* s_qa = s_queues + warp * (2 * kQueueCap);
     uint64_t* s_qb = s_qa + kQueueCap;
     __shared__ int s_cnt[kFastThreads / 32][2];
+    __shared__ unsigned s_stat[kFastThreads / 32][3];   // per warp: pairs through the exact-range / full exact path, culled (tile, keyframe) tests
     if ((threadIdx.x & 31) < 2) s_cnt[warp][threadIdx.x & 31] = 0;
+    if ((threadIdx.x & 31) < 3) s_stat[warp][threadIdx.x & 31] = 0;
     __syncthreads();
     const unsigned lane = threadIdx.x & 31;
     const uint32_t npx = (uint32_t)(g.rows * g.cols);
     const int hi_c = g.cols - 1, hi_r = g.rows - 1;
     const float kMagic = 12582912.0f;            // 1.5 * 2^23: v + kMagic has the nearest integer in its low mantissa bits
     const float thr_lo = thres - fc.m_r_abs;
-    unsigned n_a = 0, n_b = 0, n_atomics = 0, n_culled = 0;
+    unsigned n_atomics = 0;
+#ifdef LTR_PROBE_NOMAYBE
+    unsigned n_nomaybe = 0;
+#endif
     // Persistent warps: each warp claims 128-point tiles from a global counter until the map is exhausted, so warps whose
     // tiles are culled in many keyframes do not leave issue slots idle while their CTA-mates finish.
     const long long total_tiles = (map.n + (32 * kFastPts) - 1) / (32 * kFastPts);
@@ -320,19 +354,24 @@ __global__ void __launch_bounds__(kFastThreads, kFastCtasPerSm) map_project_fast
         const float4 t = ca.tiles[tile];
         const bool c = ((int)lane < nb) && tile_culled(kb.kf[lane], t, fc, g, ca, (int)lane, thres);
         cull_mask = __ballot_sync(0xffffffffu, c);
-        if (lane == 0) n_culled += __popc(cull_mask);
+        if (lane == 0) s_stat[warp][2] += __popc(cull_mask);
     }
     for (int k = 0; k < nb; ++k) {                    // a plain counted loop: k stays provably warp-uniform, so kb.kf[k] is read with LDCU
         if ((cull_mask >> k) & 1u) continue;         // warp-uniform (ballot)
         const float* __restrict__ kf = kb.kf[k];
-        const bool kf_ok = kf[15] != 0.0f;
-        const uint32_t* __restrict__ test_k = kDeferred ? nullptr : test_img + (size_t)k * npx;    // this keyframe's images
+        if (kf[15] == 0.0f) {                         // warp-uniform: no fast constants (non-rigid pose or extrinsic) -> all pairs exact
+#pragma unroll
+            for (int j = 0; j < kFastPts; ++j)
+                s_qb[atomicAdd(&s_cnt[warp][1], 1)] = q_pack((uint32_t)(base + j * 32 < map.n ? base + j * 32 : map.n - 1), 0u, (uint32_t)k);
+        } else {
+        // this keyframe's images (kPad: the padded test image)
+        const uint32_t* __restrict__ test_k = kDeferred ? nullptr : kPad ? opaque_ptr(test_img + (uint32_t)(k * fc.pad_npx)) : test_img + (size_t)k * npx;
         uint32_t* __restrict__ amin_k = kDeferred ? nullptr : approx_min + (size_t)k * npx;
         unsigned long long* __restrict__ best_k = kDeferred ? da.best + (size_t)k * npx : nullptr;
         // Phase 1, branch-free: project the thread's points and ISSUE all their image gathers, so that the (mostly L2) latencies of
         // the four loads overlap instead of being paid one after the other behind a branch each.
         float fr_[kFastPts], tv_[kFastPts];
-        uint32_t pxl_[kFastPts];
+        uint32_t pxl_[kFastPts];   // kPad: bits of the float index, else the pixel
         bool certain_[kFastPts];
 #pragma unroll
         for (int j = 0; j < kFastPts; ++j) {
@@ -342,14 +381,28 @@ __global__ void __launch_bounds__(kFastThreads, kFastCtasPerSm) map_project_fast
             const float yc = __fadd_rn(vcol, kMagic), yr = __fadd_rn(vrow, kMagic);
             const float dc = fabsf(__fsub_rn(vcol, __fsub_rn(yc, kMagic)));   // distance to the nearest integer (NaN stays NaN)
             const float dr = fabsf(__fsub_rn(vrow, __fsub_rn(yr, kMagic)));
-            const int c = min(max(__float_as_int(yc) - 0x4B400000, 0), hi_c);   // NaN -> some in-range pixel; such a pair is never "certain"
-            const int r = min(max(__float_as_int(yr) - 0x4B400000, 0), hi_r);
             // certain <=> both coordinates are farther than their margin from a rounding boundary (false for NaN)
-            certain_[j] = kf_ok & (__fmaf_rn(fc.m_col_b, f.rho_inv_r, dc) < fc.lim_c) & (dr < fc.lim_r);
-            pxl_[j] = (uint32_t)(r * g.cols + c);
+            certain_[j] = (__fmaf_rn(fc.m_col_b, f.rho_inv_r, dc) < fc.lim_c) & (dr < fc.lim_r);
             fr_[j] = f.r;
-            // unconditional: the index is always inside the image (deferred mode: the range word of the pixel's best pair)
-            tv_[j] = kDeferred ? __uint_as_float(reinterpret_cast<const uint32_t*>(best_k)[2 * pxl_[j] + 1]) : __uint_as_float(test_k[pxl_[j]]);
+            if (kPad) {
+                // guard-padded test image (scan_test_image_kernel): the rounded row n_r = yr - kMagic lies in [-g, R - 1 + g] and the rounded
+                // column in [0, C] (FastCfg::pad_*); the guard rows replicate the first / last row, which pixel_index clamps to.  Columns 0 and C
+                // hold +inf: there the azimuth is within half a pixel of +-pi, and a sensor-frame y that is zero or within the transform error
+                // of it may have the other sign in the reference, which puts the pair on the other side of the seam (column 0 <-> C - 1) even
+                // though the column looks certain.  +inf makes every such pair `maybe`, and the maybe branch sends it to the full exact path.
+                // The bits of yr and yc are 0x4B400000 + n_r and 0x4B400000 + n_c, so bits(yr) (C + 1) + bits(yc) - pad_bias is, modulo 2^32,
+                // the padded index (n_r + g)(C + 1) + n_c: one IMAD.  One unsigned min keeps every other value inside the image: a NaN, or an
+                // azimuth that left [-pi, pi] (denormal sensor-frame coordinates, rcp -> inf); neither pair is certain.
+                const uint32_t pp = min(__float_as_uint(yr) * fc.pad_w + __float_as_uint(yc) - fc.pad_bias, fc.pad_last);
+                pxl_[j] = pp;
+                tv_[j] = __uint_as_float(__ldg(test_k + pp));   // one IMAD.WIDE.U32 from the keyframe's base
+            } else {
+                const int c = min(max(__float_as_int(yc) - 0x4B400000, 0), hi_c);   // NaN -> some in-range pixel; such a pair is never "certain"
+                const int r = min(max(__float_as_int(yr) - 0x4B400000, 0), hi_r);
+                pxl_[j] = (uint32_t)(r * g.cols + c);
+                // unconditional: the index is always inside the image (deferred mode: the range word of the pixel's best pair)
+                tv_[j] = kDeferred ? __uint_as_float(reinterpret_cast<const uint32_t*>(best_k)[2 * pxl_[j] + 1]) : __uint_as_float(test_k[pxl_[j]]);
+            }
         }
         // Phase 2: decide.  Almost every pair ends at the first comparison.
         if (kDeferred) {
@@ -396,15 +449,32 @@ __global__ void __launch_bounds__(kFastThreads, kFastCtasPerSm) map_project_fast
                 }
             }
         } else {
+#ifdef LTR_PROBE_NOMAYBE
+        bool any_maybe = false;
+#endif
 #pragma unroll
         for (int j = 0; j < kFastPts; ++j) {
             const float fr = fr_[j], tv = tv_[j];
-            const uint32_t pxl = pxl_[j];
             if (certain_[j]) {
                 bool maybe;
                 if (kCandidatesOnly) maybe = !(__fmaf_rn(fr, fc.rel_m1, tv) < thr_lo);   // scan - r + m_rel r >= thres - m_abs for some range within the margin
                 else maybe = !(fr > __fadd_rn(tv, __fmaf_rn(fc.mr2_rel, fr, fc.mr2_abs)));   // not provably farther than an already-queued pair
+#ifdef LTR_PROBE_NOMAYBE
+                any_maybe |= maybe;
+#endif
                 if (maybe) {
+                    uint32_t pxl = pxl_[j];
+                    bool seam = false;
+                    if (kPad) {   // padded index -> pixel of the unpadded images (approx_min, queue entries, exact path)
+                        const uint32_t rp = pxl / (uint32_t)(g.cols + 1);
+                        const int col = (int)(pxl - rp * (uint32_t)(g.cols + 1));
+                        seam = (col == 0) | (col == g.cols);   // +inf in the test image: the reference may put the pair across the seam
+                        pxl = (uint32_t)(min(max((int)rp - fc.pad_g, 0), hi_r) * g.cols + min(col, hi_c));
+                    }
+                    if (kPad && seam) {
+                        s_qb[atomicAdd(&s_cnt[warp][1], 1)] = q_pack((uint32_t)(base + j * 32 < map.n ? base + j * 32 : map.n - 1), 0u, (uint32_t)k);
+                        continue;
+                    }
                     bool push = true;
                     if (kCandidatesOnly) {
                         const float cur = __uint_as_float(amin_k[pxl]);
@@ -417,7 +487,13 @@ __global__ void __launch_bounds__(kFastThreads, kFastCtasPerSm) map_project_fast
                 s_qb[atomicAdd(&s_cnt[warp][1], 1)] = q_pack((uint32_t)(base + j * 32 < map.n ? base + j * 32 : map.n - 1), 0u, (uint32_t)k);
             }
         }
+#ifdef LTR_PROBE_NOMAYBE
+        // diagnostic build of profiles/hd_pass_probe.py only: counts the non-culled (tile, keyframe) iterations in which no lane took the
+        // `maybe` branch -- what any tile-level cull could still remove -- and reports them in place of the atomics count
+        if (!__any_sync(0xffffffffu, any_maybe) && lane == 0) ++n_nomaybe;
+#endif
         }
+        }  // keyframe with fast constants
         __syncwarp();
         int qa = *(volatile int*)&s_cnt[warp][0];
         int qb = *(volatile int*)&s_cnt[warp][1];
@@ -426,13 +502,13 @@ __global__ void __launch_bounds__(kFastThreads, kFastCtasPerSm) map_project_fast
                 qa -= 32;
                 const uint64_t e = s_qa[qa + lane];
                 exact_range_pair<kCandidatesOnly>(map, e, poses, kf0, ext, ext_identity, order, npx, scan_rimg, thres, win, fc.empty_scan_shortcut, &n_atomics);
-                ++n_a;
+                if (lane == 0) s_stat[warp][0] += 32;
             }
             while (qb >= 32) {
                 qb -= 32;
                 const uint64_t e = s_qb[qb + lane];
                 exact_full_pair<kCandidatesOnly>(map, e, poses, kf0, ext, ext_identity, order, g, scan_rimg, thres, win, fc.empty_scan_shortcut, &n_atomics);
-                ++n_b;
+                if (lane == 0) s_stat[warp][1] += 32;
             }
             __syncwarp();
             if (lane == 0) { s_cnt[warp][0] = qa; s_cnt[warp][1] = qb; }
@@ -443,18 +519,20 @@ __global__ void __launch_bounds__(kFastThreads, kFastCtasPerSm) map_project_fast
     const int qa = *(volatile int*)&s_cnt[warp][0], qb = *(volatile int*)&s_cnt[warp][1];
     if ((int)lane < qa) {
         exact_range_pair<kCandidatesOnly>(map, s_qa[lane], poses, kf0, ext, ext_identity, order, npx, scan_rimg, thres, win, fc.empty_scan_shortcut, &n_atomics);
-        ++n_a;
     }
     if ((int)lane < qb) {
         exact_full_pair<kCandidatesOnly>(map, s_qb[lane], poses, kf0, ext, ext_identity, order, g, scan_rimg, thres, win, fc.empty_scan_shortcut, &n_atomics);
-        ++n_b;
     }
     // statistics: [0] pairs through the exact-range path (deferred mode: deferred_resolve_kernel adds the list entries), [1] atomics on
     // the winner image (deferred mode: plus those on `best`), [2] pairs through the full exact path, [3] culled pairs
+#ifdef LTR_PROBE_NOMAYBE
+    n_atomics = n_nomaybe;
+#endif
     for (int o = 16; o > 0; o >>= 1) {
-        n_a += __shfl_down_sync(0xffffffffu, n_a, o); n_b += __shfl_down_sync(0xffffffffu, n_b, o); n_atomics += __shfl_down_sync(0xffffffffu, n_atomics, o);
+        n_atomics += __shfl_down_sync(0xffffffffu, n_atomics, o);
     }
     if (lane == 0 && counters) {
+        const unsigned n_a = s_stat[warp][0] + (unsigned)qa, n_b = s_stat[warp][1] + (unsigned)qb, n_culled = s_stat[warp][2];
         atomicAdd(&counters[0], (unsigned long long)n_a); atomicAdd(&counters[1], (unsigned long long)n_atomics); atomicAdd(&counters[2], (unsigned long long)n_b);
         if (n_culled) atomicAdd(&counters[3], (unsigned long long)n_culled * (32ull * kFastPts));   // pairs skipped by tile culling
     }

@@ -43,7 +43,8 @@ def classify(ins):
 
 
 def main():
-    pat = sys.argv[1] if len(sys.argv) > 1 else "map_project_fast_kernelILb1ELb1"
+    # default: the variant the HD / revert passes run (candidates only, short elevation path, not deferred, guard-padded test image)
+    pat = sys.argv[1] if len(sys.argv) > 1 else "map_project_fast_kernelILb1ELb1ELb0ELb1"
     sass = kernel_sass(pat)
     # hot window = one keyframe step of the k loop: the densest cluster of 8 MUFU.RSQ (4 points x 2) marks phase 1; the window runs from
     # the first register-indexed constant load before it (the per-keyframe constants) to the shared-memory queue test after the step
@@ -79,8 +80,9 @@ def main():
     for name, n in sorted(cnt.items(), key=lambda kv: -kv[1]):
         print(f"| {name} | {n} | {n / pts:.1f} |")
     print(f"| **all** | **{len(win)}** | **{len(win) / pts:.1f}** |")
-    # common path: instructions before the first conditional branch of phase 2 + 3 per decision
-    br = [i for i, s in enumerate(win) if s.startswith("BRA") or " BRA " in s]
+    # common path: instructions before the first conditional branch of phase 2 + 3 per decision (the warp-uniform branch that sends a keyframe
+    # without fast constants to the exact path precedes phase 1 and is part of the straight line)
+    br = [i for i, s in enumerate(win) if (s.startswith("BRA") or " BRA " in s) and i > lo - first]
     common = br[0] if br else len(win)
     cc = collections.Counter(classify(s) for s in win[:common])
     print(f"\nStraight-line part before the first decision branch (the work EVERY pair pays): {common} instructions = {common / pts:.1f} per point:\n")
