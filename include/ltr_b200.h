@@ -201,7 +201,7 @@ int ltr_debug_pixel_index(ltr_ctx* ctx, const float* xyz /* n*3 */, int64_t n, i
  * fast_path is on): rows*cols floats, 10000.0f = no point.  Lets tests compare the image itself, not only what is derived from it. */
 int ltr_debug_scan_rimg(ltr_ctx* ctx, ltr_scanset scans, int32_t kf, float res_alpha, float* rimg /* rows*cols */);
 /* Fast-path validation: for n map points and one inverse pose, writes per point 8 floats:
- * fast pre-round column, fast pre-round row, fast range, r/rho | reference pre-round column, row, range, 0;
+ * fast pre-round column, fast pre-round row, fast range, r/rho | reference pre-round column, row, range, fast azimuth [rad];
  * margins4 (optional) = column margin a, column margin b (x r/rho), row margin, relative range margin. */
 int ltr_debug_fast_project(ltr_ctx* ctx, const float* xyz /* n*3 */, int64_t n, const double* inv_pose16, float res_alpha,
                            float* out8 /* n*8 */, float* margins4);
@@ -209,9 +209,10 @@ int ltr_debug_fast_project(ltr_ctx* ctx, const float* xyz /* n*3 */, int64_t n, 
  * which = 1 -> every float of [0, 0.5] through the short elevation polynomial; returns max |poly(a) - atan(a)| (atan in double) and
  * the argument where it occurs.  The error budget of the margins (project_fast.cuh) quotes these two numbers. */
 int ltr_debug_atan_sweep(ltr_ctx* ctx, int32_t which, double* max_abs_err, float* arg_at_max);
-/* margins8 of ltr_debug_margins: column margin a, column margin b (x r/rho), row margin, relative range margin, absolute range margin [m],
- * el_direct flag, and the derived (un-inflated) column / row error bounds in pixels at r/rho = 1 */
-int ltr_debug_margins(ltr_ctx* ctx, float res_alpha, float* margins8);
+/* margins9 of ltr_debug_margins: column margin a, column margin b (x r/rho), row margin, relative range margin, absolute range margin [m],
+ * el_direct flag, the derived (un-inflated) column / row error bounds in pixels at r/rho = 1, and the seam limit [rad]: a fast azimuth
+ * with |az| >= it is never certain (half a pixel short of +-pi) */
+int ltr_debug_margins(ltr_ctx* ctx, float res_alpha, float* margins9);
 /* resetRimgSize (utility.cpp:222-236) */
 void ltr_reset_rimg_size(float vfov, float hfov, float alpha, int32_t* rows, int32_t* cols);
 /* Statistics of the last ltr_remove_pass / ltr_parse_projected: [0] (point, keyframe) pairs projected, [1] pairs settled by

@@ -361,7 +361,7 @@ class Context:
         return e.value, a.value
 
     def debug_margins(self, res_alpha):
-        m = np.zeros(8, np.float32)
+        m = np.zeros(9, np.float32)
         self._ck(lib().ltr_debug_margins(self._h, res_alpha, m.ctypes.data))
         return m
 

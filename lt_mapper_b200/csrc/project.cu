@@ -14,6 +14,7 @@
 #include "project_fast.cuh"
 #include <algorithm>
 #include <cmath>
+#include <cstdlib>
 #include <cstring>
 
 namespace ltr {
@@ -279,7 +280,7 @@ static int empty_scan_shortcut_ok(ltr_ctx* ctx, const DevCloud& map, const DevPo
 template <bool kElDirect>
 __global__ void debug_fast_kernel(const float* __restrict__ xyz, int64_t n, const float* __restrict__ kf, const double* __restrict__ pose,
                                   const double* __restrict__ ext, int ext_identity, int order, ImgShape g, FastCfg fc,
-                                  float* __restrict__ out /* n x 8: vcol_f vrow_f r_f rho_inv_r | vcol_e vrow_e r_e unused */) {
+                                  float* __restrict__ out /* n x 8: vcol_f vrow_f r_f rho_inv_r | vcol_e vrow_e r_e az_f */) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const float x = xyz[3 * i], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
@@ -296,7 +297,7 @@ __global__ void debug_fast_kernel(const float* __restrict__ xyz, int64_t n, cons
     out[8 * i + 4] = fm((float)g.cols, fd(fa(rad2deg(s.az), fd(g.hfov, 2.0f)), fs(g.hfov, 0.0f)));
     out[8 * i + 5] = fm((float)g.rows, fs(1.0f, fd(fa(rad2deg(s.el), fd(g.vfov, 2.0f)), fs(g.vfov, 0.0f))));
     out[8 * i + 6] = s.r;
-    out[8 * i + 7] = 0.0f;
+    out[8 * i + 7] = f.az;   // the fast azimuth, for the seam rule of map_project_fast_kernel
 }
 
 // Exhaustive check of the two arctangent polynomials of the fast path: every float a with bits in [0, last_bits] (i.e. all of [0, 1]
@@ -381,13 +382,17 @@ __global__ void __launch_bounds__(256) tile_order_key_kernel(const float4* __res
 // scratch of the deferred true-minimum mode for launches of up to B keyframes: best image + overflow list + its counter
 constexpr unsigned kDeferredListCap = 8u << 20;   // entries (64 MB); a typical launch appends a few 10^4
 static int deferred_alloc(ltr_ctx* ctx, int B, int64_t npx, void** block, DeferredArgs* da) {
+    // Test knob: LTR_DEFERRED_LIST_CAP=n (clamped to kDeferredListCap) shrinks the list the launches may fill, so that tests can make it
+    // overflow and exercise the immediate-mode retry of ltr_remove_pass / ltr_parse_projected on small inputs.
+    unsigned cap = kDeferredListCap;
+    if (const char* e = std::getenv("LTR_DEFERRED_LIST_CAP")) if (*e) cap = (unsigned)std::min<long long>(std::max(std::atoll(e), 0ll), kDeferredListCap);
     const size_t best_bytes = (size_t)B * npx * sizeof(unsigned long long);
     LTR_TRY(dev_alloc(ctx, block, best_bytes + (size_t)kDeferredListCap * sizeof(unsigned long long) + 256));
     da->best = (unsigned long long*)*block;
     da->list = da->best + (size_t)B * npx;
     da->count = (unsigned int*)(da->list + kDeferredListCap);
     da->overflow = da->count + 1;
-    da->capacity = kDeferredListCap;
+    da->capacity = cap;
     LTR_CUDA(ctx, cudaMemsetAsync(da->count, 0, 2 * sizeof(unsigned int), ctx->stream));
     return LTR_OK;
 }
@@ -729,6 +734,7 @@ int ltr_debug_margins(ltr_ctx* ctx, float res_alpha, float* m) {
     const FastCfg fc = make_fast_cfg(rows, cols, ctx->cfg.vfov_deg, ctx->cfg.hfov_deg, 0);
     m[0] = fc.m_col_a; m[1] = fc.m_col_b; m[2] = fc.m_row; m[3] = fc.m_r_rel; m[4] = fc.m_r_abs; m[5] = (float)fc.el_direct;
     m[6] = (float)((fc.m_col_a + fc.m_col_b) / kMarginSafety); m[7] = (float)(fc.m_row / kMarginSafety);
+    m[8] = fc.az_seam_lim;
     return LTR_OK;
 }
 

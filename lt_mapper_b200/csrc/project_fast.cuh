@@ -42,6 +42,7 @@ struct FastCfg {
     uint32_t pad_w;             // cols + 1
     uint32_t pad_bias;          // 0x4B400000 (cols + 2) - pad_g (cols + 1), modulo 2^32 (see map_project_fast_kernel)
     uint32_t pad_last;          // pad_npx - 1
+    float az_seam_lim;          // pi - 0.5 / col_scale: a fast azimuth at least this close to +-pi is never certain (map_project_fast_kernel)
 };
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -97,6 +98,9 @@ __host__ inline FastCfg make_fast_cfg(int rows, int cols, float vfov, float hfov
     f.rel_m1 = f.m_r_rel - 1.0f;
     f.mr2_rel = 2.0f * f.m_r_rel; f.mr2_abs = 2.0f * f.m_r_abs;
     f.neg_row_scale = -f.row_scale;
+    // half a pixel of azimuth short of the seam (rounding the double to f32 moves it by at most 1.2e-7 rad, a thousandth of a pixel
+    // at 1 000 px per radian; the band only has to hold the pairs within their column margin of the seam, see the kernel)
+    f.az_seam_lim = (float)(kPi - 0.5 / ppr_c);
     // the short path's elevation is |fast_atan_half(t)| <= atan(0.5) + kElPolyErr; the rows it rounds to, with 1e-3 px for the f32 pixel arithmetic
     const double el_max = std::atan(0.5) + kElPolyErr;
     const int r_top = (int)std::floor(0.5 * rows - el_max * ppr_r - 1.0e-3 + 0.5);
@@ -381,8 +385,13 @@ __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFast
             const float yc = __fadd_rn(vcol, kMagic), yr = __fadd_rn(vrow, kMagic);
             const float dc = fabsf(__fsub_rn(vcol, __fsub_rn(yc, kMagic)));   // distance to the nearest integer (NaN stays NaN)
             const float dr = fabsf(__fsub_rn(vrow, __fsub_rn(yr, kMagic)));
-            // certain <=> both coordinates are farther than their margin from a rounding boundary (false for NaN)
-            certain_[j] = (__fmaf_rn(fc.m_col_b, f.rho_inv_r, dc) < fc.lim_c) & (dr < fc.lim_r);
+            // certain <=> both coordinates are farther than their margin from a rounding boundary (false for NaN), and the azimuth is not
+            // within half a pixel of +-pi.  The seam rule: a sensor-frame y that is zero or within the transform error of zero may have the
+            // other sign in the reference, which then puts the pair on the other side of the seam (column 0 <-> C - 1 at 360 degrees, the
+            // opposite clamped edge otherwise) although the fast column looks certain.  The column margin bounds the azimuth error modulo
+            // 2 pi, so such a pair's fast azimuth is within its margin of +-pi, and a certain pair's margin is below half a pixel: the band
+            // holds every such pair, which then takes the full exact path.  NaN compares false.  kPad keeps its sentinel columns instead.
+            certain_[j] = (__fmaf_rn(fc.m_col_b, f.rho_inv_r, dc) < fc.lim_c) & (dr < fc.lim_r) & (kPad || fabsf(f.az) < fc.az_seam_lim);
             fr_[j] = f.r;
             if (kPad) {
                 // guard-padded test image (scan_test_image_kernel): the rounded row n_r = yr - kMagic lies in [-g, R - 1 + g] and the rounded

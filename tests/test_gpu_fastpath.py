@@ -26,6 +26,43 @@ K_AZ_POLY_ERR = 6.8e-7     # project_fast.cuh kAzPolyErr
 K_EL_POLY_ERR = 0.9e-7     # project_fast.cuh kElPolyErr
 
 
+def _adversarial_world(rng, pose, n):
+    """Points in the sensor frame with log-uniform range 0.5 .. 150 m, all directions, plus near-axis and near-seam sets, in the world frame."""
+    d = rng.normal(size=(n, 3)); d /= np.linalg.norm(d, axis=1, keepdims=True)
+    d[: n // 8, :2] *= 1e-3                                     # near the vertical axis (ill-conditioned azimuth)
+    d[n // 8: n // 4, 1] = rng.uniform(-1e-4, 1e-4, n // 8); d[n // 8: n // 4, 0] = -np.abs(d[n // 8: n // 4, 0])   # azimuth seam +-pi
+    r = np.exp(rng.uniform(np.log(0.5), np.log(150.0), n))[:, None]
+    return ((d * r) @ pose[:3, :3].T + pose[:3, 3]).astype(np.float32)
+
+
+def _certain(out, mg):
+    """map_project_fast_kernel's certainty test on ltr_debug_fast_project's output (margins and seam limit of ltr_debug_margins)."""
+    magic = np.float32(12582912.0)
+    with np.errstate(invalid="ignore", over="ignore"):
+        vcol, vrow = out[:, 0], out[:, 1]
+        dc = np.abs(vcol - ((vcol + magic) - magic)); dr = np.abs(vrow - ((vrow + magic) - magic))
+        lhs = (np.float64(mg[1]) * out[:, 3] + dc).astype(np.float32)
+        return (lhs < np.float32(0.5) - mg[0]) & (dr < np.float32(0.5) - mg[2]) & (np.abs(out[:, 7]) < mg[8])
+
+
+def _clamped(v_fast, v_ref, n):
+    """Fast index (round half to even, the kernel's magic-number rounding) and reference index (std::round), both clamped to [0, n)."""
+    with np.errstate(invalid="ignore"):
+        return (np.clip(np.rint(v_fast.astype(np.float64)), 0, n - 1),
+                np.clip(np.sign(v_ref) * np.floor(np.abs(v_ref.astype(np.float64)) + 0.5), 0, n - 1))
+
+
+def _assert_certain_pixels_match(out, mg, rows, cols):
+    """The statement the kernel relies on: a pair it calls certain has the reference's clamped column and row.  (A wrapped column
+    distance hides a pair placed across the seam, and at hfov < 360 the two sides of the seam clamp to opposite edges.)"""
+    c = _certain(out, mg)
+    fc, ec = _clamped(out[:, 0], out[:, 4], cols)
+    fr, er = _clamped(out[:, 1], out[:, 5], rows)
+    assert not (c & (fc != ec)).any(), out[c & (fc != ec)][:3]
+    assert not (c & (fr != er)).any(), out[c & (fr != er)][:3]
+    return c
+
+
 def test_atan_polynomials_exhaustive():
     """All 1 065 353 217 floats of [0, 1] through the azimuth polynomial and all 1 056 964 609 floats of [0, 0.5] through the short
     elevation polynomial, against atan() in double: the maxima must not exceed the constants of the error budget."""
@@ -45,20 +82,15 @@ def test_margins_dominate_measured_deviation(alpha):
         for trial in range(6):
             pose = _random_pose(rng, big=trial % 2 == 1)
             inv = np.linalg.inv(pose)
-            n = 2_000_000
-            # points in the sensor frame with log-uniform range 0.5 .. 150 m, all directions, plus near-axis and near-seam sets
-            d = rng.normal(size=(n, 3)); d /= np.linalg.norm(d, axis=1, keepdims=True)
-            d[: n // 8, :2] *= 1e-3                                     # near the vertical axis (ill-conditioned azimuth)
-            d[n // 8: n // 4, 1] = rng.uniform(-1e-4, 1e-4, n // 8); d[n // 8: n // 4, 0] = -np.abs(d[n // 8: n // 4, 0])   # azimuth seam +-pi
-            r = np.exp(rng.uniform(np.log(0.5), np.log(150.0), n))[:, None]
-            local = d * r
-            world = (local @ pose[:3, :3].T + pose[:3, 3]).astype(np.float32)
+            world = _adversarial_world(rng, pose, 2_000_000)
             out, mg = ctx.debug_fast_project(world, inv, alpha)
             el_direct = bool(ctx.debug_margins(alpha)[5])
             ok = np.isfinite(out).all(axis=1)
             o = out[ok].astype(np.float64)
             rows, cols = ltr.reset_rimg_size(alpha)
-            dcol = np.abs(o[:, 0] - o[:, 4]); dcol = np.minimum(dcol, cols - dcol)     # the seam wraps
+            _assert_certain_pixels_match(out, ctx.debug_margins(alpha), rows, cols)
+            # the error magnitude: at 360 degrees the seam wraps (the pixel itself is checked just above)
+            dcol = np.abs(o[:, 0] - o[:, 4]); dcol = np.minimum(dcol, cols - dcol)
             m_col = mg[0] + mg[1] * o[:, 3]
             m_row = mg[2]
             m_r = mg[3] * o[:, 2] + 5e-6
@@ -81,6 +113,31 @@ def test_margins_dominate_measured_deviation(alpha):
     print("max deviation / margin (col, row, range):", worst)
     # the margins are the derived bound x K_MARGIN_SAFETY: the measured deviation must stay below the DERIVED bound itself
     assert (worst * K_MARGIN_SAFETY < 1.0).all(), worst
+
+
+@pytest.mark.parametrize("vfov,hfov", [(50.0, 360.0), (50.0, 359.0), (33.2, 180.0)])
+def test_certain_pairs_keep_the_reference_pixel(vfov, hfov):
+    """Every pair the certainty test calls certain has the reference's clamped column and row, on the adversarial geometry of the margin
+    test and on points exactly on the seam of a keyframe turned by 90 degrees about z: there the fast sensor-frame y of a point below the
+    sensor is -0 where the reference's is +0, so the fast azimuth is -pi and the reference's +pi."""
+    rng = np.random.default_rng(43)
+    quarter = np.eye(4); quarter[:3, :3] = [[0, -1, 0], [1, 0, 0], [0, 0, 1]]; quarter[:3, 3] = [3.25, -7.5, 1.125]
+    quarter_inv = np.eye(4); quarter_inv[:3, :3] = quarter[:3, :3].T; quarter_inv[:3, 3] = -quarter[:3, :3].T @ quarter[:3, 3]
+    n_seam = 4000
+    el = rng.uniform(-1.4, 1.4, n_seam); r = rng.uniform(0.5, 100.0, n_seam)
+    seam = np.stack([-r * np.cos(el), np.where(rng.random(n_seam) < 0.5, 0.0, -0.0), r * np.sin(el)], 1)   # azimuth exactly +-pi
+    seam_world = (seam @ quarter[:3, :3].T + quarter[:3, 3]).astype(np.float32)
+    with ltr.Context(vfov=vfov, hfov=hfov) as ctx:
+        for alpha in (2.5, 1.0):
+            rows, cols = ltr.reset_rimg_size(alpha, vfov, hfov)
+            mg = ctx.debug_margins(alpha)
+            for pose, inv, extra in ((_random_pose(rng), None, None), (_random_pose(rng, big=True), None, None), (quarter, quarter_inv, seam_world)):
+                world = _adversarial_world(rng, pose, 500_000)
+                if extra is not None:
+                    world = np.concatenate([world, extra])
+                out, _ = ctx.debug_fast_project(world, np.linalg.inv(pose) if inv is None else inv, alpha)
+                c = _assert_certain_pixels_match(out, mg, rows, cols)
+                assert c.mean() > 0.5
 
 
 @pytest.mark.parametrize("mode,alpha", [(ltr.MODE_HD, 2.5), (ltr.MODE_HD, 1.0), (ltr.MODE_PD, 2.5), (ltr.MODE_ND, 2.5)])
