@@ -134,9 +134,17 @@ int ltr_voxel_centroid_per_keyframe(ltr_ctx* ctx, ltr_scanset in, float leaf, lt
  * (1 = in the reference's dynamic_point_indexes set).  With accumulate != 0 the new flags are OR-ed
  * into the existing ones of the same map (keyframe-sharded multi-GPU: each rank calls with its own
  * keyframe range, then the flag arrays are max-reduced across ranks).
- * n_dynamic (optional) receives the number of flagged points of this context after the pass. */
+ * n_dynamic (optional) receives the number of flagged points of this context after the pass.
+ * The scan-side images of a pass (scan range image, test image, sliding-window maxima) do not depend on the map: the context
+ * keeps those of the last two (scan set, poses, keyframe range, image shape) combinations, so a later pass on the same scans at
+ * the same resolution does not rebuild them.  They are dropped when the scan set or the poses are freed and by
+ * ltr_scan_images_release.  Their two storage blocks are kept for the next sets until ltr_scan_images_release(ctx, 1),
+ * ltr_destroy or an allocation that runs out of memory, and never exceed a quarter of the memory the context could still use
+ * (environment: LTR_SCAN_IMAGE_CACHE_MB=n caps them at n MiB; 0 builds the images per launch, without keeping them). */
 int ltr_remove_pass(ltr_ctx* ctx, ltr_cloud map, ltr_scanset scans, ltr_poses poses, int32_t kf_begin, int32_t kf_end,
                     int32_t mode, float res_alpha, float diff_thres, int32_t accumulate, int64_t* n_dynamic);
+/* Drops the scan-side images ltr_remove_pass keeps; free_storage != 0 also returns their storage to the context's allocator cache. */
+int ltr_scan_images_release(ltr_ctx* ctx, int32_t free_storage);
 /* Device pointer to the N flag bytes of the last ltr_remove_pass on `map` (for an all-reduce hook). */
 int ltr_flags_device_ptr(ltr_ctx* ctx, ltr_cloud map, uint8_t** flags, int64_t* n);
 int ltr_flags_download(ltr_ctx* ctx, ltr_cloud map, uint8_t* flags, int64_t capacity);

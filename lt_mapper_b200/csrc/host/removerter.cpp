@@ -638,6 +638,7 @@ int Removerter::run_step3() {
 }
 
 int Removerter::reset_to_step0() {
+    CK(ltr_scan_images_release(ctx, 0));   // their storage stays for the next step's sets
     for (Session* s : {&central_sess_, &query_sess_}) {
         auto it = saved.find("OriginalNoisy" + s->sess_type_ + "MapGlobal");
         if (!owns(*s)) {   // session-split: everything held of the other session was derived after Step 0

@@ -43,8 +43,10 @@ int dev_alloc(ltr_ctx* ctx, void** p, size_t bytes) {
         return LTR_OK;
     }
     cudaError_t e = cudaMalloc(p, want);
-    if (e == cudaErrorMemoryAllocation && !ctx->free_blocks.empty()) {   // give the cache back and retry once
+    const bool can_drop_images = scan_images_have_storage(ctx) && !ctx->scan_images_busy;
+    if (e == cudaErrorMemoryAllocation && (!ctx->free_blocks.empty() || can_drop_images)) {   // give the cache back and retry once
         cudaGetLastError();
+        if (can_drop_images) scan_images_release(ctx, 0, true);   // the scan-image storage of ltr_remove_pass goes first (into the cache, freed below)
         cudaStreamSynchronize(ctx->stream);
         for (auto& kv : ctx->free_blocks) cudaFree(kv.second);
         ctx->free_blocks.clear();
@@ -120,7 +122,7 @@ int scanset_new(ltr_ctx* ctx, const std::vector<int64_t>& off, ltr_scanset* out)
     for (size_t i = 0; i < ctx->scansets.size(); ++i) if (!ctx->scansets[i].used) { slot = (int)i; break; }
     if (slot < 0) { ctx->scansets.push_back(DevScanSet()); slot = (int)ctx->scansets.size() - 1; }
     DevScanSet s;
-    s.K = K; s.h_off = off; s.used = true;
+    s.K = K; s.h_off = off; s.used = true; s.serial = ++ctx->next_serial;
     s.pts.n = off[K]; s.pts.cap = round_cap(off[K]); s.pts.used = true;
     void *p_pts = nullptr, *p_off = nullptr;
     ScratchGuard g_pts(ctx, &p_pts), g_off(ctx, &p_off);   // disarmed once the handle owns both blocks
@@ -300,6 +302,7 @@ void ltr_destroy(ltr_ctx* ctx) {
     cudaSetDevice(ctx->device);
     if (ctx->trace) ltr_trace_dump(ctx, 1);
     for (size_t i = 0; i < ctx->nccl.size(); ++i) if (ctx->nccl[i].used) ltr_nccl_destroy(ctx, (int32_t)i);
+    scan_images_release(ctx, 0, true);
     for (auto& c : ctx->clouds) if (c.used) cloud_release(ctx, &c);
     for (auto& s : ctx->scansets) if (s.used) { cloud_release(ctx, &s.pts); dev_free(ctx, s.d_off); }
     for (auto& p : ctx->poses) if (p.used) { dev_free(ctx, p.d); dev_free(ctx, p.d_fast); }
@@ -453,6 +456,7 @@ int ltr_scanset_free(ltr_ctx* ctx, ltr_scanset s) {
     ApiTrace tr__(ctx, "ltr_scanset_free");
     DevScanSet* ss;
     LTR_TRY(scanset_get(ctx, s, &ss));
+    scan_images_release(ctx, ss->serial, false);
     cloud_release(ctx, &ss->pts);
     dev_free(ctx, ss->d_off);
     *ss = DevScanSet();
@@ -496,7 +500,7 @@ int ltr_poses_upload(ltr_ctx* ctx, const double* poses, const double* inv_poses,
     for (size_t i = 0; i < ctx->poses.size(); ++i) if (!ctx->poses[i].used) { slot = (int)i; break; }
     if (slot < 0) { ctx->poses.push_back(DevPoses()); slot = (int)ctx->poses.size() - 1; }
     DevPoses p;
-    p.K = K; p.used = true;
+    p.K = K; p.used = true; p.serial = ++ctx->next_serial;
     p.h.resize((size_t)K * 24);
     for (int k = 0; k < K; ++k) {
         std::memcpy(&p.h[(size_t)k * 24], inv_poses + (size_t)k * 16, 12 * sizeof(double));
@@ -521,6 +525,7 @@ int ltr_poses_free(ltr_ctx* ctx, ltr_poses h) {
     ApiTrace tr__(ctx, "ltr_poses_free");
     DevPoses* p;
     LTR_TRY(poses_get(ctx, h, &p));
+    scan_images_release(ctx, p->serial, false);
     dev_free(ctx, p->d);
     dev_free(ctx, p->d_fast);
     *p = DevPoses();

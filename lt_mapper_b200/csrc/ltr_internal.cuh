@@ -30,6 +30,7 @@ struct DevScanSet {
     int64_t* d_off = nullptr;      // K+1 device offsets
     int K = 0;
     bool used = false;
+    uint64_t serial = 0;           // ltr_ctx::next_serial at creation; the points are written only by the call that creates the set
 };
 
 // 24 doubles per keyframe: inverse pose rows 0..2 (12) then pose rows 0..2 (12), row-major 3x4
@@ -40,6 +41,27 @@ struct DevPoses {
     std::vector<float> h_fast;
     int K = 0;
     bool used = false;
+    uint64_t serial = 0;           // as DevScanSet::serial
+};
+
+// Scan-side images of ltr_remove_pass for the keyframes [kf_begin, kf_end) of one scan set (project.cu, scan_images_get), kept between
+// passes: they depend on the scans and the image shape, never on the map.  Matched on the serials of the scan set and the poses, which are
+// never reused, so a set can never be served for a freed handle whose slot was handed out again.  Each of the context's kMaxScanImageSets
+// slots owns one storage block that outlives the sets it holds (dropping a set only marks the slot empty), so the step's passes reuse
+// two blocks instead of allocating and freeing multi-GB images.
+constexpr int kMaxScanImageSets = 2;   // remove(r), revert(0.95 r), remove(r) alternate between two resolutions
+struct ScanImageSet {
+    void* block = nullptr;        // storage: rimg | timg | pyr
+    size_t cap = 0;               // its bytes
+    bool valid = false;           // holds the images of the key below
+    uint64_t scans_serial = 0, poses_serial = 0;
+    int kf_begin = 0, kf_end = 0, rows = 0, cols = 0, order = 0, ext_identity = 0, fast_path = 0;
+    float vfov = 0.0f, hfov = 0.0f;
+    uint32_t* rimg = nullptr;     // scan range images, (kf_end - kf_begin) x rows x cols
+    float* pyr = nullptr;         // sliding-window maxima of tile culling (project_cull.cuh), built for pyr_shortcut
+    uint32_t* timg = nullptr;     // test image of the scan-minus-map fast path (scan_test_image_kernel), built for timg_shortcut
+    int pyr_shortcut = -1, timg_shortcut = -1;
+    uint64_t last_use = 0;
 };
 
 struct PtrView { const float *x, *y, *z, *i; int64_t n; };
@@ -67,6 +89,10 @@ struct ltr_ctx {
     std::vector<ltr::DevPoses> poses;
     std::vector<ltr::NcclComm> nccl;           // communicators created by ltr_nccl_init / ltr_nccl_split
     int64_t launches = 0;
+    uint64_t next_serial = 0;                  // DevScanSet / DevPoses serials
+    ltr::ScanImageSet scan_images[ltr::kMaxScanImageSets];   // the least recently used one is refilled first
+    uint64_t scan_images_tick = 0;
+    int scan_images_busy = 0;                  // a pass is reading a set: the allocator must not free their storage
     bool rs_attr_set = false;    // radix-sort scatter kernel opted in to > 48 KB shared memory on this device
     int64_t vox_shortcuts = 0;   // voxelisations answered by the already-one-point-per-voxel shortcut (util.cu)
     bool ext_identity = true;     // base2lidar/lidar2base exactly identity -> second transform step is exact and skipped
@@ -181,6 +207,11 @@ int nccl_allreduce_u32(ltr_ctx* ctx, int comm, uint32_t* dev, size_t count, int 
 // `send` holds this rank's points grouped by destination rank (segment d has scount[d] points, segments back to back); *recv_out
 // receives, in source-rank order, what every rank sent to this one
 int nccl_alltoallv_cloud(ltr_ctx* ctx, int comm, const DevCloud& send, const std::vector<int64_t>& scount, ltr_cloud* recv_out);
+
+// drops the held scan-image sets (all, or those built from the scan set / poses with that serial); free_storage also returns the slots'
+// storage blocks to the allocator (project.cu)
+void scan_images_release(ltr_ctx* ctx, uint64_t serial, bool free_storage);
+bool scan_images_have_storage(const ltr_ctx* ctx);
 
 int segment_counts(ltr_ctx* ctx, const uint8_t* flags, const DevScanSet& s, std::vector<int64_t>* counts);
 int split_scanset_by_flag(ltr_ctx* ctx, const DevScanSet& in, const uint8_t* flags, ltr_scanset* out_unflagged, ltr_scanset* out_flagged);

@@ -16,6 +16,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <tuple>
 
 namespace ltr {
 
@@ -397,6 +398,159 @@ static int deferred_alloc(ltr_ctx* ctx, int B, int64_t npx, void** block, Deferr
     return LTR_OK;
 }
 
+// Scan-side images of a remove pass for the keyframes [k0, k0 + nb) of `scans`, keyframe-major:
+//   rimg  the scan range image (scan2RangeImg), built here when make_rimg, else read;
+//   pyr   (if non-null) its sliding-window maxima for tile culling; an empty scan pixel is -inf with the shortcut, else +inf;
+//   timg  (if non-null) the test image of the scan-minus-map fast path, guard-padded when `pad`, empty pixels -inf with the shortcut.
+// None of them reads the map.  Launches cover at most kImageChunk keyframes (the window-maximum grid's z extent).
+constexpr int kImageChunk = 1024;
+static int build_scan_images(ltr_ctx* ctx, const DevScanSet& scans, int k0, int nb, const ImgShape& g, const FastCfg& fc, bool use_fast, int shortcut,
+                             bool make_rimg, uint32_t* rimg, float* pyr, uint32_t* timg, bool pad) {
+    const int64_t npx = (int64_t)g.rows * g.cols;
+    const int64_t timg_px = pad ? (int64_t)fc.pad_npx : npx;
+    const unsigned pyr_stride = (unsigned)(kPyrLevels * npx);
+    const int fill_blocks = ctx->sm_count * 8;
+    for (int c0 = 0; c0 < nb; c0 += kImageChunk) {
+        const int n = std::min(kImageChunk, nb - c0);
+        uint32_t* ri = rimg + (size_t)c0 * npx;
+        if (make_rimg) {
+            fill_u32_kernel<<<grid_for(n * npx, 256, fill_blocks), 256, 0, ctx->stream>>>(ri, kNoPointBits, n * npx);
+            LTR_LAUNCH_CHECK(ctx);
+            const int kf0 = k0 + c0;
+            const int64_t npts = scans.h_off[kf0 + n] - scans.h_off[kf0];
+            if (npts > 0) {
+                if (use_fast && fc.el_direct) scan_rimg_fast_kernel<true><<<(unsigned)((npts + 255) / 256), 256, 0, ctx->stream>>>(view(scans.pts), scans.d_off, kf0, n, g, fc, ri);
+                else if (use_fast) scan_rimg_fast_kernel<false><<<(unsigned)((npts + 255) / 256), 256, 0, ctx->stream>>>(view(scans.pts), scans.d_off, kf0, n, g, fc, ri);
+                else scan_rimg_kernel<<<(unsigned)((npts + 255) / 256), 256, 0, ctx->stream>>>(view(scans.pts), scans.d_off, kf0, n, g, ri);
+                LTR_LAUNCH_CHECK(ctx);
+            }
+        }
+        if (pyr) {
+            const float empty_value = shortcut ? -__builtin_huge_valf() : __builtin_huge_valf();   // empty scan pixel: never flags / unknown
+            const dim3 wg((unsigned)((g.cols + kWinTile - 1) / kWinTile), (unsigned)((g.rows + kWinTile - 1) / kWinTile), (unsigned)n);
+            scan_window_max_kernel<<<wg, 256, 0, ctx->stream>>>(ri, g.rows, g.cols, empty_value, pyr_stride, pyr + (size_t)c0 * pyr_stride);
+            LTR_LAUNCH_CHECK(ctx);
+        }
+        if (timg) {
+            scan_test_image_kernel<<<grid_for(n * timg_px, 256, fill_blocks), 256, 0, ctx->stream>>>(ri, timg + (size_t)c0 * timg_px, n, g.rows, g.cols,
+                                                                                                    pad ? fc.pad_g : 0, pad ? 1 : 0, shortcut);
+            LTR_LAUNCH_CHECK(ctx);
+        }
+    }
+    return LTR_OK;
+}
+
+// Kept scan-image sets (ScanImageSet): the second remove pass at a resolution and the three ND and three PD filter passes find their images.
+
+static void scan_image_set_drop(ScanImageSet& s) {
+    s.valid = false;
+    s.rimg = nullptr; s.pyr = nullptr; s.timg = nullptr;
+    s.pyr_shortcut = s.timg_shortcut = -1;
+}
+
+void scan_images_release(ltr_ctx* ctx, uint64_t serial, bool free_storage) {
+    for (ScanImageSet& s : ctx->scan_images) {
+        if (serial == 0 || s.scans_serial == serial || s.poses_serial == serial) scan_image_set_drop(s);
+        if (free_storage && serial == 0) { dev_free(ctx, s.block); s.block = nullptr; s.cap = 0; }
+    }
+}
+
+bool scan_images_have_storage(const ltr_ctx* ctx) {
+    for (const ScanImageSet& s : ctx->scan_images) if (s.block) return true;
+    return false;
+}
+
+// Bytes the slots' storage may take in all.  LTR_SCAN_IMAGE_CACHE_MB=n sets n MiB; 0 turns the sets off, and every pass builds its images
+// per launch.  Default: a quarter of the device memory this context could still use (free, its allocator cache, the slots themselves).
+static bool scan_image_cache_on(size_t* fixed_budget) {
+    *fixed_budget = 0;
+    const char* e = std::getenv("LTR_SCAN_IMAGE_CACHE_MB");
+    if (!e || !*e) return true;
+    *fixed_budget = (size_t)std::max(std::atoll(e), 0ll) << 20;
+    return *fixed_budget > 0;
+}
+
+// Pins the slots' storage for the rest of a pass: an allocation that runs out of memory must not free images the pass is reading.
+struct ScanImagesPin {
+    ltr_ctx* ctx;
+    explicit ScanImagesPin(ltr_ctx* c) : ctx(c) { ctx->scan_images_busy++; }
+    ~ScanImagesPin() { ctx->scan_images_busy--; }
+    ScanImagesPin(const ScanImagesPin&) = delete;
+    ScanImagesPin& operator=(const ScanImagesPin&) = delete;
+};
+
+// The kept set with the scan images of a pass over [kf_begin, kf_end) -- found, completed or built, in launches over the whole range.
+// A new set goes into an empty slot or the least recently used one, preferring a slot whose storage is already large enough; storage only
+// grows.  *out = nullptr when the sets are off or the storage would exceed the budget: the pass then builds its images per launch.  The
+// caller holds a ScanImagesPin.
+static int scan_images_get(ltr_ctx* ctx, const DevScanSet& scans, const DevPoses& poses, int kf_begin, int kf_end, const ImgShape& g, const FastCfg& fc,
+                           bool use_fast, int shortcut, bool need_pyr, bool need_timg, bool pad, ScanImageSet** out) {
+    *out = nullptr;
+    size_t budget = 0;
+    if (!scan_image_cache_on(&budget)) return LTR_OK;
+    const int K = kf_end - kf_begin;
+    const size_t npx = (size_t)g.rows * g.cols;
+    const size_t rimg_bytes = (size_t)K * npx * sizeof(uint32_t), pyr_bytes = rimg_bytes * kPyrLevels;
+    const size_t timg_bytes = (size_t)K * (pad ? (size_t)fc.pad_npx : npx) * sizeof(uint32_t);
+    // storage layout rimg | timg | pyr (256 B aligned): a set that needs the window table needs the whole block
+    const size_t timg_off = (rimg_bytes + 255) / 256 * 256, pyr_off = timg_off + (timg_bytes + 255) / 256 * 256;
+    const size_t need = need_pyr ? pyr_off + pyr_bytes : need_timg ? timg_off + timg_bytes : rimg_bytes;
+    const int ext = ctx->ext_identity ? 1 : 0;
+    ScanImageSet* s = nullptr;
+    for (ScanImageSet& c : ctx->scan_images)
+        if (c.valid && c.scans_serial == scans.serial && c.poses_serial == poses.serial && c.kf_begin == kf_begin && c.kf_end == kf_end && c.rows == g.rows &&
+            c.cols == g.cols && c.vfov == g.vfov && c.hfov == g.hfov && c.order == ctx->cfg.transform_order && c.ext_identity == ext &&
+            c.fast_path == ctx->cfg.fast_path)
+            s = &c;
+    if (s && s->cap < need) scan_image_set_drop(*s);   // a part it lacks does not fit its storage: rebuild the set in a larger block
+    if (!s || !s->valid) {
+        if (!s) {   // empty before occupied, large enough before too small, then least recently used
+            auto rank = [&](const ScanImageSet& c) { return std::make_tuple(c.valid ? 1 : 0, c.cap >= need ? 0 : 1, c.last_use); };
+            s = &ctx->scan_images[0];
+            for (ScanImageSet& c : ctx->scan_images) if (rank(c) < rank(*s)) s = &c;
+        }
+        scan_image_set_drop(*s);
+        if (s->cap < need) {
+            size_t others = 0;
+            for (const ScanImageSet& c : ctx->scan_images) if (&c != s) others += c.cap;
+            if (budget == 0) {
+                size_t fr = 0, tot = 0;
+                if (cudaMemGetInfo(&fr, &tot) != cudaSuccess) { cudaGetLastError(); return LTR_OK; }
+                budget = (fr + ctx->cached_bytes + others + s->cap) / 4;
+            }
+            if (others + need > budget) return LTR_OK;
+            dev_free(ctx, s->block);
+            s->block = nullptr; s->cap = 0;
+            const int rc = dev_alloc(ctx, &s->block, need);
+            if (rc != LTR_OK) {   // out of memory within the budget (memory other processes took): build per launch
+                if (rc != LTR_ERR_NOMEM) return rc;
+                ctx->err.clear();
+                return LTR_OK;
+            }
+            s->cap = need;
+        }
+        s->scans_serial = scans.serial; s->poses_serial = poses.serial; s->kf_begin = kf_begin; s->kf_end = kf_end; s->rows = g.rows; s->cols = g.cols;
+        s->vfov = g.vfov; s->hfov = g.hfov; s->order = ctx->cfg.transform_order; s->ext_identity = ext; s->fast_path = ctx->cfg.fast_path;
+    }
+    char* base = (char*)s->block;
+    const bool make_rimg = !s->valid;
+    const bool make_pyr = need_pyr && s->pyr_shortcut != shortcut;
+    const bool make_timg = need_timg && s->timg_shortcut != shortcut;
+    s->rimg = (uint32_t*)base;
+    s->timg = s->cap >= timg_off + timg_bytes ? (uint32_t*)(base + timg_off) : nullptr;
+    s->pyr = s->cap >= pyr_off + pyr_bytes ? (float*)(base + pyr_off) : nullptr;
+    if (make_rimg || make_pyr || make_timg) {
+        s->valid = false;   // until the build is enqueued
+        LTR_TRY(build_scan_images(ctx, scans, kf_begin, K, g, fc, use_fast, shortcut, make_rimg, s->rimg, make_pyr ? s->pyr : nullptr,
+                                  make_timg ? s->timg : nullptr, pad));
+        s->valid = true;
+        if (make_pyr) s->pyr_shortcut = shortcut;
+        if (make_timg) s->timg_shortcut = shortcut;
+    }
+    s->last_use = ++ctx->scan_images_tick;
+    *out = s;
+    return LTR_OK;
+}
 
 }  // namespace ltr
 
@@ -406,6 +560,13 @@ extern "C" {
 
 static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end,
                             int32_t mode, float res_alpha, float diff_thres, int32_t accumulate, int64_t* n_dynamic, bool allow_deferred, bool* overflowed);
+
+int ltr_scan_images_release(ltr_ctx* ctx, int32_t free_storage) {
+    ApiTrace tr__(ctx, "ltr_scan_images_release");
+    if (!ctx) return LTR_ERR_INVALID;
+    scan_images_release(ctx, 0, free_storage != 0);
+    return LTR_OK;
+}
 
 int ltr_remove_pass(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end,
                     int32_t mode, float res_alpha, float diff_thres, int32_t accumulate, int64_t* n_dynamic) {
@@ -460,62 +621,59 @@ static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, 
     const bool use_cull = use_fast && cand && ctx->cfg.fast_path >= 2 && B <= 32 && map->n >= kTilePts && map->n >= npx;
     void *p_tiles = nullptr, *p_pyr = nullptr;
     ScratchGuard g_tiles(ctx, &p_tiles), g_pyr(ctx, &p_pyr);
+    const bool run = map->n > 0 && kf_end > kf_begin;
+    // scan-minus-map with the short elevation path and a 360 degree field of view: the test image is guard-padded (FastCfg::pad_*) and always built
+    const bool pad = use_fast && cand && fc.pad_ok;
+    const bool need_timg = use_fast && cand && (shortcut || pad);
+    const int64_t timg_px = pad ? (int64_t)fc.pad_npx : npx;
+    // the scan-side images come from a kept set built over the whole range (scan_images_get) or, without one, are built per launch
+    ScanImagesPin pin(ctx);
+    ScanImageSet* set = nullptr;
+    if (run) LTR_TRY(scan_images_get(ctx, *scans, *poses, kf_begin, kf_end, g, fc, use_fast, shortcut, use_cull, need_timg, pad, &set));
     if (use_cull) {
         ca.enabled = 1;
         ca.ntiles = (map->n + kTilePts - 1) / kTilePts;
         ca.pyr_stride = (unsigned)(kPyrLevels * npx);
         LTR_TRY(dev_alloc(ctx, &p_tiles, (size_t)ca.ntiles * sizeof(float4)));
-        LTR_TRY(dev_alloc(ctx, &p_pyr, (size_t)B * ca.pyr_stride * sizeof(float)));
-        ca.tiles = (const float4*)p_tiles; ca.pyr = (const float*)p_pyr;
+        if (!set) LTR_TRY(dev_alloc(ctx, &p_pyr, (size_t)B * ca.pyr_stride * sizeof(float)));
+        ca.tiles = (const float4*)p_tiles;
         tile_sphere_kernel<<<(unsigned)((ca.ntiles * 32 + 255) / 256), 256, 0, ctx->stream>>>(view(*map), (float4*)p_tiles, ca.ntiles);
         LTR_LAUNCH_CHECK(ctx);
     }
     LTR_CUDA(ctx, cudaEventRecord(ctx->ev0, ctx->stream));
     std::vector<int> launch_units;
     ctx->ev_used = 0;
-    if (map->n > 0 && kf_end > kf_begin) {
+    if (run) {
         void *p_rimg = nullptr, *p_win = nullptr;
         ScratchGuard g_rimg(ctx, &p_rimg), g_win(ctx, &p_win);
-        // scan-minus-map with the short elevation path and a 360 degree field of view: the test image is guard-padded (FastCfg::pad_*) and always built
-        const bool pad = use_fast && cand && fc.pad_ok;
-        const int64_t timg_px = pad ? (int64_t)fc.pad_npx : npx;
-        LTR_TRY(dev_alloc(ctx, &p_rimg, (size_t)B * (use_fast ? 2 * npx + timg_px : npx) * sizeof(uint32_t)));
+        // per launch: the approximate running minimum (fast path), and without a kept set the scan image and the test image
+        const int64_t per_kf = (use_fast ? npx : 0) + (set ? 0 : npx + (need_timg ? timg_px : 0));
+        if (per_kf > 0) LTR_TRY(dev_alloc(ctx, &p_rimg, (size_t)B * per_kf * sizeof(uint32_t)));
         LTR_TRY(dev_alloc(ctx, &p_win, (size_t)B * npx * sizeof(uint64_t)));
-        uint32_t* rimg = (uint32_t*)p_rimg;
-        uint32_t* amin = rimg + (size_t)B * npx;   // approximate running minimum (fast path only)
-        uint32_t* timg = amin + (size_t)B * npx;   // test image of the scan-minus-map variants (padded, or pixels without a return can never flag)
+        uint32_t* amin = use_fast ? (uint32_t*)p_rimg : nullptr;   // approximate running minimum (fast path only)
+        uint32_t* l_rimg = set ? nullptr : (uint32_t*)p_rimg + (use_fast ? (size_t)B * npx : 0);
+        uint32_t* l_timg = (set || !need_timg) ? nullptr : l_rimg + (size_t)B * npx;   // test image (padded, or pixels without a return can never flag)
         uint64_t* win = (uint64_t*)p_win;
         const int fill_blocks = ctx->sm_count * 8;
         fill_u64_kernel<<<grid_for(B * npx, 256, fill_blocks), 256, 0, ctx->stream>>>(win, cand ? kWinNone : kWinEmpty, B * npx);
         LTR_LAUNCH_CHECK(ctx);
         for (int k0 = kf_begin; k0 < kf_end; k0 += B) {
             const int nb = std::min(B, kf_end - k0);
-            fill_u32_kernel<<<grid_for(nb * npx, 256, fill_blocks), 256, 0, ctx->stream>>>(rimg, kNoPointBits, nb * npx);
-            LTR_LAUNCH_CHECK(ctx);
             if (use_fast) {
                 fill_u32_kernel<<<grid_for(nb * npx, 256, fill_blocks), 256, 0, ctx->stream>>>(amin, 0x7f800000u, nb * npx);
                 LTR_LAUNCH_CHECK(ctx);
             }
-
-            const int64_t npts = scans->h_off[k0 + nb] - scans->h_off[k0];
-            if (npts > 0) {
-                if (use_fast && fc.el_direct) scan_rimg_fast_kernel<true><<<(unsigned)((npts + 255) / 256), 256, 0, ctx->stream>>>(view(scans->pts), scans->d_off, k0, nb, g, fc, rimg);
-                else if (use_fast) scan_rimg_fast_kernel<false><<<(unsigned)((npts + 255) / 256), 256, 0, ctx->stream>>>(view(scans->pts), scans->d_off, k0, nb, g, fc, rimg);
-                else scan_rimg_kernel<<<(unsigned)((npts + 255) / 256), 256, 0, ctx->stream>>>(view(scans->pts), scans->d_off, k0, nb, g, rimg);
-                LTR_LAUNCH_CHECK(ctx);
-            }
-            if (use_cull) {
-                const float empty_value = shortcut ? -__builtin_huge_valf() : __builtin_huge_valf();   // empty scan pixel: never flags / unknown
-                const dim3 wg((unsigned)((cols + kWinTile - 1) / kWinTile), (unsigned)((rows + kWinTile - 1) / kWinTile), (unsigned)nb);
-                scan_window_max_kernel<<<wg, 256, 0, ctx->stream>>>(rimg, rows, cols, empty_value, ca.pyr_stride, (float*)p_pyr);
-                LTR_LAUNCH_CHECK(ctx);
-            }
-            const uint32_t* test_img = rimg;
-            if (use_fast && cand && (shortcut || pad)) {
-                scan_test_image_kernel<<<grid_for(nb * timg_px, 256, fill_blocks), 256, 0, ctx->stream>>>(rimg, timg, nb, rows, cols, pad ? fc.pad_g : 0,
-                                                                                                         pad ? 1 : 0, shortcut);
-                LTR_LAUNCH_CHECK(ctx);
-                test_img = timg;
+            const uint32_t *rimg, *test_img;
+            if (set) {
+                const size_t j = (size_t)(k0 - kf_begin);
+                rimg = set->rimg + j * npx;
+                test_img = need_timg ? set->timg + j * timg_px : rimg;
+                if (use_cull) ca.pyr = set->pyr + j * ca.pyr_stride;
+            } else {
+                LTR_TRY(build_scan_images(ctx, *scans, k0, nb, g, fc, use_fast, shortcut, true, l_rimg, use_cull ? (float*)p_pyr : nullptr, l_timg, pad));
+                rimg = l_rimg;
+                test_img = need_timg ? l_timg : l_rimg;
+                if (use_cull) ca.pyr = (const float*)p_pyr;
             }
             prof_begin(ctx);
             launch_units.push_back(nb);
