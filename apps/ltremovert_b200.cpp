@@ -41,27 +41,23 @@ struct LoadedSession {
     std::vector<double> poses, inv_poses;
 };
 
-// the keyframes [k0, k1) of the session's keyframe list (a rank's block; everything in a single-process run)
-static bool load_keyframes(LoadedSession& s, float voxel, size_t k0, size_t k1, std::string* err) {  // Session::loadKeyframes (Session.cpp:266-302)
+// the keyframes [k0, k1) of the session's keyframe list (a rank's block; everything in a single-process run), as read from disk:
+// Session::loadKeyframes (Session.cpp:266-302) minus its VoxelGrid, which runs on the device (Removerter::load_session_raw)
+static bool load_keyframes(LoadedSession& s, size_t k0, size_t k1, std::string* err) {
     s.offsets.assign(1, 0);
-    int overflow_warnings = 0;
     for (size_t kk = k0; kk < k1; ++kk) {
         const int idx = s.files.keyframe_idx[kk];
         HostCloud pts;
         if (!read_pcd(s.files.scan_paths[(size_t)idx], &pts, err)) return false;
-        bool ov = false;
-        const HostCloud down = voxel_grid(pts, voxel, &ov);
-        overflow_warnings += ov ? 1 : 0;
-        for (const auto& p : down) { s.xyzi.push_back(p.x); s.xyzi.push_back(p.y); s.xyzi.push_back(p.z); s.xyzi.push_back(p.intensity); }
-        s.offsets.push_back(s.offsets.back() + (int64_t)down.size());
+        const float* f = reinterpret_cast<const float*>(pts.data());
+        s.xyzi.insert(s.xyzi.end(), f, f + 4 * pts.size());
+        s.offsets.push_back(s.offsets.back() + (int64_t)pts.size());
         s.keyframe_names.push_back(s.files.scan_names[(size_t)idx]);
         const Mat4& P = s.files.scan_poses[(size_t)idx];
         const Mat4& IP = s.files.scan_inverse_poses[(size_t)idx];
         s.poses.insert(s.poses.end(), P.begin(), P.end());
         s.inv_poses.insert(s.inv_poses.end(), IP.begin(), IP.end());
     }
-    if (overflow_warnings)
-        std::fprintf(stderr, "[pcl::VoxelGrid::applyFilter] Leaf size is too small for the input dataset (%d scans returned unchanged)\n", overflow_warnings);
     return true;
 }
 
@@ -189,7 +185,7 @@ int main(int argc, char** argv) {
     size_t c0, c1, q0, q1;
     block(C.files.keyframe_idx.size(), owns_c, &c0, &c1);
     block(Q.files.keyframe_idx.size(), owns_q, &q0, &q1);
-    if (!load_keyframes(C, P.downsample_voxel_size, c0, c1, &err) || !load_keyframes(Q, P.downsample_voxel_size, q0, q1, &err)) { std::fprintf(stderr, "%s\n", err.c_str()); return 1; }
+    if (!load_keyframes(C, c0, c1, &err) || !load_keyframes(Q, q0, q1, &err)) { std::fprintf(stderr, "%s\n", err.c_str()); return 1; }
 
     Removerter R(P);
     if (R.init() != LTR_OK) { std::fprintf(stderr, "GPU context: %s\n", R.err.c_str()); return 1; }
@@ -199,8 +195,16 @@ int main(int argc, char** argv) {
         if (!share_nccl_id(rank, id)) { std::fprintf(stderr, "[rank %d] could not exchange the NCCL id\n", rank); return 1; }
         ck(R.comm_init_nccl(id, rank, world, split ? 1 : 0), "NCCL init");
     }
-    ck(R.load_session(0, C.xyzi.data(), C.offsets.data(), C.poses.data(), C.inv_poses.data(), (int)C.keyframe_names.size()), "load central");
-    ck(R.load_session(1, Q.xyzi.data(), Q.offsets.data(), Q.poses.data(), Q.inv_poses.data(), (int)Q.keyframe_names.size()), "load query");
+    // upload the raw scans; loadKeyframes' VoxelGrid(downsample_voxel_size) runs on the device
+    for (int sess = 0; sess < 2; ++sess) {
+        LoadedSession& S = sess == 0 ? C : Q;
+        int32_t overflow_warnings = 0;
+        ck(R.load_session_raw(sess, S.xyzi.data(), S.offsets.data(), S.poses.data(), S.inv_poses.data(), (int)S.keyframe_names.size(), &overflow_warnings),
+           sess == 0 ? "load central" : "load query");
+        if (overflow_warnings)
+            std::fprintf(stderr, "[pcl::VoxelGrid::applyFilter] Leaf size is too small for the input dataset (%d scans returned unchanged)\n", overflow_warnings);
+        std::vector<float>().swap(S.xyzi);   // the raw scans now live on the device
+    }
     ck(R.run_step0(), "Step 0");
     ck(R.run_step12(), "Step 1-2");
     ck(R.run_step3(), "Step 3");

@@ -127,6 +127,16 @@ int ltr_voxel_centroid(ltr_ctx* ctx, ltr_cloud in, float leaf, ltr_cloud* out);
 /* Same, applied independently to every keyframe cloud (Session::updateScansScanwise, Session.cpp:374-375). */
 int ltr_voxel_centroid_per_keyframe(ltr_ctx* ctx, ltr_scanset in, float leaf, ltr_scanset* out);
 
+/* pcl::VoxelGrid as Session::loadKeyframes applies it to every scan it reads (Session.cpp:284-289), byte-identical to the host restatement
+ * voxel_grid_span (lt_mapper_b200/csrc/host/io.cpp): one centroid per occupied voxel in ascending voxel-index order, each summed in the
+ * order libstdc++'s std::sort leaves the (index, point) entries.  When the product of the three voxel extents exceeds INT32_MAX the
+ * filter takes PCL's overflow exit ("Leaf size is too small for the input dataset") and the scan is returned unchanged; *overflowed
+ * (optional) is then 1.  An empty input gives an empty output.  leaf <= 0 or non-finite: LTR_ERR_INVALID. */
+int ltr_voxel_grid(ltr_ctx* ctx, ltr_cloud in, float leaf, ltr_cloud* out, int32_t* overflowed);
+/* Same, applied to every keyframe of `in` independently (the loadKeyframes loop, Session.cpp:272-303); n_overflowed (optional) receives
+ * the number of scans that took the overflow exit. */
+int ltr_voxel_grid_per_keyframe(ltr_ctx* ctx, ltr_scanset in, float leaf, ltr_scanset* out, int32_t* n_overflowed);
+
 /* One remove / revert / ND / PD pass == calcDescrepancyAndParseDynamicPointIdxForEachScan{,ForND,ForPD}
  * (Removerter.cpp:542-593, 485-540, 429-482) over the source keyframes [kf_begin, kf_end) of `scans`:
  * scan range image, two-step map transform, map range image + index image, signed diff, threshold,

@@ -82,6 +82,10 @@ void ltrh_invert_poses(const double* poses16, int32_t K, double* out16);
 /* sess: 0 = central, 1 = query.  Keyframes are this rank's block (all keyframes when world == 1). */
 int ltrh_load_session(ltrh_removerter* r, int32_t sess, const float* xyzi, const int64_t* offsets, const double* poses,
                       const double* inv_poses, int32_t K);
+/* The same from the scans as read from disk: Session::loadKeyframes' pcl::VoxelGrid(downsample_voxel_size) (Session.cpp:284-289) runs on
+ * the device (ltr_voxel_grid_per_keyframe), then the session is left exactly as ltrh_load_session leaves it with the filtered scans. */
+int ltrh_load_session_raw(ltrh_removerter* r, int32_t sess, const float* xyzi, const int64_t* offsets, const double* poses,
+                          const double* inv_poses, int32_t K);
 
 /* Removerter::run() split at its step comments (Removerter.cpp:1655-1676) */
 int ltrh_run_step0(ltrh_removerter* r);   /* precleaningKeyframes(2.5) + makeGlobalMap            (:1660-1662) */
@@ -93,7 +97,7 @@ int ltrh_reset_to_step0(ltrh_removerter* r);
 /* LT-map cascade (multi-session chaining).  The reference has no call for this: it is done by pointing the next run's
  * central_sess_scan_dir at the previous run's scans_updated/ (written by saveUpdatedScans, Removerter.cpp:1620-1623) with the same
  * central pose file; Session::loadKeyframes (Session.cpp:272-303) then voxel-grids each scan at downsample_voxel_size.  This
- * entry does exactly that in memory after ltrh_run_step3: central keyframe_scans_ <- VoxelGrid(keyframe_scans_updated_), central poses
+ * entry does exactly that in device memory (the scans never leave the GPU) after ltrh_run_step3: central keyframe_scans_ <- VoxelGrid(keyframe_scans_updated_), central poses
  * kept, query session and every derived cloud released, log cleared.  Then ltrh_load_session(r, 1, next query) and run the steps again. */
 int ltrh_cascade_promote_updated(ltrh_removerter* r);
 /* a single member function of Removerter by name, e.g. "removeHighDynamicPoints" */

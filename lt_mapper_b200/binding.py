@@ -34,7 +34,7 @@ EXPORTS = [
     "ltr_cloud_upload", "ltr_cloud_size", "ltr_cloud_download", "ltr_cloud_free", "ltr_cloud_copy", "ltr_cloud_concat", "ltr_cloud_slice",
     "ltr_cloud_device_ptrs", "ltr_cloud_alloc", "ltr_scanset_upload", "ltr_scanset_info", "ltr_scanset_download",
     "ltr_scanset_free", "ltr_scanset_concat_per_keyframe", "ltr_scanset_flatten", "ltr_poses_upload", "ltr_poses_free",
-    "ltr_preclean", "ltr_merge_scans_global", "ltr_voxel_centroid", "ltr_voxel_centroid_per_keyframe", "ltr_remove_pass", "ltr_scan_images_release",
+    "ltr_preclean", "ltr_merge_scans_global", "ltr_voxel_centroid", "ltr_voxel_centroid_per_keyframe", "ltr_voxel_grid", "ltr_voxel_grid_per_keyframe", "ltr_remove_pass", "ltr_scan_images_release",
     "ltr_flags_device_ptr", "ltr_flags_download", "ltr_flags_upload", "ltr_apply_partition", "ltr_parse_projected",
     "ltr_knn_diff", "ltr_knn_split_cloud", "ltr_debug_pixel_index", "ltr_debug_scan_rimg", "ltr_debug_fast_project", "ltr_debug_atan_sweep", "ltr_debug_margins", "ltr_reset_rimg_size", "ltr_last_pass_stats", "ltr_profile_get", "ltr_profile_reset", "ltr_timer_start", "ltr_timer_stop", "ltr_trace_dump",
     "ltr_pinned_alloc", "ltr_pinned_free", "ltr_nccl_unique_id", "ltr_nccl_init", "ltr_nccl_split", "ltr_nccl_info", "ltr_nccl_destroy", "ltr_nccl_version", "ltr_nccl_allreduce_flags",
@@ -87,6 +87,8 @@ def lib():
     L.ltr_merge_scans_global.argtypes = [vp, i32, i32, P(i32)]
     L.ltr_voxel_centroid.argtypes = [vp, i32, f32, P(i32)]
     L.ltr_voxel_centroid_per_keyframe.argtypes = [vp, i32, f32, P(i32)]
+    L.ltr_voxel_grid.argtypes = [vp, i32, f32, P(i32), P(i32)]
+    L.ltr_voxel_grid_per_keyframe.argtypes = [vp, i32, f32, P(i32), P(i32)]
     L.ltr_remove_pass.argtypes = [vp, i32, i32, i32, i32, i32, i32, f32, f32, i32, P(i64)]
     L.ltr_scan_images_release.argtypes = [vp, i32]
     L.ltr_flags_device_ptr.argtypes = [vp, i32, P(vp), P(i64)]
@@ -287,6 +289,20 @@ class Context:
         h = ctypes.c_int32()
         self._ck(lib().ltr_voxel_centroid_per_keyframe(self._h, scans, leaf, ctypes.byref(h)))
         return h.value
+
+    def voxel_grid(self, cloud, leaf):
+        """Load-time pcl::VoxelGrid of one cloud (ltr_voxel_grid).  Returns (handle, overflowed): overflowed is True when the
+        filter took PCL's overflow exit and the output is the input unchanged."""
+        h, ov = ctypes.c_int32(), ctypes.c_int32()
+        self._ck(lib().ltr_voxel_grid(self._h, cloud, leaf, ctypes.byref(h), ctypes.byref(ov)))
+        return h.value, bool(ov.value)
+
+    def voxel_grid_per_keyframe(self, scans, leaf):
+        """Load-time pcl::VoxelGrid of every keyframe (ltr_voxel_grid_per_keyframe).  Returns (handle, number of scans returned
+        unchanged by the overflow exit)."""
+        h, ov = ctypes.c_int32(), ctypes.c_int32()
+        self._ck(lib().ltr_voxel_grid_per_keyframe(self._h, scans, leaf, ctypes.byref(h), ctypes.byref(ov)))
+        return h.value, ov.value
 
     def remove_pass(self, map_, scans, poses, mode, res_alpha, diff_thres=0.1, kf_begin=0, kf_end=None, accumulate=False):
         if kf_end is None:

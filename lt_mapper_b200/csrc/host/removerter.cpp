@@ -52,8 +52,6 @@ Removerter::Removerter(const ltrh_params& p) : P(p) {
 }
 
 Removerter::~Removerter() {
-    ltr_pinned_free(pin_in_);
-    ltr_pinned_free(pin_out_);
     if (ctx) ltr_destroy(ctx);
 }
 
@@ -208,6 +206,22 @@ int Removerter::load_session(int sess, const float* xyzi, const int64_t* offsets
     Session& S = sess == 0 ? central_sess_ : query_sess_;
     ltr_scanset ss; ltr_poses ps;
     CK(ltr_scanset_upload(ctx, xyzi, offsets, K, &ss));
+    CK(ltr_poses_upload(ctx, poses, inv_poses, K, &ps));
+    CK(set(&S.keyframe_scans_, ss, true));
+    if (S.keyframe_poses_ >= 0) CK(ltr_poses_free(ctx, S.keyframe_poses_));
+    S.keyframe_poses_ = ps;
+    S.num_keyframes_ = K;
+    return LTR_OK;
+}
+
+int Removerter::load_session_raw(int sess, const float* xyzi, const int64_t* offsets, const double* poses, const double* inv_poses, int K,
+                                 int32_t* n_overflowed) {
+    Session& S = sess == 0 ? central_sess_ : query_sess_;
+    ltr_scanset raw, ss; ltr_poses ps;
+    CK(ltr_scanset_upload(ctx, xyzi, offsets, K, &raw));
+    const int rc = ltr_voxel_grid_per_keyframe(ctx, raw, P.downsample_voxel_size, &ss, n_overflowed);   // Session.cpp:284-289
+    ltr_scanset_free(ctx, raw);
+    CK(rc);
     CK(ltr_poses_upload(ctx, poses, inv_poses, K, &ps));
     CK(set(&S.keyframe_scans_, ss, true));
     if (S.keyframe_poses_ >= 0) CK(ltr_poses_free(ctx, S.keyframe_poses_));
@@ -668,40 +682,16 @@ int Removerter::reset_to_step0() {
 
 // LT-map cascade (SURVEY.md §8f).  The reference chains sessions through its file protocol: a run's scans_updated/ directory and the
 // central pose file are handed to the next run as its central session, where Session::loadKeyframes (Session.cpp:272-303) reads
-// each scan back and passes it through pcl::VoxelGrid(downsample_voxel_size).  This does the same in memory: the updated scans
-// (Removerter.cpp:1606-1650, what saveUpdatedScans writes) are brought to the host, voxel-gridded with the same load-time
-// restatement the file driver uses (io.cpp), and become keyframe_scans_ of the central session; its poses stay.  Everything
-// derived from the finished pair, and the query session, is released; the caller loads the next query and runs Steps 0-3 again.
+// each scan back and passes it through pcl::VoxelGrid(downsample_voxel_size).  This does the same in memory and on the device: the
+// updated scans (Removerter.cpp:1606-1650, what saveUpdatedScans writes) go through the load-time filter (ltr_voxel_grid_per_keyframe,
+// byte-identical to the restatement the file driver used to apply on the host) and become keyframe_scans_ of the central session;
+// its poses stay.  Everything derived from the finished pair, and the query session, is released; the caller loads the next query and
+// runs Steps 0-3 again.  Ranks that do not own the central session hold none of its scans and only release.
 int Removerter::cascade_promote_updated() {
     Session& C = central_sess_;
     if (owns(C) && C.keyframe_scans_updated_ < 0) return fail(LTR_ERR_INVALID, "cascade: Step 3 has not run (no keyframe_scans_updated_)");
-    int32_t K = 0; int64_t total = 0;
-    if (owns(C)) CK(ltr_scanset_info(ctx, C.keyframe_scans_updated_, &K, &total));
-    // page-locked staging in both directions (a pageable 1 GB round trip costs more than Steps 0-3 of a session)
-    // (kept across promotions: page-locking a gigabyte is itself slow)
-    auto grow = [&](void** p, size_t* cap, size_t bytes) {
-        if (*cap >= bytes) return true;
-        ltr_pinned_free(*p); *p = nullptr; *cap = 0;
-        if (ltr_pinned_alloc(2 * bytes, p) != LTR_OK) return false;   // the live scans grow from session to session: leave room
-        *cap = 2 * bytes;
-        return true;
-    };
-    if (!grow(&pin_in_, &pin_in_cap_, (size_t)std::max<int64_t>(total, 1) * 16)) return fail(LTR_ERR_NOMEM, "cascade: pinned staging allocation failed");
-    float* xyzi = (float*)pin_in_;
-    std::vector<int64_t> off((size_t)K + 1, 0);
-    if (owns(C)) CK(ltr_scanset_download(ctx, C.keyframe_scans_updated_, xyzi, total, off.data()));
-    // host-side load-time VoxelGrid, keyframes are independent (the reference's loadKeyframes loop is serial; the per-scan
-    // arithmetic and its std::sort are unchanged, only different scans run on different threads).  Scans that take PCL's overflow
-    // exit -- the common case for 0.05 m leaves on outdoor scans -- go from one staging buffer to the other with a single memcpy.
-    VoxelGridBatch vg;
-    vg.plan(xyzi, off.data(), K, P.downsample_voxel_size);
-    const std::vector<int64_t>& out_off = vg.out_off;
-    const float* out = xyzi;            // every scan passed through unchanged: the downloaded buffer IS the next session's input
-    if (std::find(vg.unchanged.begin(), vg.unchanged.end(), (uint8_t)0) != vg.unchanged.end()) {
-        if (!grow(&pin_out_, &pin_out_cap_, (size_t)std::max<int64_t>(out_off[(size_t)K], 1) * 16)) return fail(LTR_ERR_NOMEM, "cascade: pinned staging allocation failed");
-        vg.emit(xyzi, off.data(), (float*)pin_out_);
-        out = (const float*)pin_out_;
-    }
+    ltr_scanset promoted = -1;
+    if (owns(C)) CK(ltr_voxel_grid_per_keyframe(ctx, C.keyframe_scans_updated_, P.downsample_voxel_size, &promoted, nullptr));
     for (Session* s : {&central_sess_, &query_sess_}) {
         for (auto& kv : s->cloud_names()) if (*kv.second >= 0) { CK(ltr_cloud_free(ctx, *kv.second)); *kv.second = -1; }
         for (auto& kv : s->scanset_names()) if (*kv.second >= 0) { CK(ltr_scanset_free(ctx, *kv.second)); *kv.second = -1; }
@@ -710,11 +700,7 @@ int Removerter::cascade_promote_updated() {
     saved.clear();
     if (query_sess_.keyframe_poses_ >= 0) { CK(ltr_poses_free(ctx, query_sess_.keyframe_poses_)); query_sess_.keyframe_poses_ = -1; }
     query_sess_.num_keyframes_ = 0;
-    if (owns(C)) {
-        ltr_scanset ss;
-        CK(ltr_scanset_upload(ctx, out, out_off.data(), K, &ss));
-        C.keyframe_scans_ = ss;
-    }
+    if (owns(C)) C.keyframe_scans_ = promoted;
     log.clear();
     timing.clear();
     return LTR_OK;
@@ -786,6 +772,11 @@ int ltrh_load_session(ltrh_removerter* r, int32_t sess, const float* xyzi, const
     if (!r || (sess != 0 && sess != 1)) return LTR_ERR_INVALID;
     r->R->err.clear();
     return r->R->load_session(sess, xyzi, offsets, poses, inv_poses, K);
+}
+int ltrh_load_session_raw(ltrh_removerter* r, int32_t sess, const float* xyzi, const int64_t* offsets, const double* poses, const double* inv_poses, int32_t K) {
+    if (!r || (sess != 0 && sess != 1)) return LTR_ERR_INVALID;
+    r->R->err.clear();
+    return r->R->load_session_raw(sess, xyzi, offsets, poses, inv_poses, K);
 }
 int ltrh_run_step0(ltrh_removerter* r) { r->R->err.clear(); return r->R->run_step0(); }
 int ltrh_run_step12(ltrh_removerter* r) { r->R->err.clear(); return r->R->run_step12(); }

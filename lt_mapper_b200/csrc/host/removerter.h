@@ -89,6 +89,10 @@ public:
 
     // ---- plumbing ----
     int load_session(int sess, const float* xyzi, const int64_t* offsets, const double* poses, const double* inv_poses, int K);
+    // raw scans as read from disk: Session::loadKeyframes' VoxelGrid(downsample_voxel_size) on the device, then load_session's state;
+    // n_overflowed (optional) = scans the filter returned unchanged
+    int load_session_raw(int sess, const float* xyzi, const int64_t* offsets, const double* poses, const double* inv_poses, int K,
+                         int32_t* n_overflowed = nullptr);
     int set(ltr_cloud* slot, ltr_cloud v);         // frees what the slot held, then stores v
     int set(ltr_scanset* slot, ltr_scanset v, bool);
     int assign(ltr_cloud* dst, ltr_cloud src);     // "*dst = *src" (deep copy)
@@ -118,8 +122,6 @@ public:
     // Off by default: on 4 NVLinked ranks the two size exchanges + the exchange + the gather of a ~10 M point cloud cost more than sorting it on
     // every rank; LTR_DIST_VOXEL_MIN turns it on (the multi-rank tests do).
     int64_t dist_voxel_min = INT64_MAX;
-    void *pin_in_ = nullptr, *pin_out_ = nullptr;     // page-locked staging of cascade_promote_updated, grown on demand
-    size_t pin_in_cap_ = 0, pin_out_cap_ = 0;
     Session central_sess_, query_sess_;
     std::map<std::string, ltr_cloud> saved;
     std::map<std::string, double> timing;

@@ -41,7 +41,7 @@ class Comm(ctypes.Structure):
 
 
 HOST_EXPORTS = ["ltrh_params_default", "ltrh_create", "ltrh_destroy", "ltrh_last_error", "ltrh_set_comm", "ltrh_context", "ltrh_comm_init_nccl", "ltrh_owns_session", "ltrh_invert_poses",
-                "ltrh_load_session", "ltrh_run_step0", "ltrh_run_step12", "ltrh_run_step3", "ltrh_reset_to_step0", "ltrh_cascade_promote_updated", "ltrh_stage", "ltrh_cloud",
+                "ltrh_load_session", "ltrh_load_session_raw", "ltrh_run_step0", "ltrh_run_step12", "ltrh_run_step3", "ltrh_reset_to_step0", "ltrh_cascade_promote_updated", "ltrh_stage", "ltrh_cloud",
                 "ltrh_scanset", "ltrh_timing", "ltrh_log_count", "ltrh_log_get", "ltrh_io_last_error", "ltrh_io_read_pcd", "ltrh_io_write_pcd",
                 "ltrh_io_read_poses", "ltrh_io_parse_keyframes", "ltrh_io_parse_keyframes_in_roi", "ltrh_io_voxel_grid", "ltrh_io_voxel_grid_scans", "ltrh_io_yaml_get"]
 
@@ -71,6 +71,7 @@ def host_lib():
     L.ltrh_invert_poses.argtypes = [vp, i32, vp]
     L.ltrh_invert_poses.restype = None
     L.ltrh_load_session.argtypes = [vp, i32, vp, vp, vp, vp, i32]
+    L.ltrh_load_session_raw.argtypes = [vp, i32, vp, vp, vp, vp, i32]
     for f in ("ltrh_run_step0", "ltrh_run_step12", "ltrh_run_step3", "ltrh_reset_to_step0", "ltrh_cascade_promote_updated"):
         getattr(L, f).argtypes = [vp]
     L.ltrh_stage.argtypes = [vp, ctypes.c_char_p]
@@ -293,6 +294,16 @@ class Removerter:
         p = np.ascontiguousarray(poses, np.float64)
         ip = np.ascontiguousarray(inv_poses, np.float64)
         self._ck(host_lib().ltrh_load_session(self._h, sess, x.ctypes.data, o.ctypes.data, p.ctypes.data, ip.ctypes.data, len(o) - 1))
+        self.K[sess] = len(o) - 1
+
+    def load_session_raw(self, sess, xyzi, offsets, poses, inv_poses):
+        """load_session from the scans as read from disk: the load-time VoxelGrid at `voxel` runs on the device first
+        (ltrh_load_session_raw, Session::loadKeyframes)."""
+        x = np.ascontiguousarray(xyzi, np.float32)
+        o = np.ascontiguousarray(offsets, np.int64)
+        p = np.ascontiguousarray(poses, np.float64)
+        ip = np.ascontiguousarray(inv_poses, np.float64)
+        self._ck(host_lib().ltrh_load_session_raw(self._h, sess, x.ctypes.data, o.ctypes.data, p.ctypes.data, ip.ctypes.data, len(o) - 1))
         self.K[sess] = len(o) - 1
 
     def run_step0(self):

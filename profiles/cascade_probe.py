@@ -1,6 +1,6 @@
 """BASELINE configs[4] shape at single-GPU scale: an S-session cascaded LT-map.  Session 0 is the live map; every further session is
 diffed against it (Steps 0-3) and the updated scans are promoted to the next live map (ltrh_cascade_promote_updated).  Wall-clock per
-stage includes the pinned-host -> device upload of the new query session and the host-side VoxelGrid of the promoted scans (what the
+stage includes the pinned-host -> device upload of the new query session and the device-side VoxelGrid of the promoted scans (what the
 reference's file protocol does at load).  Usage: python profiles/cascade_probe.py [sessions=6] [keyframes=100] > cascade.json"""
 import json
 import os
