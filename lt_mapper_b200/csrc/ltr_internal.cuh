@@ -50,13 +50,20 @@ struct DevPoses {
 // slots owns one storage block that outlives the sets it holds (dropping a set only marks the slot empty), so the step's passes reuse
 // two blocks instead of allocating and freeing multi-GB images.
 constexpr int kMaxScanImageSets = 2;   // remove(r), revert(0.95 r), remove(r) alternate between two resolutions
-struct ScanImageSet {
-    void* block = nullptr;        // storage: rimg | timg | pyr
-    size_t cap = 0;               // its bytes
-    bool valid = false;           // holds the images of the key below
+struct ScanImageKey {
     uint64_t scans_serial = 0, poses_serial = 0;
     int kf_begin = 0, kf_end = 0, rows = 0, cols = 0, order = 0, ext_identity = 0, fast_path = 0;
     float vfov = 0.0f, hfov = 0.0f;
+    bool operator==(const ScanImageKey& o) const {
+        return scans_serial == o.scans_serial && poses_serial == o.poses_serial && kf_begin == o.kf_begin && kf_end == o.kf_end && rows == o.rows &&
+               cols == o.cols && order == o.order && ext_identity == o.ext_identity && fast_path == o.fast_path && vfov == o.vfov && hfov == o.hfov;
+    }
+};
+struct ScanImageSet {
+    void* block = nullptr;        // storage: rimg | timg | pyr
+    size_t cap = 0;               // its bytes
+    bool valid = false;           // holds the images of `key`
+    ScanImageKey key;
     uint32_t* rimg = nullptr;     // scan range images, (kf_end - kf_begin) x rows x cols
     float* pyr = nullptr;         // sliding-window maxima of tile culling (project_cull.cuh), built for pyr_shortcut
     uint32_t* timg = nullptr;     // test image of the scan-minus-map fast path (scan_test_image_kernel), built for timg_shortcut

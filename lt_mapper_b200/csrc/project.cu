@@ -10,6 +10,7 @@
 // Determinism: the reference's per-pixel min is a racy OpenMP loop; its sequential meaning (min range, lowest
 // index among equal ranges) is obtained here with one 64-bit atomicMin on (float_bits(range) << 32 | index).
 #include "ltr_internal.cuh"
+#include "device_util.cuh"
 #include "ref_math.cuh"
 #include "project_fast.cuh"
 #include <algorithm>
@@ -17,6 +18,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <tuple>
+#include <type_traits>
 
 namespace ltr {
 
@@ -32,19 +34,13 @@ __global__ void fill_u64_kernel(uint64_t* __restrict__ p, uint64_t v, int64_t n)
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) p[i] = v;
 }
 
-__device__ __forceinline__ int find_kf_rel(const int64_t* __restrict__ off, int nb, int64_t i) {
-    int lo = 0, hi = nb;
-    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (off[mid] <= i) lo = mid; else hi = mid; }
-    return lo;
-}
-
 // scan2RangeImg for the keyframes [kf0, kf0+nb): per-pixel min range via 32-bit atomicMin on the float bits (ranges >= 0).
 __global__ void __launch_bounds__(256) scan_rimg_kernel(PtrView scans, const int64_t* __restrict__ off, int kf0, int nb, ImgShape g,
                                                         uint32_t* __restrict__ rimg) {
     const int64_t begin = off[kf0], end = off[kf0 + nb];
     const int64_t i = begin + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= end) return;
-    const int k = find_kf_rel(off + kf0, nb, i);
+    const int k = find_kf(off + kf0, nb, i);
     const Sph s = cart2sph(scans.x[i], scans.y[i], scans.z[i]);
     int r, c;
     pixel_index(s, g, &r, &c);
@@ -61,7 +57,7 @@ __global__ void __launch_bounds__(256) scan_rimg_fast_kernel(PtrView scans, cons
     const int64_t begin = off[kf0], end = off[kf0 + nb];
     const int64_t i = begin + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= end) return;
-    const int k = find_kf_rel(off + kf0, nb, i);
+    const int k = find_kf(off + kf0, nb, i);
     const float x = scans.x[i], y = scans.y[i], z = scans.z[i];
     const FastProj f = fast_sph<kElDirect>(x, y, z);
     int r, c;
@@ -113,23 +109,9 @@ __global__ void __launch_bounds__(256) map_project_kernel(PtrView map, const dou
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= map.n) return;
     const float x = map.x[i], y = map.y[i], z = map.z[i];
-    const size_t npx = (size_t)g.rows * g.cols;
-    for (int k = 0; k < nb; ++k) {
-        float lx, ly, lz;
-        transform_point(s_pose + 12 * k, order, x, y, z, &lx, &ly, &lz);        // utility.cpp:70
-        if (!ext_identity) transform_point(ext, order, lx, ly, lz, &lx, &ly, &lz);  // utility.cpp:71
-        const Sph s = cart2sph(lx, ly, lz);
-        int r, c;
-        pixel_index(s, g, &r, &c);
-        const size_t px = (size_t)k * npx + (size_t)r * g.cols + c;
-        const uint64_t packed = ((uint64_t)__float_as_uint(s.r) << 32) | (uint32_t)i;
-        if (kCandidatesOnly) {
-            const float sr = __uint_as_float(scan_rimg[px]);
-            if (fs(sr, s.r) > thres) atomicMin((unsigned long long*)&win[px], (unsigned long long)packed);
-        } else {
-            if (packed < win[px]) atomicMin((unsigned long long*)&win[px], (unsigned long long)packed);
-        }
-    }
+    unsigned n_atomics = 0;   // not reported by this kernel
+    for (int k = 0; k < nb; ++k)
+        exact_pair<kCandidatesOnly>(x, y, z, (uint32_t)i, (uint32_t)k, s_pose + 12 * k, ext, ext_identity, order, g, scan_rimg, thres, win, 0, &n_atomics);
 }
 
 // calcDescrepancyAndParseDynamicPointIdx (Removerter.cpp:381-413) over the batch images; also re-arms `win`.
@@ -190,30 +172,18 @@ __global__ void __launch_bounds__(1024) parse_compact_kernel(uint64_t* __restric
         if (lane == 0) s_base = b;
     }
     __syncthreads();
+    int base = s_base;
     const int p1 = min((c + 1) * kParseChunk, npx);
     for (int p0 = c * kParseChunk; p0 < p1; p0 += blockDim.x) {
         const int p = p0 + threadIdx.x;
         uint32_t idx = 0;
         if (p < p1) { const uint64_t v = w[p]; idx = (uint32_t)v; if (v != kWinEmpty) w[p] = kWinEmpty; }
-        const bool keep = idx != 0;
-        const unsigned b = __ballot_sync(0xffffffffu, keep);
-        const int wrank = __popc(b & ((1u << lane) - 1u));
-        if (lane == 0) s_warp[warp] = __popc(b);
-        __syncthreads();
-        if (warp == 0) {
-            const int v = s_warp[lane];
-            int incl = v;
-            for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, incl, o); if ((int)lane >= o) incl += t; }
-            s_warp[lane] = incl - v;
-            if (lane == 31) s_warp[32] = incl;
-        }
-        __syncthreads();
-        if (keep) out[s_base + s_warp[warp] + wrank] = idx;
-        __syncthreads();
-        if (threadIdx.x == 0) s_base += s_warp[32];
-        __syncthreads();
+        int total;
+        const int rank = block_rank(idx != 0, &total, s_warp);
+        if (idx != 0) out[base + rank] = idx;
+        base += total;
     }
-    if (c == nchunk - 1 && threadIdx.x == 0) count[k] = (unsigned int)s_base;
+    if (c == nchunk - 1 && threadIdx.x == 0) count[k] = (unsigned int)base;
 }
 
 // emits map_local[ptidx] for every listed index: exact two-step transform of the winning map point
@@ -222,11 +192,10 @@ __global__ void __launch_bounds__(256) parse_emit_kernel(PtrView map, const doub
                                                          int ext_identity, int order, DevCloud out) {
     const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= out.n) return;
-    const int k = find_kf_rel(out_off, K, j);
+    const int k = find_kf(out_off, K, j);
     const uint32_t idx = list[(size_t)k * npx + (size_t)(j - out_off[k])];
-    float x = map.x[idx], y = map.y[idx], z = map.z[idx];
-    transform_point(poses + (size_t)(kf_begin + k) * 24, order, x, y, z, &x, &y, &z);
-    if (!ext_identity) transform_point(ext, order, x, y, z, &x, &y, &z);
+    float x, y, z;
+    map_to_sensor(poses + (size_t)(kf_begin + k) * 24, ext, ext_identity, order, map.x[idx], map.y[idx], map.z[idx], &x, &y, &z);
     out.x()[j] = x; out.y()[j] = y; out.z()[j] = z; out.i()[j] = map.i[idx];
 }
 
@@ -291,8 +260,7 @@ __global__ void debug_fast_kernel(const float* __restrict__ xyz, int64_t n, cons
     out[8 * i + 2] = f.r;
     out[8 * i + 3] = f.rho_inv_r;
     float lx, ly, lz;
-    transform_point(pose, order, x, y, z, &lx, &ly, &lz);
-    if (!ext_identity) transform_point(ext, order, lx, ly, lz, &lx, &ly, &lz);
+    map_to_sensor(pose, ext, ext_identity, order, x, y, z, &lx, &ly, &lz);
     const Sph s = cart2sph(lx, ly, lz);
     // the reference's pre-round floats (utility.cpp:122-123)
     out[8 * i + 4] = fm((float)g.cols, fd(fa(rad2deg(s.az), fd(g.hfov, 2.0f)), fs(g.hfov, 0.0f)));
@@ -338,32 +306,129 @@ static inline KfBatch make_kf_batch(const DevPoses& poses, int k0, int nb) {
     return kb;
 }
 
-// one launch of the fast projection over the keyframes [k0, k0 + nb) of `poses`
-template <bool kCand, bool kDeferred = false>
-static void launch_fast(ltr_ctx* ctx, const DevCloud& map, const DevPoses& poses, int k0, int nb, const ImgShape& g, const FastCfg& fc,
-                        const uint32_t* rimg, const uint32_t* test_img, float thres, uint64_t* win, uint32_t* amin, const CullArgs& ca,
-                        DeferredArgs da = DeferredArgs{nullptr, nullptr, nullptr, nullptr, 0}) {
-    const unsigned fb = fast_grid(ctx, map.n);
-    unsigned int* work = (unsigned int*)(ctx->d_counters + 4);
-    cudaMemsetAsync(work, 0, sizeof(unsigned int), ctx->stream);
-    const KfBatch kb = make_kf_batch(poses, k0, nb);
-    if (kDeferred) {
-        cudaMemsetAsync(da.best, 0xff, (size_t)nb * g.rows * g.cols * sizeof(unsigned long long), ctx->stream);   // "no pair yet"
-        cudaMemsetAsync(da.count, 0, sizeof(unsigned int), ctx->stream);
+// What a pass resolves once per call.
+struct PassPlan {
+    ImgShape g;
+    int64_t npx;
+    bool use_fast;           // the fast path, within its queue-entry field widths and 32-bit pixel offsets (project_fast.cuh)
+    FastCfg fc;              // its constants; empty_scan_shortcut = 0 until the remove pass sets its own
+    int B;                   // keyframes per launch: fast path at most kFastMaxBatch (their constants travel as a kernel parameter), exact
+                             // path 12 doubles of shared memory per keyframe
+    std::vector<int> units;  // keyframes of each projection launch (prof_collect)
+};
+
+static int plan_pass(ltr_ctx* ctx, float res_alpha, int nkf, PassPlan* p) {
+    int32_t rows, cols;
+    ltr_reset_rimg_size(ctx->cfg.vfov_deg, ctx->cfg.hfov_deg, res_alpha, &rows, &cols);
+    if (rows < 1 || cols < 1) return fail(ctx, LTR_ERR_INVALID, "range image %dx%d is empty (res_alpha %g)", rows, cols, res_alpha);
+    p->g = ImgShape{rows, cols, ctx->cfg.vfov_deg, ctx->cfg.hfov_deg};
+    p->npx = (int64_t)rows * cols;
+    p->use_fast = ctx->cfg.fast_path && p->npx <= (1 << 18);
+    p->fc = make_fast_cfg(rows, cols, ctx->cfg.vfov_deg, ctx->cfg.hfov_deg, 0);
+    p->B = std::max(1, std::min(std::min(ctx->cfg.keyframe_batch, p->use_fast ? kFastMaxBatch : 400), nkf));
+    return LTR_OK;
+}
+
+// the keyframe range of a pass over K keyframes, and a map whose indices fit the 32-bit index half of the winner image's keys
+static int check_pass_range(ltr_ctx* ctx, const DevCloud& map, int kf_begin, int kf_end, int K) {
+    if (kf_begin < 0 || kf_end > K || kf_begin > kf_end) return fail(ctx, LTR_ERR_INVALID, "keyframe range [%d,%d) outside [0,%d)", kf_begin, kf_end, K);
+    if (map.n >= ((int64_t)1 << 32)) return fail(ctx, LTR_ERR_UNSUPPORTED, "map larger than 2^32 points");
+    return LTR_OK;
+}
+
+// start of a pass's timed part: the fast path's device counters, the start event, no event pairs yet
+static int pass_begin(ltr_ctx* ctx, const PassPlan& p) {
+    if (p.use_fast) LTR_CUDA(ctx, cudaMemsetAsync(ctx->d_counters, 0, 4 * sizeof(unsigned long long), ctx->stream));
+    LTR_CUDA(ctx, cudaEventRecord(ctx->ev0, ctx->stream));
+    ctx->ev_used = 0;
+    return LTR_OK;
+}
+
+// after the pass's final synchronisation on ev1: the projection launches' event pairs into prof[slot .. slot + 3], and stats[0..4] of a
+// pass over n map points and nkf keyframes (the fast path's device counters are fetched lazily by ltr_last_pass_stats)
+static void pass_end(ltr_ctx* ctx, const PassPlan& p, int slot, double bytes_per_launch_unit, int64_t n, int nkf) {
+    float ms = 0.0f;
+    cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
+    prof_collect(ctx, slot, bytes_per_launch_unit, (double)n, p.units);
+    ctx->stats[0] = (double)n * nkf;
+    ctx->stats[1] = 0; ctx->stats[2] = ctx->stats[0]; ctx->stats[3] = 0;
+    ctx->stats_counters_pending = p.use_fast;
+    ctx->stats[4] = (double)ms * 1000.0;
+}
+
+// FastCfg::el_direct as the kElDirect template argument: f(std::true_type{}) or f(std::false_type{})
+template <class F>
+static auto with_el_direct(const FastCfg& fc, F f) { return fc.el_direct ? f(std::true_type{}) : f(std::false_type{}); }
+
+// what one launch of the map projection computes in the winner image
+enum class Proj {
+    kScanMinusMap,      // HD / revert / PD: the pixel winner among the candidates, scan - map > thres
+    kTrueMin,           // ND, visible-point extraction: the true per-pixel minimum
+    kTrueMinDeferred,   // the same through the deferred mode of project_fast.cuh (fast path only): the fast kernel, then deferred_resolve_kernel
+};
+
+using FastKernel = decltype(&map_project_fast_kernel<true, true, false, true>);
+
+// One launch of the map projection over the keyframes [k0, k0 + nb) of `poses` into `win`, timed by an event pair.  rimg: the launch's scan
+// range images (scan-minus-map; unused by the true minimum), test_img: the test image of the scan-minus-map fast path.  amin (fast path,
+// may be null in the deferred mode): the approximate running minimum, reset here.  da: the deferred mode's scratch.
+static int project_map(ltr_ctx* ctx, PassPlan& p, const DevCloud& map, const DevPoses& poses, int k0, int nb, Proj mode, const uint32_t* rimg,
+                       const uint32_t* test_img, float thres, uint64_t* win, uint32_t* amin, const CullArgs& ca, const DeferredArgs& da) {
+    const bool cand = mode == Proj::kScanMinusMap;
+    if (amin) {
+        fill_u32_kernel<<<grid_for(nb * p.npx, 256, ctx->sm_count * 8), 256, 0, ctx->stream>>>(amin, 0x7f800000u, nb * p.npx);
+        LTR_LAUNCH_CHECK(ctx);
     }
-    if (kCand && !kDeferred && fc.pad_ok)   // test_img is the guard-padded test image
-        map_project_fast_kernel<kCand, true, kDeferred, kCand && !kDeferred><<<fb, kFastThreads, fast_smem_bytes(), ctx->stream>>>(view(map), kb, poses.d, k0, nb,
-            ctx->d_ext, ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, g, fc, rimg, test_img, thres, win, amin, ca, ctx->d_counters, work, da);
-    else if (fc.el_direct) map_project_fast_kernel<kCand, true, kDeferred><<<fb, kFastThreads, fast_smem_bytes(), ctx->stream>>>(view(map), kb, poses.d, k0, nb, ctx->d_ext,
-        ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, g, fc, rimg, test_img, thres, win, amin, ca, ctx->d_counters, work, da);
-    else map_project_fast_kernel<kCand, false, kDeferred><<<fb, kFastThreads, fast_smem_bytes(), ctx->stream>>>(view(map), kb, poses.d, k0, nb, ctx->d_ext,
-        ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, g, fc, rimg, test_img, thres, win, amin, ca, ctx->d_counters, work, da);
-    if (kDeferred) {
-        const int64_t total = (int64_t)nb * g.rows * g.cols;
-        ctx->launches++;
-        deferred_resolve_kernel<<<grid_for(total, 256, ctx->sm_count * 16), 256, 0, ctx->stream>>>(view(map), poses.d, k0, nb, ctx->d_ext, ctx->ext_identity ? 1 : 0,
-            ctx->cfg.transform_order, (uint32_t)(g.rows * g.cols), da, win, ctx->d_counters);
+    prof_begin(ctx);
+    p.units.push_back(nb);
+    if (!p.use_fast) {
+        const auto kern = cand ? map_project_kernel<true> : map_project_kernel<false>;
+        kern<<<(unsigned)((map.n + 255) / 256), 256, (size_t)nb * 12 * sizeof(double), ctx->stream>>>(view(map), poses.d, k0, nb, ctx->d_ext,
+            ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, p.g, rimg, thres, win);
+    } else {
+        unsigned int* work = (unsigned int*)(ctx->d_counters + 4);
+        LTR_CUDA(ctx, cudaMemsetAsync(work, 0, sizeof(unsigned int), ctx->stream));
+        const bool deferred = mode == Proj::kTrueMinDeferred;
+        if (deferred) {
+            LTR_CUDA(ctx, cudaMemsetAsync(da.best, 0xff, (size_t)nb * p.npx * sizeof(unsigned long long), ctx->stream));   // "no pair yet"
+            LTR_CUDA(ctx, cudaMemsetAsync(da.count, 0, sizeof(unsigned int), ctx->stream));
+        }
+        // template arguments <candidates only, short elevation path, deferred, guard-padded test image>
+        const FastKernel kern = (cand && p.fc.pad_ok) ? map_project_fast_kernel<true, true, false, true>
+            : with_el_direct(p.fc, [mode](auto el) -> FastKernel {
+                  constexpr bool kEl = decltype(el)::value;
+                  return mode == Proj::kScanMinusMap ? map_project_fast_kernel<true, kEl, false>
+                       : mode == Proj::kTrueMin      ? map_project_fast_kernel<false, kEl, false>
+                                                     : map_project_fast_kernel<false, kEl, true>;
+              });
+        kern<<<fast_grid(ctx, map.n), kFastThreads, fast_smem_bytes(), ctx->stream>>>(view(map), make_kf_batch(poses, k0, nb), poses.d, k0, nb, ctx->d_ext,
+            ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, p.g, p.fc, rimg, cand ? test_img : amin, thres, win, amin, ca, ctx->d_counters, work, da);
+        if (deferred) {
+            LTR_LAUNCH_CHECK(ctx);
+            deferred_resolve_kernel<<<grid_for(nb * p.npx, 256, ctx->sm_count * 16), 256, 0, ctx->stream>>>(view(map), poses.d, k0, nb, ctx->d_ext,
+                ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, (uint32_t)p.npx, da, win, ctx->d_counters);
+        }
     }
+    prof_end(ctx);
+    LTR_LAUNCH_CHECK(ctx);
+    return LTR_OK;
+}
+
+// scan2RangeImg of the keyframes [kf0, kf0 + n) of `scans` into n images at rimg, through the fast pixel evaluation on the fast path
+static int scan_rimg(ltr_ctx* ctx, const PassPlan& p, const DevScanSet& scans, int kf0, int n, uint32_t* rimg) {
+    fill_u32_kernel<<<grid_for(n * p.npx, 256, ctx->sm_count * 8), 256, 0, ctx->stream>>>(rimg, kNoPointBits, n * p.npx);
+    LTR_LAUNCH_CHECK(ctx);
+    const int64_t npts = scans.h_off[kf0 + n] - scans.h_off[kf0];
+    if (npts == 0) return LTR_OK;
+    const unsigned blocks = (unsigned)((npts + 255) / 256);
+    if (p.use_fast) {
+        const auto kern = with_el_direct(p.fc, [](auto el) { return scan_rimg_fast_kernel<decltype(el)::value>; });
+        kern<<<blocks, 256, 0, ctx->stream>>>(view(scans.pts), scans.d_off, kf0, n, p.g, p.fc, rimg);
+    } else {
+        scan_rimg_kernel<<<blocks, 256, 0, ctx->stream>>>(view(scans.pts), scans.d_off, kf0, n, p.g, rimg);
+    }
+    LTR_LAUNCH_CHECK(ctx);
+    return LTR_OK;
 }
 
 // Near-to-far claim order of the deferred mode (DeferredArgs::order): per tile, a lower bound of its distance from `o` (a reference
@@ -402,29 +467,21 @@ static int deferred_alloc(ltr_ctx* ctx, int B, int64_t npx, void** block, Deferr
 //   rimg  the scan range image (scan2RangeImg), built here when make_rimg, else read;
 //   pyr   (if non-null) its sliding-window maxima for tile culling; an empty scan pixel is -inf with the shortcut, else +inf;
 //   timg  (if non-null) the test image of the scan-minus-map fast path, guard-padded when `pad`, empty pixels -inf with the shortcut.
-// None of them reads the map.  Launches cover at most kImageChunk keyframes (the window-maximum grid's z extent).
+// The shortcut is the plan's FastCfg::empty_scan_shortcut.  None of them reads the map.  Launches cover at most kImageChunk keyframes (the
+// window-maximum grid's z extent).
 constexpr int kImageChunk = 1024;
-static int build_scan_images(ltr_ctx* ctx, const DevScanSet& scans, int k0, int nb, const ImgShape& g, const FastCfg& fc, bool use_fast, int shortcut,
-                             bool make_rimg, uint32_t* rimg, float* pyr, uint32_t* timg, bool pad) {
-    const int64_t npx = (int64_t)g.rows * g.cols;
-    const int64_t timg_px = pad ? (int64_t)fc.pad_npx : npx;
+static int build_scan_images(ltr_ctx* ctx, const PassPlan& p, const DevScanSet& scans, int k0, int nb, bool make_rimg, uint32_t* rimg, float* pyr,
+                             uint32_t* timg, bool pad) {
+    const ImgShape& g = p.g;
+    const int64_t npx = p.npx;
+    const int shortcut = p.fc.empty_scan_shortcut;
+    const int64_t timg_px = pad ? (int64_t)p.fc.pad_npx : npx;
     const unsigned pyr_stride = (unsigned)(kPyrLevels * npx);
     const int fill_blocks = ctx->sm_count * 8;
     for (int c0 = 0; c0 < nb; c0 += kImageChunk) {
         const int n = std::min(kImageChunk, nb - c0);
         uint32_t* ri = rimg + (size_t)c0 * npx;
-        if (make_rimg) {
-            fill_u32_kernel<<<grid_for(n * npx, 256, fill_blocks), 256, 0, ctx->stream>>>(ri, kNoPointBits, n * npx);
-            LTR_LAUNCH_CHECK(ctx);
-            const int kf0 = k0 + c0;
-            const int64_t npts = scans.h_off[kf0 + n] - scans.h_off[kf0];
-            if (npts > 0) {
-                if (use_fast && fc.el_direct) scan_rimg_fast_kernel<true><<<(unsigned)((npts + 255) / 256), 256, 0, ctx->stream>>>(view(scans.pts), scans.d_off, kf0, n, g, fc, ri);
-                else if (use_fast) scan_rimg_fast_kernel<false><<<(unsigned)((npts + 255) / 256), 256, 0, ctx->stream>>>(view(scans.pts), scans.d_off, kf0, n, g, fc, ri);
-                else scan_rimg_kernel<<<(unsigned)((npts + 255) / 256), 256, 0, ctx->stream>>>(view(scans.pts), scans.d_off, kf0, n, g, ri);
-                LTR_LAUNCH_CHECK(ctx);
-            }
-        }
+        if (make_rimg) LTR_TRY(scan_rimg(ctx, p, scans, k0 + c0, n, ri));
         if (pyr) {
             const float empty_value = shortcut ? -__builtin_huge_valf() : __builtin_huge_valf();   // empty scan pixel: never flags / unknown
             const dim3 wg((unsigned)((g.cols + kWinTile - 1) / kWinTile), (unsigned)((g.rows + kWinTile - 1) / kWinTile), (unsigned)n);
@@ -433,7 +490,7 @@ static int build_scan_images(ltr_ctx* ctx, const DevScanSet& scans, int k0, int 
         }
         if (timg) {
             scan_test_image_kernel<<<grid_for(n * timg_px, 256, fill_blocks), 256, 0, ctx->stream>>>(ri, timg + (size_t)c0 * timg_px, n, g.rows, g.cols,
-                                                                                                    pad ? fc.pad_g : 0, pad ? 1 : 0, shortcut);
+                                                                                                    pad ? p.fc.pad_g : 0, pad ? 1 : 0, shortcut);
             LTR_LAUNCH_CHECK(ctx);
         }
     }
@@ -450,7 +507,7 @@ static void scan_image_set_drop(ScanImageSet& s) {
 
 void scan_images_release(ltr_ctx* ctx, uint64_t serial, bool free_storage) {
     for (ScanImageSet& s : ctx->scan_images) {
-        if (serial == 0 || s.scans_serial == serial || s.poses_serial == serial) scan_image_set_drop(s);
+        if (serial == 0 || s.key.scans_serial == serial || s.key.poses_serial == serial) scan_image_set_drop(s);
         if (free_storage && serial == 0) { dev_free(ctx, s.block); s.block = nullptr; s.cap = 0; }
     }
 }
@@ -483,25 +540,24 @@ struct ScanImagesPin {
 // A new set goes into an empty slot or the least recently used one, preferring a slot whose storage is already large enough; storage only
 // grows.  *out = nullptr when the sets are off or the storage would exceed the budget: the pass then builds its images per launch.  The
 // caller holds a ScanImagesPin.
-static int scan_images_get(ltr_ctx* ctx, const DevScanSet& scans, const DevPoses& poses, int kf_begin, int kf_end, const ImgShape& g, const FastCfg& fc,
-                           bool use_fast, int shortcut, bool need_pyr, bool need_timg, bool pad, ScanImageSet** out) {
+static int scan_images_get(ltr_ctx* ctx, const PassPlan& p, const DevScanSet& scans, const DevPoses& poses, int kf_begin, int kf_end, bool need_pyr,
+                           bool need_timg, bool pad, ScanImageSet** out) {
     *out = nullptr;
     size_t budget = 0;
     if (!scan_image_cache_on(&budget)) return LTR_OK;
     const int K = kf_end - kf_begin;
-    const size_t npx = (size_t)g.rows * g.cols;
+    const int shortcut = p.fc.empty_scan_shortcut;
+    const size_t npx = (size_t)p.npx;
     const size_t rimg_bytes = (size_t)K * npx * sizeof(uint32_t), pyr_bytes = rimg_bytes * kPyrLevels;
-    const size_t timg_bytes = (size_t)K * (pad ? (size_t)fc.pad_npx : npx) * sizeof(uint32_t);
+    const size_t timg_bytes = (size_t)K * (pad ? (size_t)p.fc.pad_npx : npx) * sizeof(uint32_t);
     // storage layout rimg | timg | pyr (256 B aligned): a set that needs the window table needs the whole block
     const size_t timg_off = (rimg_bytes + 255) / 256 * 256, pyr_off = timg_off + (timg_bytes + 255) / 256 * 256;
     const size_t need = need_pyr ? pyr_off + pyr_bytes : need_timg ? timg_off + timg_bytes : rimg_bytes;
-    const int ext = ctx->ext_identity ? 1 : 0;
+    const ScanImageKey key{scans.serial, poses.serial, kf_begin, kf_end, p.g.rows, p.g.cols, ctx->cfg.transform_order, ctx->ext_identity ? 1 : 0,
+                           ctx->cfg.fast_path, p.g.vfov, p.g.hfov};
     ScanImageSet* s = nullptr;
     for (ScanImageSet& c : ctx->scan_images)
-        if (c.valid && c.scans_serial == scans.serial && c.poses_serial == poses.serial && c.kf_begin == kf_begin && c.kf_end == kf_end && c.rows == g.rows &&
-            c.cols == g.cols && c.vfov == g.vfov && c.hfov == g.hfov && c.order == ctx->cfg.transform_order && c.ext_identity == ext &&
-            c.fast_path == ctx->cfg.fast_path)
-            s = &c;
+        if (c.valid && c.key == key) s = &c;
     if (s && s->cap < need) scan_image_set_drop(*s);   // a part it lacks does not fit its storage: rebuild the set in a larger block
     if (!s || !s->valid) {
         if (!s) {   // empty before occupied, large enough before too small, then least recently used
@@ -529,8 +585,7 @@ static int scan_images_get(ltr_ctx* ctx, const DevScanSet& scans, const DevPoses
             }
             s->cap = need;
         }
-        s->scans_serial = scans.serial; s->poses_serial = poses.serial; s->kf_begin = kf_begin; s->kf_end = kf_end; s->rows = g.rows; s->cols = g.cols;
-        s->vfov = g.vfov; s->hfov = g.hfov; s->order = ctx->cfg.transform_order; s->ext_identity = ext; s->fast_path = ctx->cfg.fast_path;
+        s->key = key;
     }
     char* base = (char*)s->block;
     const bool make_rimg = !s->valid;
@@ -541,8 +596,7 @@ static int scan_images_get(ltr_ctx* ctx, const DevScanSet& scans, const DevPoses
     s->pyr = s->cap >= pyr_off + pyr_bytes ? (float*)(base + pyr_off) : nullptr;
     if (make_rimg || make_pyr || make_timg) {
         s->valid = false;   // until the build is enqueued
-        LTR_TRY(build_scan_images(ctx, scans, kf_begin, K, g, fc, use_fast, shortcut, make_rimg, s->rimg, make_pyr ? s->pyr : nullptr,
-                                  make_timg ? s->timg : nullptr, pad));
+        LTR_TRY(build_scan_images(ctx, p, scans, kf_begin, K, make_rimg, s->rimg, make_pyr ? s->pyr : nullptr, make_timg ? s->timg : nullptr, pad));
         s->valid = true;
         if (make_pyr) s->pyr_shortcut = shortcut;
         if (make_timg) s->timg_shortcut = shortcut;
@@ -552,31 +606,26 @@ static int scan_images_get(ltr_ctx* ctx, const DevScanSet& scans, const DevPoses
     return LTR_OK;
 }
 
+// Runs pass(allow_deferred, &overflowed) and, when the deferred true-minimum mode's candidate list filled up (8 M entries; never seen),
+// repeats it in the immediate mode.
+template <class Pass>
+static int with_deferred_retry(Pass pass) {
+    bool overflowed = false;
+    LTR_TRY(pass(true, &overflowed));
+    if (overflowed) LTR_TRY(pass(false, &overflowed));
+    return LTR_OK;
+}
+
 }  // namespace ltr
 
 using namespace ltr;
 
 extern "C" {
 
-static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end,
-                            int32_t mode, float res_alpha, float diff_thres, int32_t accumulate, int64_t* n_dynamic, bool allow_deferred, bool* overflowed);
-
 int ltr_scan_images_release(ltr_ctx* ctx, int32_t free_storage) {
     ApiTrace tr__(ctx, "ltr_scan_images_release");
     if (!ctx) return LTR_ERR_INVALID;
     scan_images_release(ctx, 0, free_storage != 0);
-    return LTR_OK;
-}
-
-int ltr_remove_pass(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end,
-                    int32_t mode, float res_alpha, float diff_thres, int32_t accumulate, int64_t* n_dynamic) {
-    ApiTrace tr__(ctx, "ltr_remove_pass");
-    if (!ctx) return LTR_ERR_INVALID;
-    bool overflowed = false;
-    // ND (true per-pixel minimum) runs in the deferred mode of project_fast.cuh unless the flags accumulate into earlier ones (a run whose
-    // overflow list filled up would have to be undone); a full list -- never seen, the list holds 8 M entries -- repeats the pass in the immediate mode
-    LTR_TRY(remove_pass_impl(ctx, map_h, scans_h, poses_h, kf_begin, kf_end, mode, res_alpha, diff_thres, accumulate, n_dynamic, !accumulate, &overflowed));
-    if (overflowed) LTR_TRY(remove_pass_impl(ctx, map_h, scans_h, poses_h, kf_begin, kf_end, mode, res_alpha, diff_thres, accumulate, n_dynamic, false, &overflowed));
     return LTR_OK;
 }
 
@@ -591,45 +640,39 @@ static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, 
     LTR_TRY(poses_get(ctx, poses_h, &poses));
     if (mode != LTR_MODE_HD && mode != LTR_MODE_ND && mode != LTR_MODE_PD) return fail(ctx, LTR_ERR_INVALID, "unknown pass mode %d", mode);
     if (scans->K != poses->K) return fail(ctx, LTR_ERR_INVALID, "pose count %d != keyframe count %d (Session.cpp:117)", poses->K, scans->K);
-    if (kf_begin < 0 || kf_end > scans->K || kf_begin > kf_end) return fail(ctx, LTR_ERR_INVALID, "keyframe range [%d,%d) outside [0,%d)", kf_begin, kf_end, scans->K);
-    if (map->n >= ((int64_t)1 << 32)) return fail(ctx, LTR_ERR_UNSUPPORTED, "map larger than 2^32 points");
-    int32_t rows, cols;
-    ltr_reset_rimg_size(ctx->cfg.vfov_deg, ctx->cfg.hfov_deg, res_alpha, &rows, &cols);
-    if (rows < 1 || cols < 1) return fail(ctx, LTR_ERR_INVALID, "range image %dx%d is empty (res_alpha %g)", rows, cols, res_alpha);
+    LTR_TRY(check_pass_range(ctx, *map, kf_begin, kf_end, scans->K));
+    PassPlan p;
+    LTR_TRY(plan_pass(ctx, res_alpha, kf_end - kf_begin, &p));
     LTR_TRY(cloud_ensure_flags(ctx, map));
     if (!accumulate && map->n > 0) LTR_CUDA(ctx, cudaMemsetAsync(map->flags, 0, (size_t)map->n, ctx->stream));
-    const ImgShape g{rows, cols, ctx->cfg.vfov_deg, ctx->cfg.hfov_deg};
-    const int64_t npx = (int64_t)rows * cols;
+    const int64_t npx = p.npx;
+    const int B = p.B;
     const bool cand = (mode != LTR_MODE_ND);
-    const bool use_fast = ctx->cfg.fast_path && npx <= (1 << 18);   // queue-entry field widths, 32-bit pixel offsets (project_fast.cuh)
-    // fast path: at most kFastMaxBatch keyframes per launch (their constants travel as a kernel parameter); exact path: 12 doubles of shared memory per keyframe
-    const int B = std::max(1, std::min(std::min(ctx->cfg.keyframe_batch, use_fast ? kFastMaxBatch : 400), kf_end - kf_begin));
+    const bool run = map->n > 0 && kf_end > kf_begin;
     int shortcut = 0;
-    if (use_fast && cand && map->n > 0 && kf_end > kf_begin) LTR_TRY(empty_scan_shortcut_ok(ctx, *map, *poses, kf_begin, kf_end, &shortcut));
-    const FastCfg fc = make_fast_cfg(rows, cols, ctx->cfg.vfov_deg, ctx->cfg.hfov_deg, shortcut);
-    if (use_fast) LTR_CUDA(ctx, cudaMemsetAsync(ctx->d_counters, 0, 4 * sizeof(unsigned long long), ctx->stream));
-    const bool use_deferred = use_fast && !cand && allow_deferred;
+    if (p.use_fast && cand && run) LTR_TRY(empty_scan_shortcut_ok(ctx, *map, *poses, kf_begin, kf_end, &shortcut));
+    p.fc.empty_scan_shortcut = shortcut;
+    const bool use_deferred = p.use_fast && !cand && allow_deferred;
     void* p_def = nullptr;
     ScratchGuard g_def(ctx, &p_def);
-    DeferredArgs da{nullptr, nullptr, nullptr, nullptr, 0};
-    if (use_deferred && map->n > 0 && kf_end > kf_begin) LTR_TRY(deferred_alloc(ctx, B, npx, &p_def, &da));
+    DeferredArgs da{};
+    if (use_deferred && run) LTR_TRY(deferred_alloc(ctx, B, npx, &p_def, &da));
     // tile culling (project_cull.cuh): scan-minus-map variants only, one keyframe per lane -> launches of at most 32 keyframes
     CullArgs ca;
     std::memset(&ca, 0, sizeof(ca));
     // the sliding-window maxima cost 5 stores per pixel and keyframe: below one map point per pixel they cost more than the culling saves
     // (the small ND / PD candidate maps), so those passes project every pair
-    const bool use_cull = use_fast && cand && ctx->cfg.fast_path >= 2 && B <= 32 && map->n >= kTilePts && map->n >= npx;
+    const bool use_cull = p.use_fast && cand && ctx->cfg.fast_path >= 2 && B <= 32 && map->n >= kTilePts && map->n >= npx;
     void *p_tiles = nullptr, *p_pyr = nullptr;
     ScratchGuard g_tiles(ctx, &p_tiles), g_pyr(ctx, &p_pyr);
-    const bool run = map->n > 0 && kf_end > kf_begin;
     // scan-minus-map with the short elevation path and a 360 degree field of view: the test image is guard-padded (FastCfg::pad_*) and always built
-    const bool pad = use_fast && cand && fc.pad_ok;
-    const bool need_timg = use_fast && cand && (shortcut || pad);
-    const int64_t timg_px = pad ? (int64_t)fc.pad_npx : npx;
+    const bool pad = p.use_fast && cand && p.fc.pad_ok;
+    const bool need_timg = p.use_fast && cand && (shortcut || pad);
+    const int64_t timg_px = pad ? (int64_t)p.fc.pad_npx : npx;
     // the scan-side images come from a kept set built over the whole range (scan_images_get) or, without one, are built per launch
     ScanImagesPin pin(ctx);
     ScanImageSet* set = nullptr;
-    if (run) LTR_TRY(scan_images_get(ctx, *scans, *poses, kf_begin, kf_end, g, fc, use_fast, shortcut, use_cull, need_timg, pad, &set));
+    if (run) LTR_TRY(scan_images_get(ctx, p, *scans, *poses, kf_begin, kf_end, use_cull, need_timg, pad, &set));
     if (use_cull) {
         ca.enabled = 1;
         ca.ntiles = (map->n + kTilePts - 1) / kTilePts;
@@ -640,29 +683,23 @@ static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, 
         tile_sphere_kernel<<<(unsigned)((ca.ntiles * 32 + 255) / 256), 256, 0, ctx->stream>>>(view(*map), (float4*)p_tiles, ca.ntiles);
         LTR_LAUNCH_CHECK(ctx);
     }
-    LTR_CUDA(ctx, cudaEventRecord(ctx->ev0, ctx->stream));
-    std::vector<int> launch_units;
-    ctx->ev_used = 0;
+    LTR_TRY(pass_begin(ctx, p));
     if (run) {
         void *p_rimg = nullptr, *p_win = nullptr;
         ScratchGuard g_rimg(ctx, &p_rimg), g_win(ctx, &p_win);
         // per launch: the approximate running minimum (fast path), and without a kept set the scan image and the test image
-        const int64_t per_kf = (use_fast ? npx : 0) + (set ? 0 : npx + (need_timg ? timg_px : 0));
+        const int64_t per_kf = (p.use_fast ? npx : 0) + (set ? 0 : npx + (need_timg ? timg_px : 0));
         if (per_kf > 0) LTR_TRY(dev_alloc(ctx, &p_rimg, (size_t)B * per_kf * sizeof(uint32_t)));
         LTR_TRY(dev_alloc(ctx, &p_win, (size_t)B * npx * sizeof(uint64_t)));
-        uint32_t* amin = use_fast ? (uint32_t*)p_rimg : nullptr;   // approximate running minimum (fast path only)
-        uint32_t* l_rimg = set ? nullptr : (uint32_t*)p_rimg + (use_fast ? (size_t)B * npx : 0);
+        uint32_t* amin = p.use_fast ? (uint32_t*)p_rimg : nullptr;   // approximate running minimum (fast path only)
+        uint32_t* l_rimg = set ? nullptr : (uint32_t*)p_rimg + (p.use_fast ? (size_t)B * npx : 0);
         uint32_t* l_timg = (set || !need_timg) ? nullptr : l_rimg + (size_t)B * npx;   // test image (padded, or pixels without a return can never flag)
         uint64_t* win = (uint64_t*)p_win;
-        const int fill_blocks = ctx->sm_count * 8;
-        fill_u64_kernel<<<grid_for(B * npx, 256, fill_blocks), 256, 0, ctx->stream>>>(win, cand ? kWinNone : kWinEmpty, B * npx);
+        fill_u64_kernel<<<grid_for(B * npx, 256, ctx->sm_count * 8), 256, 0, ctx->stream>>>(win, cand ? kWinNone : kWinEmpty, B * npx);
         LTR_LAUNCH_CHECK(ctx);
+        const Proj proj = cand ? Proj::kScanMinusMap : use_deferred ? Proj::kTrueMinDeferred : Proj::kTrueMin;
         for (int k0 = kf_begin; k0 < kf_end; k0 += B) {
             const int nb = std::min(B, kf_end - k0);
-            if (use_fast) {
-                fill_u32_kernel<<<grid_for(nb * npx, 256, fill_blocks), 256, 0, ctx->stream>>>(amin, 0x7f800000u, nb * npx);
-                LTR_LAUNCH_CHECK(ctx);
-            }
             const uint32_t *rimg, *test_img;
             if (set) {
                 const size_t j = (size_t)(k0 - kf_begin);
@@ -670,27 +707,12 @@ static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, 
                 test_img = need_timg ? set->timg + j * timg_px : rimg;
                 if (use_cull) ca.pyr = set->pyr + j * ca.pyr_stride;
             } else {
-                LTR_TRY(build_scan_images(ctx, *scans, k0, nb, g, fc, use_fast, shortcut, true, l_rimg, use_cull ? (float*)p_pyr : nullptr, l_timg, pad));
+                LTR_TRY(build_scan_images(ctx, p, *scans, k0, nb, true, l_rimg, use_cull ? (float*)p_pyr : nullptr, l_timg, pad));
                 rimg = l_rimg;
                 test_img = need_timg ? l_timg : l_rimg;
                 if (use_cull) ca.pyr = (const float*)p_pyr;
             }
-            prof_begin(ctx);
-            launch_units.push_back(nb);
-            if (use_fast) {
-                if (cand) launch_fast<true>(ctx, *map, *poses, k0, nb, g, fc, rimg, test_img, diff_thres, win, amin, ca);
-                else if (use_deferred) launch_fast<false, true>(ctx, *map, *poses, k0, nb, g, fc, rimg, amin, diff_thres, win, amin, ca, da);
-                else launch_fast<false>(ctx, *map, *poses, k0, nb, g, fc, rimg, amin, diff_thres, win, amin, ca);
-            } else {
-                const unsigned mb = (unsigned)((map->n + 255) / 256);
-                const size_t smem = (size_t)nb * 12 * sizeof(double);
-                if (cand) map_project_kernel<true><<<mb, 256, smem, ctx->stream>>>(view(*map), poses->d, k0, nb, ctx->d_ext, ctx->ext_identity ? 1 : 0,
-                                                                                 ctx->cfg.transform_order, g, rimg, diff_thres, win);
-                else map_project_kernel<false><<<mb, 256, smem, ctx->stream>>>(view(*map), poses->d, k0, nb, ctx->d_ext, ctx->ext_identity ? 1 : 0,
-                                                                              ctx->cfg.transform_order, g, rimg, diff_thres, win);
-            }
-            prof_end(ctx);
-            LTR_LAUNCH_CHECK(ctx);
+            LTR_TRY(project_map(ctx, p, *map, *poses, k0, nb, proj, rimg, test_img, diff_thres, win, amin, ca, da));
             const unsigned rb = (unsigned)((nb * npx + 255) / 256);
             if (cand) resolve_kernel<true><<<rb, 256, 0, ctx->stream>>>(rimg, win, nb * npx, diff_thres, map->flags);
             else resolve_kernel<false><<<rb, 256, 0, ctx->stream>>>(rimg, win, nb * npx, diff_thres, map->flags);
@@ -706,31 +728,23 @@ static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, 
     LTR_CUDA(ctx, cudaEventSynchronize(ctx->ev1));
     if (da.overflow) { LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); *overflowed = h_over != 0; }
     g_def.release();
-    float ms = 0.0f;
-    cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
-    prof_collect(ctx, 0, 12.0 * (double)map->n + (double)map->n / 8.0, (double)map->n, launch_units);
-    ctx->stats[0] = (double)map->n * (kf_end - kf_begin);
-    ctx->stats[1] = 0; ctx->stats[2] = ctx->stats[0]; ctx->stats[3] = 0;
-    ctx->stats_counters_pending = use_fast;   // device counters are fetched lazily by ltr_last_pass_stats
-    ctx->stats[4] = (double)ms * 1000.0;
+    pass_end(ctx, p, 0, 12.0 * (double)map->n + (double)map->n / 8.0, map->n, kf_end - kf_begin);
     return LTR_OK;
 }
 
-static int parse_projected_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end, float res_alpha, ltr_scanset* out,
-                                bool allow_deferred, bool* overflowed);
-
-int ltr_parse_projected(ltr_ctx* ctx, ltr_cloud map_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end, float res_alpha, ltr_scanset* out) {
-    ApiTrace tr__(ctx, "ltr_parse_projected");
-    if (!ctx || !out) return fail(ctx, LTR_ERR_INVALID, "null argument");
-    bool overflowed = false;
-    LTR_TRY(parse_projected_impl(ctx, map_h, poses_h, kf_begin, kf_end, res_alpha, out, true, &overflowed));
-    if (overflowed) {   // the deferred mode's candidate list filled up (8 M entries; never seen): repeat with the immediate mode
-        LTR_TRY(ltr_scanset_free(ctx, *out));
-        LTR_TRY(parse_projected_impl(ctx, map_h, poses_h, kf_begin, kf_end, res_alpha, out, false, &overflowed));
-    }
-    return LTR_OK;
+int ltr_remove_pass(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end,
+                    int32_t mode, float res_alpha, float diff_thres, int32_t accumulate, int64_t* n_dynamic) {
+    ApiTrace tr__(ctx, "ltr_remove_pass");
+    if (!ctx) return LTR_ERR_INVALID;
+    // ND (true per-pixel minimum) runs in the deferred mode of project_fast.cuh unless the flags accumulate into earlier ones (a run whose
+    // overflow list filled up would have to be undone)
+    return with_deferred_retry([&](bool allow_deferred, bool* overflowed) {
+        return remove_pass_impl(ctx, map_h, scans_h, poses_h, kf_begin, kf_end, mode, res_alpha, diff_thres, accumulate, n_dynamic,
+                                allow_deferred && !accumulate, overflowed);
+    });
 }
 
+// An overflowed run (*overflowed) frees its output again.
 static int parse_projected_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end, float res_alpha, ltr_scanset* out,
                                 bool allow_deferred, bool* overflowed) {
     *overflowed = false;
@@ -738,34 +752,26 @@ static int parse_projected_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_poses poses_h
     DevPoses* poses;
     LTR_TRY(cloud_get(ctx, map_h, &map));
     LTR_TRY(poses_get(ctx, poses_h, &poses));
-    if (kf_begin < 0 || kf_end > poses->K || kf_begin > kf_end) return fail(ctx, LTR_ERR_INVALID, "keyframe range [%d,%d) outside [0,%d)", kf_begin, kf_end, poses->K);
-    if (map->n >= ((int64_t)1 << 32)) return fail(ctx, LTR_ERR_UNSUPPORTED, "map larger than 2^32 points");
-    int32_t rows, cols;
-    ltr_reset_rimg_size(ctx->cfg.vfov_deg, ctx->cfg.hfov_deg, res_alpha, &rows, &cols);
-    if (rows < 1 || cols < 1) return fail(ctx, LTR_ERR_INVALID, "range image %dx%d is empty", rows, cols);
-    const ImgShape g{rows, cols, ctx->cfg.vfov_deg, ctx->cfg.hfov_deg};
-    const int64_t npx = (int64_t)rows * cols;
+    LTR_TRY(check_pass_range(ctx, *map, kf_begin, kf_end, poses->K));
     const int K = kf_end - kf_begin;
+    PassPlan p;
+    LTR_TRY(plan_pass(ctx, res_alpha, K, &p));
+    const int64_t npx = p.npx;
     const DevCloud mapc = *map;
     const DevPoses posc = *poses;
     std::vector<int64_t> off((size_t)K + 1, 0);
-    const FastCfg fc = make_fast_cfg(rows, cols, ctx->cfg.vfov_deg, ctx->cfg.hfov_deg, 0);
-    const bool use_fast = ctx->cfg.fast_path && npx <= (1 << 18);
-    if (use_fast) LTR_CUDA(ctx, cudaMemsetAsync(ctx->d_counters, 0, 4 * sizeof(unsigned long long), ctx->stream));
-    LTR_CUDA(ctx, cudaEventRecord(ctx->ev0, ctx->stream));
+    LTR_TRY(pass_begin(ctx, p));
     void *p_list = nullptr, *p_cnt = nullptr, *p_def = nullptr;
     ScratchGuard g_list(ctx, &p_list), g_cnt(ctx, &p_cnt), g_def(ctx, &p_def);
-    DeferredArgs da{nullptr, nullptr, nullptr, nullptr, 0};
-    const bool use_deferred = use_fast && allow_deferred;
-    std::vector<int> launch_units;
-    ctx->ev_used = 0;
+    DeferredArgs da{};
+    const bool use_deferred = p.use_fast && allow_deferred;
     if (K > 0 && mapc.n > 0) {
-        const int B = std::max(1, std::min(std::min(ctx->cfg.keyframe_batch, use_fast ? kFastMaxBatch : 400), K));
+        const int B = p.B;
         if (use_deferred) LTR_TRY(deferred_alloc(ctx, B, npx, &p_def, &da));
         void *p_win = nullptr, *p_amin = nullptr, *p_tiles = nullptr, *p_keys = nullptr;
         ScratchGuard g_win(ctx, &p_win), g_amin(ctx, &p_amin), g_tiles(ctx, &p_tiles), g_keys(ctx, &p_keys);
         LTR_TRY(dev_alloc(ctx, &p_win, (size_t)B * npx * sizeof(uint64_t)));
-        if (use_fast && !use_deferred) LTR_TRY(dev_alloc(ctx, &p_amin, (size_t)B * npx * sizeof(uint32_t)));   // the deferred mode keeps `best` instead
+        if (p.use_fast && !use_deferred) LTR_TRY(dev_alloc(ctx, &p_amin, (size_t)B * npx * sizeof(uint32_t)));   // the deferred mode keeps `best` instead
         uint32_t* amin = (uint32_t*)p_amin;
         // deferred mode: the tiles are claimed near to far from each launch's keyframes (DeferredArgs::order); their bounding spheres
         // are computed once per call
@@ -790,33 +796,20 @@ static int parse_projected_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_poses poses_h
         LTR_LAUNCH_CHECK(ctx);
         for (int k0 = 0; k0 < K; k0 += B) {
             const int nb = std::min(B, K - k0);
-            prof_begin(ctx);
-            launch_units.push_back(nb);
-            if (use_deferred) {
-                if (use_order) {
-                    // reference origin of the launch: the mean sensor origin of its keyframes (KfFast::chi)
-                    double o[3] = {0.0, 0.0, 0.0};
-                    for (int k = 0; k < nb; ++k)
-                        for (int d = 0; d < 3; ++d) o[d] += (double)posc.h_fast[(size_t)(kf_begin + k0 + k) * 16 + 9 + d] / nb;
-                    tile_order_key_kernel<<<(unsigned)((ntiles + 255) / 256), 256, 0, ctx->stream>>>((const float4*)p_tiles, ntiles, (float)o[0], (float)o[1],
-                                                                                                      (float)o[2], keys);
-                    LTR_LAUNCH_CHECK(ctx);
-                    uint64_t* sorted = nullptr;
-                    LTR_TRY(radix_sort_pairs(ctx, keys, keys + ntiles, nullptr, nullptr, ntiles, 32, 48, &sorted, nullptr));
-                    da.order = (const unsigned long long*)sorted;
-                }
-                launch_fast<false, true>(ctx, mapc, posc, kf_begin + k0, nb, g, fc, nullptr, nullptr, 0.0f, win, nullptr, no_cull, da);
-            } else if (use_fast) {
-                fill_u32_kernel<<<grid_for(nb * npx, 256, ctx->sm_count * 8), 256, 0, ctx->stream>>>(amin, 0x7f800000u, nb * npx);
+            if (use_order) {
+                // reference origin of the launch: the mean sensor origin of its keyframes (KfFast::chi)
+                double o[3] = {0.0, 0.0, 0.0};
+                for (int k = 0; k < nb; ++k)
+                    for (int d = 0; d < 3; ++d) o[d] += (double)posc.h_fast[(size_t)(kf_begin + k0 + k) * 16 + 9 + d] / nb;
+                tile_order_key_kernel<<<(unsigned)((ntiles + 255) / 256), 256, 0, ctx->stream>>>((const float4*)p_tiles, ntiles, (float)o[0], (float)o[1],
+                                                                                                  (float)o[2], keys);
                 LTR_LAUNCH_CHECK(ctx);
-                launch_fast<false>(ctx, mapc, posc, kf_begin + k0, nb, g, fc, nullptr, amin, 0.0f, win, amin, no_cull);
-            } else {
-                const unsigned mb = (unsigned)((mapc.n + 255) / 256);
-                map_project_kernel<false><<<mb, 256, (size_t)nb * 12 * sizeof(double), ctx->stream>>>(view(mapc), posc.d, kf_begin + k0, nb, ctx->d_ext,
-                    ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, g, nullptr, 0.0f, win);
+                uint64_t* sorted = nullptr;
+                LTR_TRY(radix_sort_pairs(ctx, keys, keys + ntiles, nullptr, nullptr, ntiles, 32, 48, &sorted, nullptr));
+                da.order = (const unsigned long long*)sorted;
             }
-            prof_end(ctx);
-            LTR_LAUNCH_CHECK(ctx);
+            LTR_TRY(project_map(ctx, p, mapc, posc, kf_begin + k0, nb, use_deferred ? Proj::kTrueMinDeferred : Proj::kTrueMin, nullptr, nullptr, 0.0f,
+                                win, amin, no_cull, da));
             parse_count_kernel<<<dim3((unsigned)nchunk, (unsigned)nb), 1024, 0, ctx->stream>>>(win, (int)npx, nchunk, chunk_cnt);
             LTR_LAUNCH_CHECK(ctx);
             parse_compact_kernel<<<dim3((unsigned)nchunk, (unsigned)nb), 1024, 0, ctx->stream>>>(win, (int)npx, nchunk, chunk_cnt, (uint32_t*)p_list + (size_t)k0 * npx,
@@ -847,14 +840,17 @@ static int parse_projected_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_poses poses_h
     g_cnt.release();
     LTR_CUDA(ctx, cudaEventRecord(ctx->ev1, ctx->stream));
     LTR_CUDA(ctx, cudaEventSynchronize(ctx->ev1));
-    float ms = 0.0f;
-    cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
-    prof_collect(ctx, 4, 12.0 * (double)mapc.n, (double)mapc.n, launch_units);
-    ctx->stats[0] = (double)mapc.n * K;
-    ctx->stats[1] = 0; ctx->stats[2] = ctx->stats[0]; ctx->stats[3] = 0;
-    ctx->stats_counters_pending = use_fast;
-    ctx->stats[4] = (double)ms * 1000.0;
+    pass_end(ctx, p, 4, 12.0 * (double)mapc.n, mapc.n, K);
+    if (*overflowed) return ltr_scanset_free(ctx, *out);
     return LTR_OK;
+}
+
+int ltr_parse_projected(ltr_ctx* ctx, ltr_cloud map_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end, float res_alpha, ltr_scanset* out) {
+    ApiTrace tr__(ctx, "ltr_parse_projected");
+    if (!ctx || !out) return fail(ctx, LTR_ERR_INVALID, "null argument");
+    return with_deferred_retry([&](bool allow_deferred, bool* overflowed) {
+        return parse_projected_impl(ctx, map_h, poses_h, kf_begin, kf_end, res_alpha, out, allow_deferred, overflowed);
+    });
 }
 
 int ltr_debug_pixel_index(ltr_ctx* ctx, const float* xyz, int64_t n, int32_t rows, int32_t cols, int32_t* row, int32_t* col, float* range,
@@ -887,9 +883,9 @@ int ltr_debug_pixel_index(ltr_ctx* ctx, const float* xyz, int64_t n, int32_t row
 
 int ltr_debug_margins(ltr_ctx* ctx, float res_alpha, float* m) {
     if (!ctx || !m) return fail(ctx, LTR_ERR_INVALID, "bad argument");
-    int32_t rows, cols;
-    ltr_reset_rimg_size(ctx->cfg.vfov_deg, ctx->cfg.hfov_deg, res_alpha, &rows, &cols);
-    const FastCfg fc = make_fast_cfg(rows, cols, ctx->cfg.vfov_deg, ctx->cfg.hfov_deg, 0);
+    PassPlan plan;
+    LTR_TRY(plan_pass(ctx, res_alpha, 1, &plan));
+    const FastCfg& fc = plan.fc;
     m[0] = fc.m_col_a; m[1] = fc.m_col_b; m[2] = fc.m_row; m[3] = fc.m_r_rel; m[4] = fc.m_r_abs; m[5] = (float)fc.el_direct;
     m[6] = (float)((fc.m_col_a + fc.m_col_b) / kMarginSafety); m[7] = (float)(fc.m_row / kMarginSafety);
     m[8] = fc.az_seam_lim;
@@ -920,27 +916,13 @@ int ltr_debug_scan_rimg(ltr_ctx* ctx, ltr_scanset scans_h, int32_t kf, float res
     DevScanSet* scans;
     LTR_TRY(scanset_get(ctx, scans_h, &scans));
     if (kf < 0 || kf >= scans->K) return fail(ctx, LTR_ERR_INVALID, "keyframe %d outside [0,%d)", kf, scans->K);
-    int32_t rows, cols;
-    ltr_reset_rimg_size(ctx->cfg.vfov_deg, ctx->cfg.hfov_deg, res_alpha, &rows, &cols);
-    if (rows < 1 || cols < 1) return fail(ctx, LTR_ERR_INVALID, "range image %dx%d is empty", rows, cols);
-    const ImgShape g{rows, cols, ctx->cfg.vfov_deg, ctx->cfg.hfov_deg};
-    const int64_t npx = (int64_t)rows * cols;
+    PassPlan plan;
+    LTR_TRY(plan_pass(ctx, res_alpha, 1, &plan));
     void* p = nullptr;
     ScratchGuard g_p(ctx, &p);
-    LTR_TRY(dev_alloc(ctx, &p, (size_t)npx * sizeof(uint32_t)));
-    fill_u32_kernel<<<grid_for(npx, 256, ctx->sm_count * 8), 256, 0, ctx->stream>>>((uint32_t*)p, kNoPointBits, npx);
-    LTR_LAUNCH_CHECK(ctx);
-    const int64_t npts = scans->h_off[kf + 1] - scans->h_off[kf];
-    if (npts > 0) {
-        const FastCfg fcd = make_fast_cfg(rows, cols, ctx->cfg.vfov_deg, ctx->cfg.hfov_deg, 0);
-        if (ctx->cfg.fast_path && npx <= (1 << 18) && fcd.el_direct)
-            scan_rimg_fast_kernel<true><<<(unsigned)((npts + 255) / 256), 256, 0, ctx->stream>>>(view(scans->pts), scans->d_off, kf, 1, g, fcd, (uint32_t*)p);
-        else if (ctx->cfg.fast_path && npx <= (1 << 18))
-            scan_rimg_fast_kernel<false><<<(unsigned)((npts + 255) / 256), 256, 0, ctx->stream>>>(view(scans->pts), scans->d_off, kf, 1, g, fcd, (uint32_t*)p);
-        else scan_rimg_kernel<<<(unsigned)((npts + 255) / 256), 256, 0, ctx->stream>>>(view(scans->pts), scans->d_off, kf, 1, g, (uint32_t*)p);
-        LTR_LAUNCH_CHECK(ctx);
-    }
-    LTR_CUDA(ctx, cudaMemcpyAsync(out, p, (size_t)npx * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    LTR_TRY(dev_alloc(ctx, &p, (size_t)plan.npx * sizeof(uint32_t)));
+    LTR_TRY(scan_rimg(ctx, plan, *scans, kf, 1, (uint32_t*)p));
+    LTR_CUDA(ctx, cudaMemcpyAsync(out, p, (size_t)plan.npx * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
     LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return LTR_OK;
 }
@@ -948,10 +930,9 @@ int ltr_debug_scan_rimg(ltr_ctx* ctx, ltr_scanset scans_h, int32_t kf, float res
 int ltr_debug_fast_project(ltr_ctx* ctx, const float* xyz, int64_t n, const double* inv_pose16, float res_alpha, float* out8, float* margins4) {
     ApiTrace tr__(ctx, "ltr_debug_fast_project");
     if (!ctx || !xyz || !inv_pose16 || !out8 || n < 0) return fail(ctx, LTR_ERR_INVALID, "bad argument");
-    int32_t rows, cols;
-    ltr_reset_rimg_size(ctx->cfg.vfov_deg, ctx->cfg.hfov_deg, res_alpha, &rows, &cols);
-    const ImgShape g{rows, cols, ctx->cfg.vfov_deg, ctx->cfg.hfov_deg};
-    const FastCfg fc = make_fast_cfg(rows, cols, ctx->cfg.vfov_deg, ctx->cfg.hfov_deg, 0);
+    PassPlan plan;
+    LTR_TRY(plan_pass(ctx, res_alpha, 1, &plan));
+    const FastCfg& fc = plan.fc;
     if (margins4) { margins4[0] = fc.m_col_a; margins4[1] = fc.m_col_b; margins4[2] = fc.m_row; margins4[3] = fc.m_r_rel; }
     if (n == 0) return LTR_OK;
     ltr_poses ph;
@@ -965,10 +946,9 @@ int ltr_debug_fast_project(ltr_ctx* ctx, const float* xyz, int64_t n, const doub
     float* d_xyz = (float*)p;
     float* d_out = d_xyz + 3 * n;
     LTR_CUDA(ctx, cudaMemcpyAsync(d_xyz, xyz, (size_t)n * 12, cudaMemcpyHostToDevice, ctx->stream));
-    if (fc.el_direct) debug_fast_kernel<true><<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(d_xyz, n, pp.d_fast, pp.d, ctx->d_ext, ctx->ext_identity ? 1 : 0,
-                                                                        ctx->cfg.transform_order, g, fc, d_out);
-    else debug_fast_kernel<false><<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(d_xyz, n, pp.d_fast, pp.d, ctx->d_ext, ctx->ext_identity ? 1 : 0,
-                                                                        ctx->cfg.transform_order, g, fc, d_out);
+    const auto kern = with_el_direct(fc, [](auto el) { return debug_fast_kernel<decltype(el)::value>; });
+    kern<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(d_xyz, n, pp.d_fast, pp.d, ctx->d_ext, ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order,
+                                                               plan.g, fc, d_out);
     LTR_LAUNCH_CHECK(ctx);
     LTR_CUDA(ctx, cudaMemcpyAsync(out8, d_out, (size_t)n * 32, cudaMemcpyDeviceToHost, ctx->stream));
     LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));

@@ -204,6 +204,35 @@ constexpr uint32_t kNoPointBitsF = 0x461C4000u;  // 10000.0f
 // queue entry: [63:32] map index | [31:14] pixel (row * cols + col, < 2^18) | [13:0] keyframe within the batch
 LTR_DEV uint64_t q_pack(uint32_t i, uint32_t px, uint32_t k) { return ((uint64_t)i << 32) | (px << 14) | k; }
 
+// Offers the exact key (range r, map index i) to pixel px of the winner image.  kCandidatesOnly: only a candidate (scan - r > thres) enters,
+// and with the empty-scan shortcut a pixel without a scan return turns every pair away (diff > 200 for every map point there).  A key that
+// is not below the pixel's current one skips the atomic.
+template <bool kCandidatesOnly>
+LTR_DEV void offer(uint64_t* __restrict__ win, size_t px, float r, uint32_t i, const uint32_t* __restrict__ scan_rimg, float thres, int shortcut,
+                   unsigned* n_atomics) {
+    const uint64_t packed = ((uint64_t)__float_as_uint(r) << 32) | i;
+    if (kCandidatesOnly) {
+        const uint32_t sb = scan_rimg[px];
+        if (shortcut && sb == kNoPointBitsF && r < 9000.0f) return;
+        if (!(fs(__uint_as_float(sb), r) > thres)) return;
+    }
+    if (packed < win[px]) { atomicMin((unsigned long long*)&win[px], (unsigned long long)packed); ++*n_atomics; }
+}
+
+// The reference arithmetic of one pair: map point i at (x, y, z) projected into keyframe k of the launch (inv_pose: its inverse pose) and
+// offered at its pixel.
+template <bool kCandidatesOnly>
+LTR_DEV void exact_pair(float x, float y, float z, uint32_t i, uint32_t k, const double* __restrict__ inv_pose, const double* __restrict__ ext,
+                        int ext_identity, int order, const ImgShape& g, const uint32_t* __restrict__ scan_rimg, float thres,
+                        uint64_t* __restrict__ win, int shortcut, unsigned* n_atomics) {
+    float lx, ly, lz;
+    map_to_sensor(inv_pose, ext, ext_identity, order, x, y, z, &lx, &ly, &lz);
+    const Sph s = cart2sph(lx, ly, lz);
+    int r, c;
+    pixel_index(s, g, &r, &c);
+    offer<kCandidatesOnly>(win, (size_t)k * g.rows * g.cols + (size_t)r * g.cols + c, s.r, i, scan_rimg, thres, shortcut, n_atomics);
+}
+
 // Kind A: pixel index known to be right, only the exact range is needed (double transform + sqrt): ~60 instructions.
 template <bool kCandidatesOnly>
 LTR_DEV void exact_range_pair(const PtrView& map, uint64_t e, const double* __restrict__ poses, int kf0, const double* __restrict__ ext,
@@ -211,43 +240,21 @@ LTR_DEV void exact_range_pair(const PtrView& map, uint64_t e, const double* __re
                               uint64_t* __restrict__ win, int shortcut, unsigned* n_atomics) {
     const uint32_t i = (uint32_t)(e >> 32), pxl = ((uint32_t)e >> 14) & 0x3ffffu, k = (uint32_t)e & 0x3fffu;
     float lx, ly, lz;
-    transform_point(poses + (size_t)(kf0 + k) * 24, order, map.x[i], map.y[i], map.z[i], &lx, &ly, &lz);
-    if (!ext_identity) transform_point(ext, order, lx, ly, lz, &lx, &ly, &lz);
+    map_to_sensor(poses + (size_t)(kf0 + k) * 24, ext, ext_identity, order, map.x[i], map.y[i], map.z[i], &lx, &ly, &lz);
     const float r = __fsqrt_rn(fa(fa(fm(lx, lx), fm(ly, ly)), fm(lz, lz)));   // == cart2sph().r
-    const size_t px = (size_t)k * npx + pxl;
-    const uint64_t packed = ((uint64_t)__float_as_uint(r) << 32) | i;
-    if (kCandidatesOnly) {
-        const uint32_t sb = scan_rimg[px];
-        if (shortcut && sb == kNoPointBitsF && r < 9000.0f) return;
-        if (fs(__uint_as_float(sb), r) > thres && packed < win[px]) { atomicMin((unsigned long long*)&win[px], (unsigned long long)packed); ++*n_atomics; }
-    } else {
-        if (packed < win[px]) { atomicMin((unsigned long long*)&win[px], (unsigned long long)packed); ++*n_atomics; }
-    }
+    offer<kCandidatesOnly>(win, (size_t)k * npx + pxl, r, i, scan_rimg, thres, shortcut, n_atomics);
 }
 
-// Kind B: nothing is known (pixel near a rounding boundary, degenerate geometry, keyframe without fast constants):
-// the full reference arithmetic, identical to map_project_kernel's body.
+// Kind B: nothing is known (pixel near a rounding boundary, degenerate geometry, keyframe without fast constants): the full reference
+// arithmetic, as in map_project_kernel.
 template <bool kCandidatesOnly>
 __device__ __noinline__ void exact_full_pair(const PtrView& map, uint64_t e, const double* __restrict__ poses, int kf0,
                                              const double* __restrict__ ext, int ext_identity, int order, const ImgShape& g,
                                              const uint32_t* __restrict__ scan_rimg, float thres, uint64_t* __restrict__ win, int shortcut,
                                              unsigned* n_atomics) {
     const uint32_t i = (uint32_t)(e >> 32), k = (uint32_t)e & 0x3fffu;
-    float lx, ly, lz;
-    transform_point(poses + (size_t)(kf0 + k) * 24, order, map.x[i], map.y[i], map.z[i], &lx, &ly, &lz);
-    if (!ext_identity) transform_point(ext, order, lx, ly, lz, &lx, &ly, &lz);
-    const Sph s = cart2sph(lx, ly, lz);
-    int r, c;
-    pixel_index(s, g, &r, &c);
-    const size_t px = (size_t)k * g.rows * g.cols + (size_t)r * g.cols + c;
-    const uint64_t packed = ((uint64_t)__float_as_uint(s.r) << 32) | i;
-    if (kCandidatesOnly) {
-        const uint32_t sb = scan_rimg[px];
-        if (shortcut && sb == kNoPointBitsF && s.r < 9000.0f) return;  // empty scan pixel: diff > 200 for every map point there
-        if (fs(__uint_as_float(sb), s.r) > thres && packed < win[px]) { atomicMin((unsigned long long*)&win[px], (unsigned long long)packed); ++*n_atomics; }
-    } else {
-        if (packed < win[px]) { atomicMin((unsigned long long*)&win[px], (unsigned long long)packed); ++*n_atomics; }
-    }
+    exact_pair<kCandidatesOnly>(map.x[i], map.y[i], map.z[i], i, k, poses + (size_t)(kf0 + k) * 24, ext, ext_identity, order, g, scan_rimg, thres,
+                                win, shortcut, n_atomics);
 }
 
 }  // namespace ltr
@@ -344,6 +351,10 @@ __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFast
     if ((long long)tile_u >= total_tiles) break;
     const long long tile = (kDeferred && da.order) ? (long long)(uint32_t)da.order[tile_u] : (long long)tile_u;
     const int64_t base = (int64_t)tile * (32 * kFastPts) + lane;
+    // map index of the lane's point j, and the push of its pair with keyframe k onto the full exact queue.  Recomputed at each use: caching
+    // the indices across the keyframe loop would cost the padded variant its 64-register bound.
+    const auto point_index = [&](int j) { return (uint32_t)(base + j * 32 < map.n ? base + j * 32 : map.n - 1); };
+    const auto push_full = [&](int j, int k) { s_qb[atomicAdd(&s_cnt[warp][1], 1)] = q_pack(point_index(j), 0u, (uint32_t)k); };
     float px_[kFastPts], py_[kFastPts], pz_[kFastPts];
 #pragma unroll
     for (int j = 0; j < kFastPts; ++j) {
@@ -365,8 +376,7 @@ __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFast
         const float* __restrict__ kf = kb.kf[k];
         if (kf[15] == 0.0f) {                         // warp-uniform: no fast constants (non-rigid pose or extrinsic) -> all pairs exact
 #pragma unroll
-            for (int j = 0; j < kFastPts; ++j)
-                s_qb[atomicAdd(&s_cnt[warp][1], 1)] = q_pack((uint32_t)(base + j * 32 < map.n ? base + j * 32 : map.n - 1), 0u, (uint32_t)k);
+            for (int j = 0; j < kFastPts; ++j) push_full(j, k);
         } else {
         // this keyframe's images (kPad: the padded test image)
         const uint32_t* __restrict__ test_k = kDeferred ? nullptr : kPad ? opaque_ptr(test_img + (uint32_t)(k * fc.pad_npx)) : test_img + (size_t)k * npx;
@@ -430,8 +440,7 @@ __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFast
                 lead_[j] = enter_[j] && !(fr >= tv);             // looks like a new best
                 old_[j] = 0ull; rwin_[j] = tv;
                 if (lead_[j]) {
-                    const uint32_t mi = (uint32_t)(base + j * 32 < map.n ? base + j * 32 : map.n - 1);
-                    old_[j] = atomicMin(&best_k[pxl_[j]], ((unsigned long long)__float_as_uint(fr) << 32) | mi);
+                    old_[j] = atomicMin(&best_k[pxl_[j]], ((unsigned long long)__float_as_uint(fr) << 32) | point_index(j));
                     ++n_atomics;
                 }
             }
@@ -439,8 +448,7 @@ __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFast
             for (int j = 0; j < kFastPts; ++j) {
                 if (enter_[j]) {
                     const float fr = fr_[j];
-                    const uint32_t mi = (uint32_t)(base + j * 32 < map.n ? base + j * 32 : map.n - 1);
-                    const unsigned long long v = ((unsigned long long)__float_as_uint(fr) << 32) | mi;
+                    const unsigned long long v = ((unsigned long long)__float_as_uint(fr) << 32) | point_index(j);
                     // not the group's representative (or not better than what was read): v is a candidate that loses to a pair of range rwin_
                     unsigned long long loser = v;
                     float r_win = rwin_[j];
@@ -454,7 +462,7 @@ __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFast
                         if (slot < da.capacity) da.list[slot] = q_pack((uint32_t)loser, pxl_[j], (uint32_t)k);
                     }
                 } else if (!certain_[j]) {
-                    s_qb[atomicAdd(&s_cnt[warp][1], 1)] = q_pack((uint32_t)(base + j * 32 < map.n ? base + j * 32 : map.n - 1), 0u, (uint32_t)k);
+                    push_full(j, k);
                 }
             }
         } else {
@@ -481,7 +489,7 @@ __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFast
                         pxl = (uint32_t)(min(max((int)rp - fc.pad_g, 0), hi_r) * g.cols + min(col, hi_c));
                     }
                     if (kPad && seam) {
-                        s_qb[atomicAdd(&s_cnt[warp][1], 1)] = q_pack((uint32_t)(base + j * 32 < map.n ? base + j * 32 : map.n - 1), 0u, (uint32_t)k);
+                        push_full(j, k);
                         continue;
                     }
                     bool push = true;
@@ -490,10 +498,10 @@ __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFast
                         push = !(fr > __fadd_rn(cur, __fmaf_rn(fc.mr2_rel, fr, fc.mr2_abs)));
                         if (push && fr < cur) atomicMin(&amin_k[pxl], __float_as_uint(fr));
                     } else if (fr < tv) atomicMin(&amin_k[pxl], __float_as_uint(fr));
-                    if (push) s_qa[atomicAdd(&s_cnt[warp][0], 1)] = q_pack((uint32_t)(base + j * 32 < map.n ? base + j * 32 : map.n - 1), pxl, (uint32_t)k);
+                    if (push) s_qa[atomicAdd(&s_cnt[warp][0], 1)] = q_pack(point_index(j), pxl, (uint32_t)k);
                 }
             } else {
-                s_qb[atomicAdd(&s_cnt[warp][1], 1)] = q_pack((uint32_t)(base + j * 32 < map.n ? base + j * 32 : map.n - 1), 0u, (uint32_t)k);
+                push_full(j, k);
             }
         }
 #ifdef LTR_PROBE_NOMAYBE

@@ -151,6 +151,14 @@ LTR_DEV void transform_point(const double* __restrict__ m, int order, float x, f
     }
 }
 
+// transformGlobalMapToLocal for one map point (utility.cpp:70-71): the keyframe's inverse pose, then the extrinsic unless it is exactly
+// the identity (ext: base2lidar rows 0..2)
+LTR_DEV void map_to_sensor(const double* __restrict__ inv_pose, const double* __restrict__ ext, int ext_identity, int order, float x, float y,
+                           float z, float* lx, float* ly, float* lz) {
+    transform_point(inv_pose, order, x, y, z, lx, ly, lz);
+    if (!ext_identity) transform_point(ext, order, *lx, *ly, *lz, lx, ly, lz);
+}
+
 // FLANN L2_Simple<float> squared distance: ((dx*dx) + dy*dy) + dz*dz with dx = query - point
 LTR_DEV float l2_simple(float qx, float qy, float qz, float px, float py, float pz) {
     const float dx = fs(qx, px), dy = fs(qy, py), dz = fs(qz, pz);
