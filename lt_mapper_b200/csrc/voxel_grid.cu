@@ -19,6 +19,7 @@
 #include <cfloat>
 #include <climits>
 #include <cmath>
+#include <cstdlib>
 
 namespace ltr {
 
@@ -28,6 +29,15 @@ constexpr uint32_t kVgSmall = 1024;          // segments at most this long are s
 constexpr uint32_t kVgThreshold = 16;        // libstdc++ _S_threshold
 constexpr int kVgStack = 128;                // CTA segment stack (LIFO: at most one entry per depth level, depth <= 62)
 constexpr int64_t kVgChunkPoints = (int64_t)64 << 20;   // points per launch: bounds the 24 B/point sort scratch to 1.5 GiB
+
+// Test knob: LTR_VOXEL_GRID_CHUNK_POINTS=n (clamped to [1, kVgChunkPoints]; unset or empty: kVgChunkPoints) takes the place of
+// kVgChunkPoints in voxel_grid_run, so that tests can split small inputs into many launches and check the scratch indexing relative to
+// each launch's first scan.
+static int64_t vg_chunk_points() {
+    int64_t n = kVgChunkPoints;
+    if (const char* e = std::getenv("LTR_VOXEL_GRID_CHUNK_POINTS")) if (*e) n = std::min<int64_t>(std::max<int64_t>(std::atoll(e), 1), kVgChunkPoints);
+    return n;
+}
 
 // x86-64 cvttss2si: NaN and out-of-range values give the "integer indefinite" 0x80000000 (CUDA saturates, and NaN -> 0)
 __device__ __forceinline__ int32_t x86_f2i32(float f) {
@@ -413,7 +423,7 @@ static int voxel_grid_run(ltr_ctx* ctx, const PtrView& src, const std::vector<in
         if (n >= ((int64_t)1 << 31)) return fail(ctx, LTR_ERR_UNSUPPORTED, "voxel grid: scan %d has %lld points (>= 2^31)", k, (long long)n);
         max_chunk = std::max(max_chunk, n);
     }
-    max_chunk = std::max(max_chunk, std::min<int64_t>(off[K], kVgChunkPoints));
+    max_chunk = std::max(max_chunk, std::min<int64_t>(off[K], vg_chunk_points()));
     void *p_ent = nullptr, *p_pos = nullptr, *p_segs = nullptr, *p_cnt = nullptr, *p_status = nullptr, *p_oo = nullptr;
     ScratchGuard g_ent(ctx, &p_ent), g_pos(ctx, &p_pos), g_segs(ctx, &p_segs), g_cnt(ctx, &p_cnt), g_status(ctx, &p_status), g_oo(ctx, &p_oo);
     ltr_cloud sc_h = -1;

@@ -22,6 +22,8 @@ def _free_port():
 
 def _worker(rank, world, port, q):
     sys.path.insert(0, ROOT)
+    # the hooks get host buffers here: with a visible GPU, TorchDistComm would take them for device memory
+    os.environ["CUDA_VISIBLE_DEVICES"] = ""
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
     dist.init_process_group("gloo", rank=rank, world_size=world)
