@@ -5,10 +5,16 @@
 // on the GPU through libltr_removert/libltr_b200, and writes the same output tree (Removerter.cpp:26-50, 231, 1446-1477,
 // 1517-1520, 1600-1601, 1607-1650).  No ROS, no PCL; rviz publishing is dropped (side effect only).
 //
-//   ltremovert_b200 --config params.yaml [--selfremovert] [--pcl110] [--no-split]
+//   ltremovert_b200 --config params.yaml [--selfremovert] [--pcl110] [--no-split] [--clean-scans[=map|scan-minus-map]]
 //     --selfremovert   run selfRemovert over remove_resolution_list (Removerter.cpp:1378-1393) instead of the shipped
 //                      single removeOnce(2.5) (Removerter.cpp:1584, 1587)
 //     --pcl110         PCL >= 1.10 transformPointCloud summation order (ltr_config.transform_order = 1)
+//     --clean-scans    after Step 3, scansideRemovalForEachScan (C,C) and (Q,Q) (Removerter.cpp:1253-1310, commented out in the reference)
+//                      with the "map" criterion (the overload its loop calls, :1306) or "scan-minus-map" (:1071-1123); writes every
+//                      keyframe's static / dynamic part to scan_static/<central|query>/ and scan_dynamic/<central|query>/ under the
+//                      input scan's name (saveCleanedScans, :1143-1195), and with saveMapPCD the merged, 0.05-voxelised maps of
+//                      saveMapPointcloudByMergingCleanedScans (:1197-1251) to map_static/ and map_dynamic/.  Off by default: without it
+//                      the output tree is the one the node writes.
 //
 // Multi-GPU: start one process per GPU with RANK / WORLD_SIZE / LOCAL_RANK in the environment (torchrun, mpirun -x, a shell loop);
 // every rank reads the yaml and the pose files, but loads only the scans of ITS keyframe block (even world: ranks < world/2 take the
@@ -111,12 +117,15 @@ static bool share_nccl_id(int rank, unsigned char id[128]) {
 int main(int argc, char** argv) {
     std::string cfg_path;
     bool selfremovert = false, pcl110 = false, no_split = false;
-    const char* usage = "usage: %s --config params.yaml [--selfremovert] [--pcl110] [--no-split]\n";
+    int clean_scans = -1;   // -1 off, else ltr_scanside_criterion
+    const char* usage = "usage: %s --config params.yaml [--selfremovert] [--pcl110] [--no-split] [--clean-scans[=map|scan-minus-map]]\n";
     for (int i = 1; i < argc; ++i) {
         if (!std::strcmp(argv[i], "--config") && i + 1 < argc) cfg_path = argv[++i];
         else if (!std::strcmp(argv[i], "--selfremovert")) selfremovert = true;
         else if (!std::strcmp(argv[i], "--pcl110")) pcl110 = true;
         else if (!std::strcmp(argv[i], "--no-split")) no_split = true;
+        else if (!std::strcmp(argv[i], "--clean-scans") || !std::strcmp(argv[i], "--clean-scans=map")) clean_scans = LTR_SCANSIDE_MAP;
+        else if (!std::strcmp(argv[i], "--clean-scans=scan-minus-map")) clean_scans = LTR_SCANSIDE_SCAN_MINUS_MAP;
         else { std::fprintf(stderr, usage, argv[0]); return 2; }
     }
     if (cfg_path.empty()) { std::fprintf(stderr, usage, argv[0]); return 2; }
@@ -229,6 +238,33 @@ int main(int argc, char** argv) {
         ok &= save_scans(R, S.keyframe_scans_pd_, C.keyframe_names, d_pd, false);
         ok &= save_scans(R, S.keyframe_scans_strong_pd_, C.keyframe_names, d_pd_strong, false);
         ok &= save_scans(R, S.keyframe_scans_strong_nd_, C.keyframe_names, d_nd_strong, false);
+    }
+    if (clean_scans >= 0) {
+        for (int sess = 0; sess < 2; ++sess) {
+            Session& X = sess == 0 ? R.central_sess_ : R.query_sess_;
+            const LoadedSession& L = sess == 0 ? C : Q;
+            const std::string name = sess == 0 ? "central" : "query";
+            ck(R.scansideRemovalForEachScan(X, X, clean_scans), "scansideRemovalForEachScan");   // (C,C), (Q,Q)
+            if (R.owns(X)) {
+                const std::string ds = save_dir + "scan_static/" + name, dd = save_dir + "scan_dynamic/" + name;
+                fsmkdir(ds);
+                fsmkdir(dd);
+                ok &= save_scans(R, X.scans_static_, L.keyframe_names, ds, false);
+                ok &= save_scans(R, X.scans_dynamic_, L.keyframe_names, dd, false);
+            }
+            if (save_map_pcd && R.owns(X)) {   // saveMapPointcloudByMergingCleanedScans: collective over the ranks holding the session
+                const std::string tag = sess == 0 ? "Central" : "Query";
+                ltr_cloud ms = -1, md = -1;
+                ck(R.mergeAndDownsample(X, X.scans_static_, 0.05f, &ms), "merge static scans");
+                ck(R.mergeAndDownsample(X, X.scans_dynamic_, 0.05f, &md), "merge dynamic scans");
+                if (group_leader) {
+                    ok &= save_cloud(R, ms, save_dir + "map_static/" + tag + "StaticScansMergedMapGlobal.pcd", true);
+                    ok &= save_cloud(R, md, save_dir + "map_dynamic/" + tag + "DynamicScansMergedMapGlobal.pcd", true);
+                }
+                ltr_cloud_free(R.ctx, ms);
+                ltr_cloud_free(R.ctx, md);
+            }
+        }
     }
     if (world > 1 && R.nccl_world >= 0) ltr_nccl_barrier(R.ctx, R.nccl_world);   // nobody leaves before everybody's files are written
     if (rank == 0) std::printf(" outputs written to %s (%s)\n", save_dir.c_str(), ok ? "ok" : "WITH ERRORS");

@@ -183,6 +183,29 @@ int ltr_knn_diff(ltr_ctx* ctx, ltr_scanset scans, ltr_poses poses, int32_t pose_
  * With any query point, a target of k or more points with a non-finite coordinate fails with LTR_ERR_UNSUPPORTED. */
 int ltr_knn_split_cloud(ltr_ctx* ctx, ltr_cloud query, ltr_cloud target, int32_t k, float thr, ltr_cloud* out_near, ltr_cloud* out_far);
 
+/* criteria of ltr_scanside_split */
+typedef enum ltr_scanside_criterion {
+    LTR_SCANSIDE_MAP = 0,             /* static iff |avg_map| < thr                         (Removerter.cpp:1049-1060) */
+    LTR_SCANSIDE_SCAN_MINUS_MAP = 1   /* static iff fabsf(avg_scan - avg_map) < thr, in f32 (Removerter.cpp:1094-1114) */
+} ltr_scanside_criterion;
+
+/* Scan-side removal, Removerter::removeDynamicPointsOfScanByKnn (Removerter.cpp:1019-1069, 1071-1123) as
+ * scansideRemovalForEachScan (Removerter.cpp:1253-1310) calls it for every keyframe k of `scans` (poses index pose_offset + k):
+ * scan_global = local2global(scan_k, pose, lidar2base), the live 3-argument utility.cpp:160-168 (two steps, f32 rounding after
+ * each, as ltr_merge_scans_global); every point, in input order, gets
+ *   avg_map  = (float)(sum_double of its k smallest SQUARED distances to `map`) / float(k)
+ *   avg_scan = the same over scan_global itself (the point is its own first neighbour; duplicates count)
+ * with FLANN's L2_Simple distances ((dx*dx + dy*dy) + dz*dz in f32) summed in ascending order; a target of n < k points contributes
+ * all n and is still divided by k.  Static and dynamic points keep their input order and are moved back with
+ * global2local(..., inv_pose, base2lidar) (utility.cpp:194-202).  Either output may be NULL.
+ * 1 <= k <= 16, thr > 0.  An empty map, or a non-finite coordinate in the map or in any scan, fails with LTR_ERR_UNSUPPORTED.
+ * Keyframes are processed in launches of at most LTR_SCANSIDE_CHUNK_POINTS points (environment; default 2^24, one keyframe at least). */
+int ltr_scanside_split(ltr_ctx* ctx, ltr_scanset scans, ltr_poses poses, int32_t pose_offset, ltr_cloud map, int32_t criterion,
+                       int32_t k, float thr, ltr_scanset* out_static, ltr_scanset* out_dynamic);
+/* Counters of the last ltr_scanside_split: [0] points, [1] map searches and [2] own-scan searches that the bounded pass on the finest
+ * grid did not settle (they went on to the expanding pass), [3] launches (keyframe chunks). */
+int ltr_scanside_stats(ltr_ctx* ctx, int64_t* stats4);
+
 /* ---- multi-GPU exchange points (NCCL, on the context's stream; libnccl is dlopen'ed at first use) ----------------
  * The path shards by keyframe: every per-keyframe loop of the reference (Removerter.cpp:429-593, Session.cpp:348-427) runs on the
  * rank owning the keyframe.  What crosses ranks: the OR of the per-pass dynamic flags (the reference's set union over scans,

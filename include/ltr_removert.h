@@ -100,6 +100,13 @@ int ltrh_reset_to_step0(ltrh_removerter* r);
  * entry does exactly that in device memory (the scans never leave the GPU) after ltrh_run_step3: central keyframe_scans_ <- VoxelGrid(keyframe_scans_updated_), central poses
  * kept, query session and every derived cloud released, log cleared.  Then ltrh_load_session(r, 1, next query) and run the steps again. */
 int ltrh_cascade_promote_updated(ltrh_removerter* r);
+/* Removerter::scansideRemovalForEachScan(map_sess, scan_sess) (Removerter.cpp:1253-1310, commented out in the reference; what
+ * saveCleanScansPCD asks for): every keyframe of scan_sess held by this rank is split by ltr_scanside_split against map_sess's
+ * map_global_curr_static_ with num_nn_points_within / dist_nn_points_within; criterion = ltr_scanside_criterion.  Results: the scan sets
+ * "scans_static_" / "scans_dynamic_" of scan_sess (ltrh_scanset).  (C,C) / (Q,Q) clean a session by itself, (C,Q) / (Q,C) give
+ * scan-level positive / negative differences.  Valid after ltrh_run_step12 until ltrh_reset_to_step0 or ltrh_cascade_promote_updated
+ * (which release the results).  Multi-GPU: each rank splits its own keyframe block; no collective. */
+int ltrh_scanside_removal(ltrh_removerter* r, int32_t map_sess, int32_t scan_sess, int32_t criterion);
 /* a single member function of Removerter by name, e.g. "removeHighDynamicPoints" */
 int ltrh_stage(ltrh_removerter* r, const char* name);
 

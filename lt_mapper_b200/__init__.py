@@ -5,4 +5,4 @@ Removerter / Session call graph on top of it.  CUDA-only: importing works anywhe
 context without libltr_b200.so or without an sm_90 GPU raises.
 """
 from . import binding  # noqa: F401
-from .binding import Context, LtrError, MODE_HD, MODE_ND, MODE_PD, reset_rimg_size  # noqa: F401
+from .binding import Context, LtrError, MODE_HD, MODE_ND, MODE_PD, SCANSIDE_MAP, SCANSIDE_SCAN_MINUS_MAP, reset_rimg_size  # noqa: F401

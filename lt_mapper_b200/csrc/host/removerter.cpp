@@ -42,7 +42,7 @@ std::map<std::string, ltr_scanset*> Session::scanset_names() {
             {"scans_knn_diff_", &scans_knn_diff_}, {"keyframe_scans_updated_", &keyframe_scans_updated_},
             {"keyframe_scans_updated_strong_", &keyframe_scans_updated_strong_}, {"keyframe_scans_pd_", &keyframe_scans_pd_},
             {"keyframe_scans_strong_pd_", &keyframe_scans_strong_pd_}, {"keyframe_scans_strong_nd_", &keyframe_scans_strong_nd_},
-            {"keyframe_scans_weak_nd_", &keyframe_scans_weak_nd_}};
+            {"keyframe_scans_weak_nd_", &keyframe_scans_weak_nd_}, {"scans_static_", &scans_static_}, {"scans_dynamic_", &scans_dynamic_}};
 }
 
 Removerter::Removerter(const ltrh_params& p) : P(p) {
@@ -434,6 +434,21 @@ int Removerter::removeHighDynamicPoints() {
     return LTR_OK;
 }
 
+// Multi-GPU: every rank splits the keyframes of scan_sess it holds (its own block, poses included) and needs no collective: after
+// removeHighDynamicPoints every rank holds both sessions' static maps -- replicated over all ranks, or in session-split mode its own
+// session's map from Step 1 and the other one from the exchange above.
+int Removerter::scansideRemovalForEachScan(Session& map_sess, Session& scan_sess, int criterion) {
+    StageTimer t(*this, "scanside");
+    if (!owns(scan_sess)) return LTR_OK;
+    if (map_sess.map_global_curr_static_ < 0) return fail(LTR_ERR_INVALID, "scansideRemovalForEachScan: no static map of the " + map_sess.sess_type_ + " session (run Steps 1-2 first)");
+    if (scan_sess.keyframe_scans_ < 0) return fail(LTR_ERR_INVALID, "scansideRemovalForEachScan: no keyframe scans of the " + scan_sess.sess_type_ + " session");
+    ltr_scanset st, dy;
+    CK(ltr_scanside_split(ctx, scan_sess.keyframe_scans_, scan_sess.keyframe_poses_, 0, map_sess.map_global_curr_static_, criterion,
+                          P.num_nn_points_within, P.dist_nn_points_within, &st, &dy));   // :1302-1309
+    CK(set(&scan_sess.scans_static_, st, true));
+    return set(&scan_sess.scans_dynamic_, dy, true);
+}
+
 int Removerter::parseScansViaProjection(Session& s, ltr_cloud map, ltr_scanset* vec_to_store) {
     ltr_scanset out;
     CK(ltr_parse_projected(ctx, map, s.keyframe_poses_, 0, s.num_keyframes_, Session::kReprojectionAlpha, &out));
@@ -783,6 +798,13 @@ int ltrh_run_step12(ltrh_removerter* r) { r->R->err.clear(); return r->R->run_st
 int ltrh_run_step3(ltrh_removerter* r) { r->R->err.clear(); return r->R->run_step3(); }
 int ltrh_reset_to_step0(ltrh_removerter* r) { r->R->err.clear(); return r->R->reset_to_step0(); }
 int ltrh_cascade_promote_updated(ltrh_removerter* r) { if (!r) return LTR_ERR_INVALID; r->R->err.clear(); return r->R->cascade_promote_updated(); }
+
+int ltrh_scanside_removal(ltrh_removerter* r, int32_t map_sess, int32_t scan_sess, int32_t criterion) {
+    if (!r || (map_sess != 0 && map_sess != 1) || (scan_sess != 0 && scan_sess != 1)) return LTR_ERR_INVALID;
+    Removerter& R = *r->R;
+    R.err.clear();
+    return R.scansideRemovalForEachScan(map_sess == 0 ? R.central_sess_ : R.query_sess_, scan_sess == 0 ? R.central_sess_ : R.query_sess_, criterion);
+}
 
 int ltrh_stage(ltrh_removerter* r, const char* name) {
     Removerter& R = *r->R;

@@ -30,6 +30,8 @@ public:
     ltr_scanset scans_knn_coexist_ = -1, scans_knn_diff_ = -1;
     ltr_scanset keyframe_scans_updated_ = -1, keyframe_scans_updated_strong_ = -1, keyframe_scans_pd_ = -1,
                 keyframe_scans_strong_pd_ = -1, keyframe_scans_strong_nd_ = -1, keyframe_scans_weak_nd_ = -1;
+    // scan-side removal of this session's scans (the commented central_/query_scans_{static,dynamic}_ of Removerter.h)
+    ltr_scanset scans_static_ = -1, scans_dynamic_ = -1;
     // maps (Session.h:67-87)
     ltr_cloud map_global_orig_ = -1, map_global_curr_ = -1, map_global_curr_static_ = -1, map_global_curr_dynamic_ = -1;
     ltr_cloud map_global_updated_ = -1, map_global_updated_strong_ = -1;
@@ -65,6 +67,9 @@ public:
     int parseUpdatedStaticScansViaProjection();                                // :1551-1561
     int parseLDScansViaProjection();                                           // :1564-1577
     int updateScansScanwise();                                                 // :1540-1548 -> Session.cpp:362-380
+    // :1253-1310 (commented out in the reference): scan_sess.scans_{static,dynamic}_ <- removeDynamicPointsOfScanByKnn (:1019-1123) of
+    // every keyframe of scan_sess this rank holds, against map_sess.map_global_curr_static_; criterion = ltr_scanside_criterion
+    int scansideRemovalForEachScan(Session& map_sess, Session& scan_sess, int criterion);
     int run_step0();
     int run_step12();
     int run_step3();

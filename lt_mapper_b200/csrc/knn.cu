@@ -239,6 +239,29 @@ static int build_grid(ltr_ctx* ctx, const DevCloud& target, int k, float thr, Gr
     return LTR_OK;
 }
 
+int knn_target_build(ltr_ctx* ctx, const DevCloud& target, int k, float thr, KnnTarget* t, void** block) {
+    *t = KnnTarget();
+    if (target.n < k) { t->small = view(target); return LTR_OK; }
+    GridBuf gb;
+    LTR_TRY(build_grid(ctx, target, k, thr, &gb));
+    for (int d = 0; d < 3; ++d) { t->origin[d] = gb.g.origin[d]; t->dim[d] = gb.g.dim[d]; }
+    t->inv_cell = gb.g.inv_cell;
+    t->cell_start = gb.cell_start;
+    t->sorted = gb.sorted;
+    *block = gb.block;
+    return LTR_OK;
+}
+
+int knn_target_label(ltr_ctx* ctx, const KnnTarget& t, PtrView q, int k, float thr, uint8_t* label) {
+    if (q.n == 0) return LTR_OK;
+    Grid g;
+    for (int d = 0; d < 3; ++d) { g.origin[d] = t.origin[d]; g.dim[d] = t.dim[d]; }
+    g.inv_cell = t.inv_cell;
+    knn_cloud_label_kernel<<<(unsigned)((q.n + 127) / 128), 128, 0, ctx->stream>>>(q, g, t.cell_start, t.sorted, k, thr, label, t.small);
+    LTR_LAUNCH_CHECK(ctx);
+    return LTR_OK;
+}
+
 }  // namespace ltr
 
 using namespace ltr;

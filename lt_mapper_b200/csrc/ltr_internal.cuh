@@ -102,6 +102,7 @@ struct ltr_ctx {
     int scan_images_busy = 0;                  // a pass is reading a set: the allocator must not free their storage
     bool rs_attr_set = false;    // radix-sort scatter kernel opted in to > 48 KB shared memory on this device
     int64_t vox_shortcuts = 0;   // voxelisations answered by the already-one-point-per-voxel shortcut (util.cu)
+    int64_t scanside_stats[4] = {0, 0, 0, 0};   // ltr_scanside_stats (scanside.cu)
     bool ext_identity = true;     // base2lidar/lidar2base exactly identity -> second transform step is exact and skipped
     double* d_ext = nullptr;      // 24 doubles: base2lidar rows 0..2, lidar2base rows 0..2
     double stats[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -222,5 +223,19 @@ bool scan_images_have_storage(const ltr_ctx* ctx);
 
 int segment_counts(ltr_ctx* ctx, const uint8_t* flags, const DevScanSet& s, std::vector<int64_t>* counts);
 int split_scanset_by_flag(ltr_ctx* ctx, const DevScanSet& in, const uint8_t* flags, ltr_scanset* out_unflagged, ltr_scanset* out_flagged);
+
+// The thresholded kNN decision of ltr_knn_split_cloud (knn.cu) against one target, built once and applied to any number of query views
+// already in the target's frame (scan-side removal, scanside.cu).  knn_target_build: 1 <= k <= 16, thr > 0, target of >= 1 finite points;
+// the caller returns *block to the allocator.  knn_target_label: label[i] = 1 if |avg| >= thr ("far"), else 0.
+struct KnnTarget {
+    double origin[3] = {0, 0, 0};
+    double inv_cell = 0;
+    int dim[3] = {0, 0, 0};
+    const uint32_t* cell_start = nullptr;
+    const float4* sorted = nullptr;
+    PtrView small{nullptr, nullptr, nullptr, nullptr, 0};   // targets of fewer than k points are searched by brute force
+};
+int knn_target_build(ltr_ctx* ctx, const DevCloud& target, int k, float thr, KnnTarget* t, void** block);
+int knn_target_label(ltr_ctx* ctx, const KnnTarget& t, PtrView q, int k, float thr, uint8_t* label);
 
 }  // namespace ltr

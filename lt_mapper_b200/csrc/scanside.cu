@@ -1,0 +1,549 @@
+// libltr_b200.so -- scan-side removal: every keyframe's own scan, at full resolution, split into static and dynamic points.
+//
+// Reference functions (kept in the node's sources but commented out; params_ltmapper.yaml's saveCleanScansPCD asks for their output):
+//   Removerter::removeDynamicPointsOfScanByKnn(int, const Session&, kdtree)   ltremovert/src/Removerter.cpp:1019-1069   criterion "map"
+//   Removerter::removeDynamicPointsOfScanByKnn(int)                             ltremovert/src/Removerter.cpp:1071-1123   "scan minus map"
+//   Removerter::scansideRemovalForEachScan(map_sess, scan_sess)                 ltremovert/src/Removerter.cpp:1253-1310
+// Transforms: scan_global = local2global(scan, pose, kSE3MatExtrinsicLiDARtoPoseBase), the live 3-argument overload of
+// utility.cpp:160-168 (the commented code calls a 2-argument overload that no longer exists; partitionLowDynamicPointsOfScanByKnn passes
+// the other extrinsic; with the identity extrinsic all of them agree); both parts go back with global2local(..., inv_pose,
+// kSE3MatExtrinsicPoseBasetoLiDAR) (utility.cpp:194-202).
+//
+// "map" needs only the decision |avg_map| < thr: that is knn.cu's bounded 27-cell grid search (its header has the proof).
+// "scan minus map" needs the exact VALUES of avg_scan and avg_map -- two large averages can differ by less than thr -- so no radius bound
+// applies.  Both averages come from an exact k-NN over sparse grids:
+//   * a grid level sorts its points by the 64-bit key (segment, cz, cy, cx) with the project's radix sort (util.cu) and keeps the sorted
+//     unique keys and each cell's first point.  Segment = keyframe of the launch for the own-scan targets, 0 for the map.  A row of cells
+//     (one segment, cz, cy; consecutive cx) is one contiguous key range: one binary search per row.
+//   * a query searches shell by shell (Chebyshev radius s = 0, 1, ... in cells around its own cell) and stops after shell s when the
+//     block holds every cell of the level, or when its current k-th smallest computed distance D_k satisfies
+//         D_k <= ((s - 2^-6) c)^2 (1 - 2^-20)        (c = 1 / inv_cell, the cell side the indices are computed with), or D_k = 0.
+// Why the stop is exact.  A point p outside the block lies in a cell whose index differs from the query's by >= s + 1 on some axis a.
+// Both indices are floor(fl(fl(v - origin) * inv_cell)) with |.| clamped to 2^40 (a clamp only moves a query's index towards the box, so
+// its true distance is larger still); each evaluation carries a relative error below 3 * 2^-53, i.e. below 2^-11 cells for |index| <= 2^40,
+// so |p_a - q_a| >= (s - 2^-10) c > (s - 2^-6) c in exact arithmetic.  FLANN's L2_Simple in f32 (((dx*dx) + dy*dy) + dz*dz, no FMA):
+// rounding is monotone, so |dx| = |fl(q_a - p_a)| >= fl((s - 2^-6) c) >= (s - 2^-6) c (1 - u), u = 2^-24, fl(dx*dx) >= dx^2 (1 - u), and the
+// two additions of non-negative terms round to no less than fl(dx*dx).  The computed distance of p is therefore
+// >= ((s - 2^-6) c)^2 (1 - u)^3 > ((s - 2^-6) c)^2 (1 - 2^-20) >= D_k: no point outside the block can displace a value of the k smallest
+// (a tie at D_k leaves the multiset unchanged), so the double sum in ascending order, its float rounding and the division by float(k) are
+// final.  D_k = 0 cannot be undercut by any distance.  How many values enter the sum is min(k, points evaluated), never "finite ones":
+// an overflowed +inf distance is summed as FLANN would return it.
+// Two passes: a bounded pass on the finest level (c0 = 0.25 m, shells 0..2) settles almost every point.  The rest (isolated returns at
+// long range, queries far from the map) are compacted into a list and searched on levels of 4x, 16x, ... the cell side, bounded again
+// except on the coarsest level (at most 10 cells per axis), which searches until the stop rule holds.  A level changes the cost only.
+// Memory: keyframes go through in launches of at most LTR_SCANSIDE_CHUNK_POINTS points (default 2^24, a keyframe is never split); per
+// launch the global coordinates (16 B/point), two averages (8 B/point), two unsettled lists (8 B/point) and one own-scan grid level
+// (28 B/point, plus 32 B/point of sort scratch while it is built).  The map's levels (28 B per map point each) are built once per call and
+// only as far as some query needs them.  Beside that the call holds one flag byte per point and a relocalised copy of the scans
+// (16 B/point) for the final order-preserving compaction, as ltr_knn_diff does.  All of it comes from the context's caching allocator and
+// is returned before the call ends.
+#include "ltr_internal.cuh"
+#include "ref_math.cuh"
+#include "device_util.cuh"
+#include <algorithm>
+#include <cmath>
+#include <cstdlib>
+
+namespace ltr {
+
+namespace {
+
+constexpr int kMaxK = 16;
+constexpr int kCellBits = 17;                 // per axis: indices < 2^17
+constexpr int kSegShift = 3 * kCellBits;      // 51: segment above the three cell indices
+constexpr int kMaxSegments = 1 << (64 - kSegShift);   // 8192 keyframes per launch
+constexpr int kMaxDim = (1 << kCellBits) - 1;
+constexpr double kCell0 = 0.25;               // finest cell side [m]
+constexpr double kLevelRatio = 4.0;
+constexpr int kMaxLevels = 8;
+constexpr int kFinalDim = 10;                 // a level of at most this many cells per axis is searched without a shell bound
+constexpr int kBoundedShells = 2;
+constexpr int64_t kChunkPoints = (int64_t)1 << 24;
+
+int64_t chunk_points() {
+    int64_t n = kChunkPoints;
+    if (const char* e = std::getenv("LTR_SCANSIDE_CHUNK_POINTS")) if (*e) n = std::min<int64_t>(std::max<int64_t>(std::atoll(e), 1), (int64_t)1 << 30);
+    return n;
+}
+
+struct Level {
+    double origin[3];
+    double inv_cell, cell;          // cell = 1 / inv_cell
+    int dim[3];
+    int final_level;
+    const unsigned long long* keys; // sorted unique (segment, cell) keys
+    const uint32_t* start;          // first point of each cell, [ncell] = number of points
+    const float4* pts;              // points in key order
+    const uint32_t* seg_first;      // cells of segment s: [seg_first[s], seg_first[s + 1])
+};
+
+struct LevelBuf {
+    Level L{};
+    void* block = nullptr;
+};
+
+__device__ __forceinline__ unsigned long long cell_key(int seg, long long cx, long long cy, long long cz) {
+    return ((unsigned long long)seg << kSegShift) | ((unsigned long long)cz << (2 * kCellBits)) | ((unsigned long long)cy << kCellBits) |
+           (unsigned long long)cx;
+}
+
+__device__ __forceinline__ long long cell_index(double v, double origin, double inv_cell) {
+    const double t = fmin(fmax((v - origin) * inv_cell, -0x1p40), 0x1p40);
+    return (long long)floor(t);
+}
+
+// ---- level build -------------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) level_key_kernel(PtrView p, const int64_t* __restrict__ off, int nseg, Level L,
+                                                        unsigned long long* __restrict__ keys, uint32_t* __restrict__ idx) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= p.n) return;
+    const int seg = off ? find_kf(off, nseg, i) : 0;
+    long long c[3];
+    const float v[3] = {p.x[i], p.y[i], p.z[i]};
+#pragma unroll
+    for (int d = 0; d < 3; ++d) c[d] = min(max(cell_index((double)v[d], L.origin[d], L.inv_cell), 0ll), (long long)L.dim[d] - 1);
+    keys[i] = cell_key(seg, c[0], c[1], c[2]);
+    idx[i] = (uint32_t)i;
+}
+
+__global__ void __launch_bounds__(256) level_head_kernel(const unsigned long long* __restrict__ keys, int64_t n, uint32_t* __restrict__ head) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    head[i] = (i == 0 || keys[i] != keys[i - 1]) ? 1u : 0u;
+}
+
+__global__ void __launch_bounds__(256) level_compact_kernel(PtrView p, const unsigned long long* __restrict__ keys, const uint32_t* __restrict__ idx,
+                                                            const uint32_t* __restrict__ head, const uint32_t* __restrict__ pos, int64_t n,
+                                                            unsigned long long* __restrict__ ukeys, uint32_t* __restrict__ start,
+                                                            float4* __restrict__ pts, uint32_t* __restrict__ ncell) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    if (head[i]) { ukeys[pos[i]] = keys[i]; start[pos[i]] = (uint32_t)i; }
+    if (i == n - 1) { const uint32_t m = pos[i] + head[i]; start[m] = (uint32_t)n; *ncell = m; }
+    const uint32_t j = idx[i];
+    pts[i] = make_float4(p.x[j], p.y[j], p.z[j], 0.0f);
+}
+
+__global__ void level_segments_kernel(const unsigned long long* __restrict__ ukeys, const uint32_t* __restrict__ ncell, int nseg,
+                                      uint32_t* __restrict__ seg_first) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s > nseg) return;
+    const unsigned long long key = (unsigned long long)s << kSegShift;
+    uint32_t lo = 0, hi = *ncell;
+    if (s < nseg) {
+        while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (ukeys[mid] < key) lo = mid + 1; else hi = mid; }
+    } else lo = hi;
+    seg_first[s] = lo;
+}
+
+// Grid level of cell side `cell` over the points of p (segments from off, or one segment), box [mn, mx] of p.
+int build_level(ltr_ctx* ctx, PtrView p, const int64_t* d_off, int nseg, const float mn[3], const float mx[3], double cell, bool final_level,
+                LevelBuf* out) {
+    Level L{};
+    L.inv_cell = 1.0 / cell;
+    L.cell = 1.0 / L.inv_cell;
+    for (int d = 0; d < 3; ++d) {
+        L.origin[d] = (double)mn[d] - cell;   // one guard cell below the minimum
+        L.dim[d] = (int)std::floor(((double)mx[d] - L.origin[d]) * L.inv_cell) + 2;
+    }
+    L.final_level = final_level ? 1 : 0;
+    const int64_t n = p.n;
+    auto pad = [](size_t b) { return (b + 255) / 256 * 256; };
+    const size_t b_keys = pad((size_t)n * 8), b_start = pad((size_t)(n + 1) * 4), b_pts = pad((size_t)n * 16), b_seg = pad((size_t)(nseg + 2) * 4);
+    void* blk = nullptr;
+    ScratchGuard g_blk(ctx, &blk);
+    LTR_TRY(dev_alloc(ctx, &blk, b_keys + b_start + b_pts + b_seg));
+    char* c = (char*)blk;
+    unsigned long long* ukeys = (unsigned long long*)c;
+    uint32_t* start = (uint32_t*)(c + b_keys);
+    float4* pts = (float4*)(c + b_keys + b_start);
+    uint32_t* seg_first = (uint32_t*)(c + b_keys + b_start + b_pts);
+    uint32_t* ncell = seg_first + nseg + 1;
+    void* tmp = nullptr;
+    ScratchGuard g_tmp(ctx, &tmp);
+    const size_t b_k = pad((size_t)n * 8), b_v = pad((size_t)n * 4);
+    LTR_TRY(dev_alloc(ctx, &tmp, 2 * b_k + 4 * b_v));
+    char* t = (char*)tmp;
+    unsigned long long* k0 = (unsigned long long*)t;
+    unsigned long long* k1 = (unsigned long long*)(t + b_k);
+    uint32_t* v0 = (uint32_t*)(t + 2 * b_k);
+    uint32_t* v1 = (uint32_t*)(t + 2 * b_k + b_v);
+    uint32_t* head = (uint32_t*)(t + 2 * b_k + 2 * b_v);
+    uint32_t* pos = (uint32_t*)(t + 2 * b_k + 3 * b_v);
+    const unsigned nb = (unsigned)((n + 255) / 256);
+    level_key_kernel<<<nb, 256, 0, ctx->stream>>>(p, d_off, nseg, L, k0, v0);
+    LTR_LAUNCH_CHECK(ctx);
+    int seg_bits = 0;
+    while ((1 << seg_bits) < nseg) ++seg_bits;
+    uint64_t* ks;
+    uint32_t* vs;
+    LTR_TRY(radix_sort_pairs(ctx, (uint64_t*)k0, (uint64_t*)k1, v0, v1, n, 0, kSegShift + seg_bits, &ks, &vs));
+    level_head_kernel<<<nb, 256, 0, ctx->stream>>>((const unsigned long long*)ks, n, head);
+    LTR_LAUNCH_CHECK(ctx);
+    LTR_TRY(exclusive_scan_u32(ctx, head, pos, n));
+    level_compact_kernel<<<nb, 256, 0, ctx->stream>>>(p, (const unsigned long long*)ks, vs, head, pos, n, ukeys, start, pts, ncell);
+    LTR_LAUNCH_CHECK(ctx);
+    level_segments_kernel<<<(nseg + 1 + 127) / 128, 128, 0, ctx->stream>>>(ukeys, ncell, nseg, seg_first);
+    LTR_LAUNCH_CHECK(ctx);
+    g_tmp.release();
+    L.keys = ukeys; L.start = start; L.pts = pts; L.seg_first = seg_first;
+    out->L = L;
+    out->block = blk;
+    blk = nullptr;   // ownership moves to out
+    return LTR_OK;
+}
+
+// ---- exact k-NN ----------------------------------------------------------------------------------------------------------------------
+template <int K>
+struct Best {
+    float d[K];
+    long long seen;
+    __device__ __forceinline__ void init() {
+#pragma unroll
+        for (int j = 0; j < K; ++j) d[j] = __int_as_float(0x7f800000);
+        seen = 0;
+    }
+    __device__ __forceinline__ void push(float v) {
+        ++seen;
+        if (v < d[K - 1]) {
+            d[K - 1] = v;
+#pragma unroll
+            for (int j = K - 1; j > 0; --j)
+                if (d[j] < d[j - 1]) { const float t = d[j]; d[j] = d[j - 1]; d[j - 1] = t; }
+        }
+    }
+};
+
+template <int K>
+__device__ __forceinline__ void scan_row(const Level& L, uint32_t c0, uint32_t c1, int seg, long long xa, long long xb, long long y, long long z,
+                                         float qx, float qy, float qz, Best<K>& b) {
+    const unsigned long long ka = cell_key(seg, xa, y, z), kb = cell_key(seg, xb, y, z);
+    uint32_t lo = c0, hi = c1;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (L.keys[mid] < ka) lo = mid + 1; else hi = mid; }
+    for (uint32_t ci = lo; ci < c1 && L.keys[ci] <= kb; ++ci) {
+        const uint32_t e = L.start[ci + 1];
+        for (uint32_t p = L.start[ci]; p < e; ++p) {
+            const float4 t = L.pts[p];
+            b.push(l2_simple(qx, qy, qz, t.x, t.y, t.z));
+        }
+    }
+}
+
+// Exact mean of the k smallest squared distances from q to the points of segment `seg` (file header).  false: not settled within
+// max_shell shells on a bounded level.
+template <int K>
+__device__ bool knn_exact_avg(const Level& L, int seg, float qx, float qy, float qz, int max_shell, float* avg) {
+    Best<K> b;
+    b.init();
+    const float q[3] = {qx, qy, qz};
+    long long c[3], s0 = 0, cover = 0;
+#pragma unroll
+    for (int d = 0; d < 3; ++d) {
+        c[d] = cell_index((double)q[d], L.origin[d], L.inv_cell);
+        const long long hi = (long long)L.dim[d] - 1;
+        s0 = max(s0, max(-c[d], c[d] - hi));       // Chebyshev distance from the query's cell to the box: nearer shells are empty
+        cover = max(cover, max(c[d], hi - c[d]));  // from this radius on the block holds every cell
+    }
+    const uint32_t c0 = L.seg_first[seg], c1 = L.seg_first[seg + 1];
+    bool done = c0 == c1;
+    for (long long s = s0; !done; ++s) {
+        if (!L.final_level && s > max_shell) return false;
+        const long long z0 = max(c[2] - s, 0ll), z1 = min(c[2] + s, (long long)L.dim[2] - 1);
+        const long long y0 = max(c[1] - s, 0ll), y1 = min(c[1] + s, (long long)L.dim[1] - 1);
+        const long long xa = max(c[0] - s, 0ll), xb = min(c[0] + s, (long long)L.dim[0] - 1);
+        for (long long z = z0; z <= z1; ++z) {
+            const bool zface = z == c[2] - s || z == c[2] + s;
+            for (long long y = y0; y <= y1; ++y) {
+                if (zface || y == c[1] - s || y == c[1] + s) {
+                    if (xa <= xb) scan_row<K>(L, c0, c1, seg, xa, xb, y, z, qx, qy, qz, b);
+                } else {
+                    if (c[0] - s >= 0 && c[0] - s < L.dim[0]) scan_row<K>(L, c0, c1, seg, c[0] - s, c[0] - s, y, z, qx, qy, qz, b);
+                    if (s > 0 && c[0] + s >= 0 && c[0] + s < L.dim[0]) scan_row<K>(L, c0, c1, seg, c[0] + s, c[0] + s, y, z, qx, qy, qz, b);
+                }
+            }
+        }
+        if (s >= cover) break;
+        if (b.seen >= K) {
+            const double dk = (double)b.d[K - 1];
+            const double r = ((double)s - 0x1p-6) * L.cell;
+            if (dk == 0.0 || (s > 0 && dk <= r * r * (1.0 - 0x1p-20))) done = true;
+        }
+    }
+    // accumulate(..., 0.0) in double, ascending (Removerter.cpp:1052, 1097); float(sum) / float(k) (:1053, 1098)
+    const int cnt = b.seen < K ? (int)b.seen : K;
+    double sum = 0.0;
+#pragma unroll
+    for (int j = 0; j < K; ++j) if (j < cnt) sum = da(sum, (double)b.d[j]);
+    *avg = fd(__double2float_rn(sum), (float)K);
+    return true;
+}
+
+// One level for the queries list[0..n) (list == nullptr: the queries 0..n): settled ones write avg[i], the others go to next.
+template <int K>
+__global__ void __launch_bounds__(128) exact_knn_kernel(Level L, PtrView q, const int64_t* __restrict__ q_off, int nseg,
+                                                        const uint32_t* __restrict__ list, int64_t n, int max_shell, float* __restrict__ avg,
+                                                        uint32_t* __restrict__ next, unsigned int* __restrict__ next_cnt) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    const uint32_t i = list ? list[t] : (uint32_t)t;
+    const int seg = q_off ? find_kf(q_off, nseg, i) : 0;
+    float a;
+    if (knn_exact_avg<K>(L, seg, q.x[i], q.y[i], q.z[i], max_shell, &a)) avg[i] = a;
+    else next[atomicAdd(next_cnt, 1u)] = i;
+}
+
+int launch_exact_knn(ltr_ctx* ctx, int k, const Level& L, PtrView q, const int64_t* q_off, int nseg, const uint32_t* list, int64_t n,
+                     float* avg, uint32_t* next, unsigned int* next_cnt) {
+    if (n == 0) return LTR_OK;
+    const unsigned nb = (unsigned)((n + 127) / 128);
+    switch (k) {
+#define LTR_SCANSIDE_CASE(KK) \
+        case KK: exact_knn_kernel<KK><<<nb, 128, 0, ctx->stream>>>(L, q, q_off, nseg, list, n, kBoundedShells, avg, next, next_cnt); break;
+        LTR_SCANSIDE_CASE(1) LTR_SCANSIDE_CASE(2) LTR_SCANSIDE_CASE(3) LTR_SCANSIDE_CASE(4) LTR_SCANSIDE_CASE(5) LTR_SCANSIDE_CASE(6)
+        LTR_SCANSIDE_CASE(7) LTR_SCANSIDE_CASE(8) LTR_SCANSIDE_CASE(9) LTR_SCANSIDE_CASE(10) LTR_SCANSIDE_CASE(11) LTR_SCANSIDE_CASE(12)
+        LTR_SCANSIDE_CASE(13) LTR_SCANSIDE_CASE(14) LTR_SCANSIDE_CASE(15) LTR_SCANSIDE_CASE(16)
+#undef LTR_SCANSIDE_CASE
+        default: return fail(ctx, LTR_ERR_UNSUPPORTED, "k = %d outside [1, %d]", k, kMaxK);
+    }
+    LTR_LAUNCH_CHECK(ctx);
+    return LTR_OK;
+}
+
+// The levels of one target, finest first, built as far as some query needs them.
+struct Pyramid {
+    PtrView pts{nullptr, nullptr, nullptr, nullptr, 0};
+    const int64_t* d_off = nullptr;
+    int nseg = 1;
+    float mn[3], mx[3];
+    double cell0 = kCell0;
+    std::vector<LevelBuf> levels;
+
+    void init(PtrView p, const int64_t* off, int ns, const float lo[3], const float hi[3]) {
+        pts = p; d_off = off; nseg = ns;
+        double ext = 0.0;
+        for (int d = 0; d < 3; ++d) { mn[d] = lo[d]; mx[d] = hi[d]; ext = std::max(ext, (double)hi[d] - (double)lo[d]); }
+        cell0 = std::max(kCell0, ext / (double)(kMaxDim - 4));   // indices < 2^17 on the finest level
+    }
+    int get(ltr_ctx* ctx, int l, const Level** out) {
+        while ((int)levels.size() <= l) {
+            const int m = (int)levels.size();
+            const double cell = cell0 * std::pow(kLevelRatio, m);
+            int dmax = 0;
+            for (int d = 0; d < 3; ++d) dmax = std::max(dmax, (int)std::floor(((double)mx[d] - (double)mn[d]) / cell) + 3);
+            LevelBuf b;
+            LTR_TRY(build_level(ctx, pts, d_off, nseg, mn, mx, cell, dmax <= kFinalDim || m == kMaxLevels - 1, &b));
+            levels.push_back(b);
+        }
+        *out = &levels[(size_t)l].L;
+        return LTR_OK;
+    }
+    void release(ltr_ctx* ctx) { for (auto& b : levels) if (b.block) dev_free(ctx, b.block); levels.clear(); }
+};
+
+// avg[i] for every query of q against the target pyramid; *unsettled = queries the bounded pass on the finest level left over.
+int exact_avg_all(ltr_ctx* ctx, Pyramid& T, int k, PtrView q, const int64_t* q_off, int nseg, float* avg, uint32_t* list_a,
+                  uint32_t* list_b, unsigned int* d_cnt, int64_t* unsettled) {
+    const uint32_t* list = nullptr;
+    int64_t n = q.n;
+    *unsettled = 0;
+    for (int l = 0; n > 0; ++l) {
+        const Level* L;
+        LTR_TRY(T.get(ctx, l, &L));
+        uint32_t* next = (list == list_a) ? list_b : list_a;
+        LTR_CUDA(ctx, cudaMemsetAsync(d_cnt, 0, sizeof(unsigned int), ctx->stream));
+        LTR_TRY(launch_exact_knn(ctx, k, *L, q, q_off, nseg, list, n, avg, next, d_cnt));
+        if (L->final_level) break;
+        unsigned int h = 0;
+        LTR_CUDA(ctx, cudaMemcpyAsync(&h, d_cnt, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
+        LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        if (l == 0) *unsettled = h;
+        list = next;
+        n = h;
+    }
+    return LTR_OK;
+}
+
+// ---- transforms and decisions --------------------------------------------------------------------------------------------------------
+// local2global (utility.cpp:164-165): lidar2base, then the pose, f32 rounding after each step
+__global__ void __launch_bounds__(256) scanside_global_kernel(PtrView in, const int64_t* __restrict__ off, int K, int64_t base,
+                                                              const double* __restrict__ poses, int pose_offset, const double* __restrict__ ext,
+                                                              int ext_identity, int order, int64_t n, float* __restrict__ gx,
+                                                              float* __restrict__ gy, float* __restrict__ gz) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    const int64_t i = base + t;
+    const int k = find_kf(off, K, i);
+    float x = in.x[i], y = in.y[i], z = in.z[i];
+    if (!ext_identity) transform_point(ext + 12, order, x, y, z, &x, &y, &z);
+    transform_point(poses + (size_t)(pose_offset + k) * 24 + 12, order, x, y, z, &x, &y, &z);
+    gx[t] = x; gy[t] = y; gz[t] = z;
+}
+
+// global2local (utility.cpp:198-199): inverse pose, then base2lidar
+__global__ void __launch_bounds__(256) scanside_local_kernel(const float* __restrict__ gx, const float* __restrict__ gy, const float* __restrict__ gz,
+                                                             const int64_t* __restrict__ off, int K, int64_t base, const double* __restrict__ poses,
+                                                             int pose_offset, const double* __restrict__ ext, int ext_identity, int order,
+                                                             int64_t n, DevCloud out) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    const int64_t i = base + t;
+    const int k = find_kf(off, K, i);
+    float x = gx[t], y = gy[t], z = gz[t];
+    transform_point(poses + (size_t)(pose_offset + k) * 24, order, x, y, z, &x, &y, &z);
+    if (!ext_identity) transform_point(ext, order, x, y, z, &x, &y, &z);
+    out.x()[i] = x; out.y()[i] = y; out.z()[i] = z;
+}
+
+// fabsf(avg_scan - avg_map) < thr -> static (Removerter.cpp:1107), the subtraction in f32
+__global__ void __launch_bounds__(256) scanside_diff_kernel(const float* __restrict__ avg_scan, const float* __restrict__ avg_map, int64_t n,
+                                                            float thr, uint8_t* __restrict__ flag) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    flag[t] = (fabsf(fs(avg_scan[t], avg_map[t])) < thr) ? 0 : 1;
+}
+
+__global__ void __launch_bounds__(256) chunk_offsets_kernel(const int64_t* __restrict__ off, int kf0, int nkf, int64_t* __restrict__ out) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j <= nkf) out[j] = off[kf0 + j] - off[kf0];
+}
+
+}  // namespace
+}  // namespace ltr
+
+using namespace ltr;
+
+extern "C" {
+
+int ltr_scanside_split(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_offset, ltr_cloud map_h, int32_t criterion,
+                       int32_t k, float thr, ltr_scanset* out_static, ltr_scanset* out_dynamic) {
+    ApiTrace tr__(ctx, "ltr_scanside_split");
+    if (!ctx) return LTR_ERR_INVALID;
+    DevScanSet* sp;
+    DevPoses* pp;
+    DevCloud* mp;
+    LTR_TRY(scanset_get(ctx, scans_h, &sp));
+    LTR_TRY(poses_get(ctx, poses_h, &pp));
+    LTR_TRY(cloud_get(ctx, map_h, &mp));
+    if (criterion != LTR_SCANSIDE_MAP && criterion != LTR_SCANSIDE_SCAN_MINUS_MAP) return fail(ctx, LTR_ERR_INVALID, "unknown criterion %d", criterion);
+    if (k < 1 || k > kMaxK) return fail(ctx, LTR_ERR_UNSUPPORTED, "k = %d outside [1, %d]", k, kMaxK);
+    if (!(thr > 0.0f)) return fail(ctx, LTR_ERR_INVALID, "threshold must be positive");
+    if (pose_offset < 0 || pose_offset + sp->K > pp->K) return fail(ctx, LTR_ERR_INVALID, "pose range [%d,%d) outside [0,%d)", pose_offset, pose_offset + sp->K, pp->K);
+    if (mp->n < 1) return fail(ctx, LTR_ERR_UNSUPPORTED, "empty map (PCL's nearestKSearch asserts on an empty tree)");
+    const DevScanSet scans = *sp;
+    const DevPoses poses = *pp;
+    const DevCloud map = *mp;
+    for (int j = 0; j < 4; ++j) ctx->scanside_stats[j] = 0;
+    ctx->scanside_stats[0] = scans.pts.n;
+    {
+        float mn[3], mx[3];
+        uint32_t nonfinite = 0;
+        LTR_TRY(minmax_xyz(ctx, map, mn, mx, &nonfinite));
+        if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite map coordinates (%u points)", nonfinite);
+    }
+    const int64_t n = scans.pts.n;
+    const int ext_id = ctx->ext_identity ? 1 : 0, order = ctx->cfg.transform_order;
+    ltr_cloud reloc_h = -1;
+    struct CloudGuard { ltr_ctx* c; ltr_cloud* h; ~CloudGuard() { if (*h >= 0) ltr_cloud_free(c, *h); } } g_reloc{ctx, &reloc_h};
+    void* flags = nullptr;
+    ScratchGuard g_flags(ctx, &flags);
+    LTR_TRY(dev_alloc(ctx, &flags, (size_t)std::max<int64_t>(n, 1)));
+    if (n > 0) {
+        LTR_TRY(cloud_new(ctx, n, &reloc_h));
+        const DevCloud reloc = ctx->clouds[reloc_h];
+        LTR_CUDA(ctx, cudaMemcpyAsync(reloc.i(), scans.pts.i(), (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
+        // keyframe chunks: at most chunk_points() points (a keyframe is never split) and kMaxSegments keyframes
+        const int64_t cap = chunk_points();
+        std::vector<int> kf_cut{0};
+        for (int kf = 0; kf < scans.K;) {
+            int e = kf + 1;
+            while (e < scans.K && e - kf < kMaxSegments && scans.h_off[e + 1] - scans.h_off[kf] <= cap) ++e;
+            kf_cut.push_back(e);
+            kf = e;
+        }
+        int64_t max_chunk = 0;
+        for (size_t c = 0; c + 1 < kf_cut.size(); ++c) max_chunk = std::max(max_chunk, scans.h_off[kf_cut[c + 1]] - scans.h_off[kf_cut[c]]);
+        if (max_chunk >= ((int64_t)1 << 32)) return fail(ctx, LTR_ERR_UNSUPPORTED, "a keyframe of %lld points", (long long)max_chunk);
+        const int64_t ccap = round_cap(max_chunk);
+        void* work = nullptr;
+        ScratchGuard g_work(ctx, &work);
+        // chunk global coordinates (a DevCloud layout, for minmax_xyz) | avg_map | avg_scan | two lists | counter | chunk offsets
+        const size_t b_g = (size_t)ccap * 16, b_f = (size_t)ccap * 4, b_off = ((size_t)kMaxSegments + 1) * 8;
+        LTR_TRY(dev_alloc(ctx, &work, b_g + 4 * b_f + 256 + b_off));
+        DevCloud g;
+        g.base = (float*)work; g.cap = ccap;
+        float* avg_map = (float*)((char*)work + b_g);
+        float* avg_scan = avg_map + ccap;
+        uint32_t* list_a = (uint32_t*)(avg_scan + ccap);
+        uint32_t* list_b = list_a + ccap;
+        unsigned int* d_cnt = (unsigned int*)(list_b + ccap);
+        int64_t* c_off = (int64_t*)((char*)work + b_g + 4 * b_f + 256);
+        KnnTarget kt;
+        void* kt_block = nullptr;
+        ScratchGuard g_kt(ctx, &kt_block);
+        Pyramid mapT;
+        struct PyrGuard { ltr_ctx* c; Pyramid* p; ~PyrGuard() { p->release(c); } } g_mapT{ctx, &mapT};
+        if (criterion == LTR_SCANSIDE_MAP) LTR_TRY(knn_target_build(ctx, map, k, thr, &kt, &kt_block));
+        else {
+            float mn[3], mx[3];
+            LTR_TRY(minmax_xyz(ctx, map, mn, mx));
+            mapT.init(view(map), nullptr, 1, mn, mx);
+        }
+        for (size_t c = 0; c + 1 < kf_cut.size(); ++c) {
+            const int kf0 = kf_cut[c], kf1 = kf_cut[c + 1], nkf = kf1 - kf0;
+            const int64_t base = scans.h_off[kf0], m = scans.h_off[kf1] - base;
+            ctx->scanside_stats[3]++;
+            if (m == 0) continue;
+            const unsigned nb = (unsigned)((m + 255) / 256);
+            scanside_global_kernel<<<nb, 256, 0, ctx->stream>>>(view(scans.pts), scans.d_off, scans.K, base, poses.d, pose_offset, ctx->d_ext, ext_id,
+                                                                order, m, g.x(), g.y(), g.z());
+            LTR_LAUNCH_CHECK(ctx);
+            g.n = m;
+            float mn[3], mx[3];
+            uint32_t nonfinite = 0;
+            LTR_TRY(minmax_xyz(ctx, g, mn, mx, &nonfinite));
+            if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite scan coordinates (%u points in keyframes [%d,%d))", nonfinite, kf0, kf1);
+            const PtrView q = view(g);
+            uint8_t* fl = (uint8_t*)flags + base;
+            if (criterion == LTR_SCANSIDE_MAP) {
+                // |avg_map| < thr -> static (Removerter.cpp:1056)
+                LTR_TRY(knn_target_label(ctx, kt, q, k, thr, fl));
+            } else {
+                chunk_offsets_kernel<<<(nkf + 1 + 255) / 256, 256, 0, ctx->stream>>>(scans.d_off, kf0, nkf, c_off);
+                LTR_LAUNCH_CHECK(ctx);
+                int64_t un = 0;
+                LTR_TRY(exact_avg_all(ctx, mapT, k, q, nullptr, 1, avg_map, list_a, list_b, d_cnt, &un));
+                ctx->scanside_stats[1] += un;
+                Pyramid self;
+                struct PyrGuard2 { ltr_ctx* c; Pyramid* p; ~PyrGuard2() { p->release(c); } } g_self{ctx, &self};
+                self.init(q, c_off, nkf, mn, mx);
+                LTR_TRY(exact_avg_all(ctx, self, k, q, c_off, nkf, avg_scan, list_a, list_b, d_cnt, &un));
+                ctx->scanside_stats[2] += un;
+                self.release(ctx);
+                scanside_diff_kernel<<<nb, 256, 0, ctx->stream>>>(avg_scan, avg_map, m, thr, fl);
+                LTR_LAUNCH_CHECK(ctx);
+            }
+            scanside_local_kernel<<<nb, 256, 0, ctx->stream>>>(g.x(), g.y(), g.z(), scans.d_off, scans.K, base, poses.d, pose_offset, ctx->d_ext,
+                                                               ext_id, order, m, reloc);
+            LTR_LAUNCH_CHECK(ctx);
+        }
+        mapT.release(ctx);
+        g_kt.release();
+        g_work.release();
+        DevScanSet set = scans;
+        set.pts = reloc;
+        LTR_TRY(split_scanset_by_flag(ctx, set, (const uint8_t*)flags, out_static, out_dynamic));
+        return LTR_OK;
+    }
+    std::vector<int64_t> off((size_t)scans.K + 1, 0);
+    if (out_static) LTR_TRY(scanset_new(ctx, off, out_static));
+    if (out_dynamic) LTR_TRY(scanset_new(ctx, off, out_dynamic));
+    return LTR_OK;
+}
+
+int ltr_scanside_stats(ltr_ctx* ctx, int64_t* stats4) {
+    if (!ctx || !stats4) return LTR_ERR_INVALID;
+    for (int j = 0; j < 4; ++j) stats4[j] = ctx->scanside_stats[j];
+    return LTR_OK;
+}
+
+}  // extern "C"

@@ -41,7 +41,7 @@ class Comm(ctypes.Structure):
 
 
 HOST_EXPORTS = ["ltrh_params_default", "ltrh_create", "ltrh_destroy", "ltrh_last_error", "ltrh_set_comm", "ltrh_context", "ltrh_comm_init_nccl", "ltrh_owns_session", "ltrh_invert_poses",
-                "ltrh_load_session", "ltrh_load_session_raw", "ltrh_run_step0", "ltrh_run_step12", "ltrh_run_step3", "ltrh_reset_to_step0", "ltrh_cascade_promote_updated", "ltrh_stage", "ltrh_cloud",
+                "ltrh_load_session", "ltrh_load_session_raw", "ltrh_run_step0", "ltrh_run_step12", "ltrh_run_step3", "ltrh_reset_to_step0", "ltrh_cascade_promote_updated", "ltrh_scanside_removal", "ltrh_stage", "ltrh_cloud",
                 "ltrh_scanset", "ltrh_timing", "ltrh_log_count", "ltrh_log_get", "ltrh_io_last_error", "ltrh_io_read_pcd", "ltrh_io_write_pcd",
                 "ltrh_io_read_poses", "ltrh_io_parse_keyframes", "ltrh_io_parse_keyframes_in_roi", "ltrh_io_voxel_grid", "ltrh_io_voxel_grid_scans", "ltrh_io_yaml_get"]
 
@@ -74,6 +74,7 @@ def host_lib():
     L.ltrh_load_session_raw.argtypes = [vp, i32, vp, vp, vp, vp, i32]
     for f in ("ltrh_run_step0", "ltrh_run_step12", "ltrh_run_step3", "ltrh_reset_to_step0", "ltrh_cascade_promote_updated"):
         getattr(L, f).argtypes = [vp]
+    L.ltrh_scanside_removal.argtypes = [vp, i32, i32, i32]
     L.ltrh_stage.argtypes = [vp, ctypes.c_char_p]
     L.ltrh_cloud.argtypes = [vp, ctypes.c_char_p, i32, P(i32)]
     L.ltrh_scanset.argtypes = [vp, ctypes.c_char_p, i32, P(i32)]
@@ -321,6 +322,10 @@ class Removerter:
     def cascade_promote_updated(self):
         """LT-map cascade: the updated scans become the central session of the next run (ltrh_cascade_promote_updated)."""
         self._ck(host_lib().ltrh_cascade_promote_updated(self._h))
+
+    def scanside_removal(self, map_sess, scan_sess, criterion=0):
+        """scansideRemovalForEachScan (ltrh_scanside_removal): fills the scan sets "scans_static_" / "scans_dynamic_" of scan_sess."""
+        self._ck(host_lib().ltrh_scanside_removal(self._h, map_sess, scan_sess, criterion))
 
     def stage(self, name):
         self._ck(host_lib().ltrh_stage(self._h, name.encode()))
