@@ -5,7 +5,7 @@
 // on the GPU through libltr_removert/libltr_b200, and writes the same output tree (Removerter.cpp:26-50, 231, 1446-1477,
 // 1517-1520, 1600-1601, 1607-1650).  No ROS, no PCL; rviz publishing is dropped (side effect only).
 //
-//   ltremovert_b200 --config params.yaml [--selfremovert] [--pcl110] [--no-split] [--clean-scans[=map|scan-minus-map]]
+//   ltremovert_b200 --config params.yaml [--selfremovert] [--pcl110] [--no-split] [--clean-scans[=map|scan-minus-map]] [--icp-refinement]
 //     --selfremovert   run selfRemovert over remove_resolution_list (Removerter.cpp:1378-1393) instead of the shipped
 //                      single removeOnce(2.5) (Removerter.cpp:1584, 1587)
 //     --pcl110         PCL >= 1.10 transformPointCloud summation order (ltr_config.transform_order = 1)
@@ -15,12 +15,17 @@
 //                      input scan's name (saveCleanedScans, :1143-1195), and with saveMapPCD the merged, 0.05-voxelised maps of
 //                      saveMapPointcloudByMergingCleanedScans (:1197-1251) to map_static/ and map_dynamic/.  Off by default: without it
 //                      the output tree is the one the node writes.
+//     --icp-refinement Step 2's kNN diff registers every keyframe to the other session's 0.4 m map first and keeps the registered scan
+//                      when its fitness is below 1.0 (partitionLowDynamicPointsOfScanByKnn's `useICPrefinement`, Session.cpp:549-584,
+//                      off in the reference); prints one summary line (keyframes accepted, median iterations).  The output tree keeps
+//                      its layout; the files derived from Step 2 hold the refined results.
 //
 // Multi-GPU: start one process per GPU with RANK / WORLD_SIZE / LOCAL_RANK in the environment (torchrun, mpirun -x, a shell loop);
 // every rank reads the yaml and the pose files, but loads only the scans of ITS keyframe block (even world: ranks < world/2 take the
 // central session, the others the query session; --no-split: a block of both).  The NCCL id travels through a file
 // ($LTR_NCCL_ID_FILE, default /tmp/ltr_nccl_id_<parent pid>_<MASTER_PORT>).  Maps are written by the first rank of the group that holds
 // them, per-keyframe scans by the rank that owns the keyframe; the output tree is the single-process one.
+#include <algorithm>
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
@@ -118,7 +123,8 @@ int main(int argc, char** argv) {
     std::string cfg_path;
     bool selfremovert = false, pcl110 = false, no_split = false;
     int clean_scans = -1;   // -1 off, else ltr_scanside_criterion
-    const char* usage = "usage: %s --config params.yaml [--selfremovert] [--pcl110] [--no-split] [--clean-scans[=map|scan-minus-map]]\n";
+    bool icp_refinement = false;
+    const char* usage = "usage: %s --config params.yaml [--selfremovert] [--pcl110] [--no-split] [--clean-scans[=map|scan-minus-map]] [--icp-refinement]\n";
     for (int i = 1; i < argc; ++i) {
         if (!std::strcmp(argv[i], "--config") && i + 1 < argc) cfg_path = argv[++i];
         else if (!std::strcmp(argv[i], "--selfremovert")) selfremovert = true;
@@ -126,6 +132,7 @@ int main(int argc, char** argv) {
         else if (!std::strcmp(argv[i], "--no-split")) no_split = true;
         else if (!std::strcmp(argv[i], "--clean-scans") || !std::strcmp(argv[i], "--clean-scans=map")) clean_scans = LTR_SCANSIDE_MAP;
         else if (!std::strcmp(argv[i], "--clean-scans=scan-minus-map")) clean_scans = LTR_SCANSIDE_SCAN_MINUS_MAP;
+        else if (!std::strcmp(argv[i], "--icp-refinement")) icp_refinement = true;
         else { std::fprintf(stderr, usage, argv[0]); return 2; }
     }
     if (cfg_path.empty()) { std::fprintf(stderr, usage, argv[0]); return 2; }
@@ -215,7 +222,29 @@ int main(int argc, char** argv) {
         std::vector<float>().swap(S.xyzi);   // the raw scans now live on the device
     }
     ck(R.run_step0(), "Step 0");
+    R.useICPrefinement_ = icp_refinement;
     ck(R.run_step12(), "Step 1-2");
+    if (icp_refinement) {
+        // over both sessions and every rank: [0, kMaxIt] iteration histogram, accepted, keyframes
+        constexpr int kMaxIt = 100;
+        std::vector<int64_t> h(kMaxIt + 3, 0);
+        for (const Session* X : {&R.central_sess_, &R.query_sess_})
+            for (size_t k = 0; k < X->icp_iterations_.size(); ++k) {
+                h[(size_t)std::min(std::max(X->icp_iterations_[k], 0), kMaxIt)]++;
+                h[kMaxIt + 1] += X->icp_accepted_[k];
+                h[kMaxIt + 2]++;
+            }
+        if (world > 1 && R.nccl_world >= 0) {
+            std::vector<int64_t> all(h.size() * (size_t)world);
+            ck(ltr_nccl_allgather_i64(R.ctx, R.nccl_world, h.data(), (int32_t)h.size(), all.data()), "ICP summary");
+            for (size_t j = 0; j < h.size(); ++j) { h[j] = 0; for (int r = 0; r < world; ++r) h[j] += all[(size_t)r * h.size() + j]; }
+        }
+        int median = 0;
+        for (int64_t seen = 0; median <= kMaxIt; ++median) { seen += h[(size_t)median]; if (2 * seen > h[kMaxIt + 2] - 1) break; }
+        if (rank == 0)
+            std::printf(" ICP refinement: %lld of %lld keyframes accepted, median iterations %d\n", (long long)h[kMaxIt + 1], (long long)h[kMaxIt + 2],
+                        h[kMaxIt + 2] ? median : 0);
+    }
     ck(R.run_step3(), "Step 3");
     if (rank == 0) for (const auto& l : R.log)
         std::printf(" %-18s map %lld  dynamic %lld  -> static %lld  dynamic %lld\n", l.what.c_str(), (long long)l.n_map, (long long)l.n_dynamic,

@@ -206,6 +206,42 @@ int ltr_scanside_split(ltr_ctx* ctx, ltr_scanset scans, ltr_poses poses, int32_t
  * grid did not settle (they went on to the expanding pass), [3] launches (keyframe chunks). */
 int ltr_scanside_stats(ltr_ctx* ctx, int64_t* stats4);
 
+/* ICP refinement of the low-dynamic kNN diff (Session.cpp:393-402, 549-584, switched off in the reference by useICPrefinement):
+ * PCL's IterativeClosestPoint control flow with the reference's parameters and arithmetic fixed by this project (DESIGN.md §5.2,
+ * lt_mapper_b200/csrc/icp.cu).  ltr_icp_params_default fills the reference's values. */
+typedef struct ltr_icp_params {
+    double max_correspondence_distance;   /* 150 (setMaxCorrespondenceDistance): pairs with d2 > 150^2 are dropped */
+    int32_t max_iterations;               /* 100 (setMaximumIterations), >= 1 */
+    double transformation_epsilon;        /* 1e-6 (setTransformationEpsilon): rotation threshold 1 - eps, squared-translation threshold eps */
+    double euclidean_fitness_epsilon;     /* 1e-6 (setEuclideanFitnessEpsilon): relative MSE change */
+    double mse_threshold_absolute;        /* 1e-12 (DefaultConvergenceCriteria): absolute MSE change */
+    int32_t min_correspondences;          /* 3: fewer correspondences stop the loop, not converged */
+    float source_leaf;                    /* 0.4 m: octreeDownsampling of each keyframe's global scan (Session.cpp:558-559) */
+} ltr_icp_params;
+/* exit reasons of ltr_icp_refine (pcl::registration::DefaultConvergenceCriteria::ConvergenceState) */
+typedef enum ltr_icp_exit {
+    LTR_ICP_ITERATIONS = 1,           /* iterations >= max_iterations */
+    LTR_ICP_TRANSFORM = 2,            /* the last increment is below the rotation and translation thresholds */
+    LTR_ICP_ABS_MSE = 3,              /* |mse - prev_mse| < mse_threshold_absolute */
+    LTR_ICP_REL_MSE = 4,              /* |mse - prev_mse| / prev_mse < euclidean_fitness_epsilon */
+    LTR_ICP_NO_CORRESPONDENCES = 5    /* fewer than min_correspondences correspondences (an empty keyframe among them) */
+} ltr_icp_exit;
+void ltr_icp_params_default(ltr_icp_params* p);
+/* Registers every keyframe k of `scans` (poses index pose_offset + k), moved to the global frame as ltr_knn_diff moves it and voxelised
+ * per keyframe at source_leaf, to `target_down` (the other session's map at 0.4 m, ltr_voxel_centroid), one CTA per keyframe.  Outputs
+ * (host arrays of K entries, each may be NULL): the final float 4x4 (row-major, 16 per keyframe), getFitnessScore() (mean nearest
+ * squared distance of the moved source to target_down, DBL_MAX without source points), iterations and the exit reason.  params NULL:
+ * the defaults.  An empty target_down or a non-finite coordinate in it or in any moved scan fails with LTR_ERR_UNSUPPORTED.  Keyframes
+ * go in launches of at most LTR_ICP_CHUNK_POINTS source points (environment; default 2^24, one keyframe at least). */
+int ltr_icp_refine(ltr_ctx* ctx, ltr_scanset scans, ltr_poses poses, int32_t pose_offset, ltr_cloud target_down, const ltr_icp_params* params,
+                   float* T16_out, double* fitness_out, int32_t* iterations_out, int32_t* exit_out);
+/* ltr_knn_diff with the refinement applied: the global points of keyframe k with accepted[k] != 0 are moved by T16[16k..16k+16) in f32
+ * (((m0 x + m1 y) + m2 z) + m3) before the kNN test against the FULL `target`; both parts go back with global2local, so they hold the
+ * registered points.  A keyframe with accepted[k] == 0 gives exactly ltr_knn_diff's bytes.  T16 and accepted are host arrays of K
+ * entries (the reference accepts iff fitness < 1.0, Session.cpp:571). */
+int ltr_knn_diff_refined(ltr_ctx* ctx, ltr_scanset scans, ltr_poses poses, int32_t pose_offset, ltr_cloud target, int32_t k, float thr,
+                         const float* T16, const uint8_t* accepted, ltr_scanset* out_coexist, ltr_scanset* out_diff);
+
 /* ---- multi-GPU exchange points (NCCL, on the context's stream; libnccl is dlopen'ed at first use) ----------------
  * The path shards by keyframe: every per-keyframe loop of the reference (Removerter.cpp:429-593, Session.cpp:348-427) runs on the
  * rank owning the keyframe.  What crosses ranks: the OR of the per-pass dynamic flags (the reference's set union over scans,

@@ -107,6 +107,17 @@ int ltrh_cascade_promote_updated(ltrh_removerter* r);
  * scan-level positive / negative differences.  Valid after ltrh_run_step12 until ltrh_reset_to_step0 or ltrh_cascade_promote_updated
  * (which release the results).  Multi-GPU: each rank splits its own keyframe block; no collective. */
 int ltrh_scanside_removal(ltrh_removerter* r, int32_t map_sess, int32_t scan_sess, int32_t criterion);
+/* Session::partitionLowDynamicPointsOfScanByKnn's ICP refinement (Session.cpp:549-584; `useICPrefinement`, false in the reference and by
+ * default here).  With on != 0 every later detectLowDynamicPoints (ltrh_run_step12) registers each keyframe to the other session's map at
+ * 0.4 m (ltr_icp_refine with the reference's parameters) and runs the kNN diff on the registered scan when its fitness is below 1.0
+ * (ltr_knn_diff_refined): scans_knn_coexist_ / scans_knn_diff_ then hold the registered points.  Multi-GPU: each rank refines its own
+ * keyframe block against its replica of the target map; no collective. */
+int ltrh_set_icp_refinement(ltrh_removerter* r, int32_t on);
+/* Per-keyframe results of the last refinement of session `sess` on this rank: *K_out keyframes (0 when the last detectLowDynamicPoints ran
+ * without refinement, and after ltrh_reset_to_step0 or ltrh_cascade_promote_updated, which release Step 2's results), and, when capacity >= *K_out, the final float 4x4 (16 per keyframe), fitness, iterations, exit reason (ltr_icp_exit)
+ * and the accepted flag (fitness < 1.0).  Any array may be NULL. */
+int ltrh_icp_stats(ltrh_removerter* r, int32_t sess, int32_t capacity, int32_t* K_out, float* T16, double* fitness, int32_t* iterations,
+                   int32_t* exit_reason, uint8_t* accepted);
 /* a single member function of Removerter by name, e.g. "removeHighDynamicPoints" */
 int ltrh_stage(ltrh_removerter* r, const char* name);
 

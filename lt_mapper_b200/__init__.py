@@ -6,3 +6,4 @@ context without libltr_b200.so or without an sm_90 GPU raises.
 """
 from . import binding  # noqa: F401
 from .binding import Context, LtrError, MODE_HD, MODE_ND, MODE_PD, SCANSIDE_MAP, SCANSIDE_SCAN_MINUS_MAP, reset_rimg_size  # noqa: F401
+from .binding import ICP_ITERATIONS, ICP_TRANSFORM, ICP_ABS_MSE, ICP_REL_MSE, ICP_NO_CORRESPONDENCES  # noqa: F401

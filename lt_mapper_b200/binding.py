@@ -15,6 +15,7 @@ _LIB = None
 
 MODE_HD, MODE_ND, MODE_PD = 0, 1, 2
 SCANSIDE_MAP, SCANSIDE_SCAN_MINUS_MAP = 0, 1   # ltr_scanside_criterion
+ICP_ITERATIONS, ICP_TRANSFORM, ICP_ABS_MSE, ICP_REL_MSE, ICP_NO_CORRESPONDENCES = 1, 2, 3, 4, 5   # ltr_icp_exit
 LTR_OK = 0
 
 
@@ -30,6 +31,12 @@ class Config(ctypes.Structure):
                 ("transform_order", ctypes.c_int32), ("keyframe_batch", ctypes.c_int32), ("fast_path", ctypes.c_int32)]
 
 
+class IcpParams(ctypes.Structure):
+    _fields_ = [("max_correspondence_distance", ctypes.c_double), ("max_iterations", ctypes.c_int32),
+                ("transformation_epsilon", ctypes.c_double), ("euclidean_fitness_epsilon", ctypes.c_double),
+                ("mse_threshold_absolute", ctypes.c_double), ("min_correspondences", ctypes.c_int32), ("source_leaf", ctypes.c_float)]
+
+
 EXPORTS = [
     "ltr_config_default", "ltr_create", "ltr_destroy", "ltr_last_error", "ltr_synchronize", "ltr_kernel_launches", "ltr_voxel_shortcuts", "ltr_memory_stats",
     "ltr_cloud_upload", "ltr_cloud_size", "ltr_cloud_download", "ltr_cloud_free", "ltr_cloud_copy", "ltr_cloud_concat", "ltr_cloud_slice",
@@ -37,7 +44,7 @@ EXPORTS = [
     "ltr_scanset_free", "ltr_scanset_concat_per_keyframe", "ltr_scanset_flatten", "ltr_poses_upload", "ltr_poses_free",
     "ltr_preclean", "ltr_merge_scans_global", "ltr_voxel_centroid", "ltr_voxel_centroid_per_keyframe", "ltr_voxel_grid", "ltr_voxel_grid_per_keyframe", "ltr_remove_pass", "ltr_scan_images_release",
     "ltr_flags_device_ptr", "ltr_flags_download", "ltr_flags_upload", "ltr_apply_partition", "ltr_parse_projected",
-    "ltr_knn_diff", "ltr_knn_split_cloud", "ltr_scanside_split", "ltr_scanside_stats", "ltr_debug_pixel_index", "ltr_debug_scan_rimg", "ltr_debug_fast_project", "ltr_debug_atan_sweep", "ltr_debug_margins", "ltr_reset_rimg_size", "ltr_last_pass_stats", "ltr_profile_get", "ltr_profile_reset", "ltr_timer_start", "ltr_timer_stop", "ltr_trace_dump",
+    "ltr_knn_diff", "ltr_knn_split_cloud", "ltr_scanside_split", "ltr_scanside_stats", "ltr_icp_params_default", "ltr_icp_refine", "ltr_knn_diff_refined", "ltr_debug_pixel_index", "ltr_debug_scan_rimg", "ltr_debug_fast_project", "ltr_debug_atan_sweep", "ltr_debug_margins", "ltr_reset_rimg_size", "ltr_last_pass_stats", "ltr_profile_get", "ltr_profile_reset", "ltr_timer_start", "ltr_timer_stop", "ltr_trace_dump",
     "ltr_pinned_alloc", "ltr_pinned_free", "ltr_nccl_unique_id", "ltr_nccl_init", "ltr_nccl_split", "ltr_nccl_info", "ltr_nccl_destroy", "ltr_nccl_version", "ltr_nccl_allreduce_flags",
     "ltr_nccl_allgather_clouds", "ltr_nccl_exchange_clouds", "ltr_nccl_voxel_centroid_merged", "ltr_nccl_allgather_i64", "ltr_nccl_max_f64", "ltr_nccl_barrier", "ltr_stream_handle",
 ]
@@ -101,6 +108,10 @@ def lib():
     L.ltr_knn_split_cloud.argtypes = [vp, i32, i32, i32, f32, P(i32), P(i32)]
     L.ltr_scanside_split.argtypes = [vp, i32, i32, i32, i32, i32, i32, f32, P(i32), P(i32)]
     L.ltr_scanside_stats.argtypes = [vp, vp]
+    L.ltr_icp_params_default.argtypes = [P(IcpParams)]
+    L.ltr_icp_params_default.restype = None
+    L.ltr_icp_refine.argtypes = [vp, i32, i32, i32, i32, P(IcpParams), vp, vp, vp, vp]
+    L.ltr_knn_diff_refined.argtypes = [vp, i32, i32, i32, i32, i32, f32, vp, vp, P(i32), P(i32)]
     L.ltr_debug_pixel_index.argtypes = [vp, vp, i64, i32, i32, vp, vp, vp, vp, vp]
     L.ltr_debug_scan_rimg.argtypes = [vp, i32, i32, ctypes.c_float, vp]
     L.ltr_debug_fast_project.argtypes = [vp, vp, i64, vp, f32, vp, vp]
@@ -358,6 +369,34 @@ class Context:
         """(static, dynamic) scan sets of ltr_scanside_split."""
         a, b = ctypes.c_int32(), ctypes.c_int32()
         self._ck(lib().ltr_scanside_split(self._h, scans, poses, pose_offset, map_, criterion, k, thr, ctypes.byref(a), ctypes.byref(b)))
+        return a.value, b.value
+
+    def icp_refine(self, scans, poses, target_down, pose_offset=0, **params):
+        """ltr_icp_refine: per keyframe (T (K, 4, 4) float32, fitness (K,) float64, iterations (K,) int32, exit reason (K,) int32).
+        Keyword arguments override fields of ltr_icp_params (defaults: the reference's values), e.g. max_iterations=5."""
+        prm = IcpParams()
+        lib().ltr_icp_params_default(ctypes.byref(prm))
+        for key, v in params.items():
+            if not hasattr(prm, key):
+                raise TypeError(f"unknown ICP parameter {key}")
+            setattr(prm, key, v)
+        K = self.scanset_info(scans)[0]
+        T = np.empty((K, 4, 4), np.float32)
+        fit = np.empty(K, np.float64)
+        it = np.empty(K, np.int32)
+        ex = np.empty(K, np.int32)
+        self._ck(lib().ltr_icp_refine(self._h, scans, poses, pose_offset, target_down, ctypes.byref(prm), T.ctypes.data, fit.ctypes.data,
+                                      it.ctypes.data, ex.ctypes.data))
+        return T, fit, it, ex
+
+    def knn_diff_refined(self, scans, poses, target, k, thr, T, accepted, pose_offset=0):
+        """(coexist, diff) scan sets of ltr_knn_diff_refined: keyframes with accepted[k] are moved by T[k] (float32 4x4) first."""
+        K = self.scanset_info(scans)[0]
+        Tf = np.ascontiguousarray(T, np.float32).reshape(K * 16)
+        acc = np.ascontiguousarray(accepted, np.uint8).reshape(K)
+        a, b = ctypes.c_int32(), ctypes.c_int32()
+        self._ck(lib().ltr_knn_diff_refined(self._h, scans, poses, pose_offset, target, k, thr, Tf.ctypes.data, acc.ctypes.data,
+                                            ctypes.byref(a), ctypes.byref(b)))
         return a.value, b.value
 
     def scanside_stats(self):

@@ -463,9 +463,30 @@ int Removerter::parseStaticScansViaProjection() {
 }
 
 int Removerter::extractLowDynPointsViaKnnDiff(Session& s, ltr_cloud target_map) {
-    // Session.cpp:395-402 (0.4 m downsample + ICP target) feed an ICP refinement that is hard-disabled (Session.cpp:551): skipped.
     ltr_scanset co, di;
-    CK(ltr_knn_diff(ctx, s.keyframe_scans_static_projected_, s.keyframe_poses_, 0, target_map, P.num_nn_points_within, P.dist_nn_points_within, &co, &di));
+    s.clear_icp_stats();
+    if (!useICPrefinement_) {
+        // Session.cpp:395-402 (0.4 m downsample + ICP target) only feed the refinement, which the reference switches off (Session.cpp:551)
+        CK(ltr_knn_diff(ctx, s.keyframe_scans_static_projected_, s.keyframe_poses_, 0, target_map, P.num_nn_points_within, P.dist_nn_points_within, &co, &di));
+    } else {
+        // Session.cpp:394-402: the ICP target is the other session's map at 0.4 m; partitionLowDynamicPointsOfScanByKnn (:549-584) registers
+        // every keyframe to it and keeps the registered scan iff getFitnessScore() < 1.0.  Multi-GPU: this rank's keyframe block against
+        // its replica of the target map, no collective.
+        int32_t K = 0;
+        int64_t npts = 0;
+        CK(ltr_scanset_info(ctx, s.keyframe_scans_static_projected_, &K, &npts));
+        s.icp_T16_.resize((size_t)K * 16); s.icp_fitness_.resize((size_t)K); s.icp_iterations_.resize((size_t)K); s.icp_exit_.resize((size_t)K);
+        s.icp_accepted_.resize((size_t)K);
+        ltr_cloud tgt = -1;
+        CK(ltr_voxel_centroid(ctx, target_map, 0.4f, &tgt));   // Session.cpp:400
+        const int rc = ltr_icp_refine(ctx, s.keyframe_scans_static_projected_, s.keyframe_poses_, 0, tgt, nullptr, s.icp_T16_.data(), s.icp_fitness_.data(),
+                                      s.icp_iterations_.data(), s.icp_exit_.data());
+        ltr_cloud_free(ctx, tgt);
+        CK(rc);
+        for (int32_t k = 0; k < K; ++k) s.icp_accepted_[(size_t)k] = s.icp_fitness_[(size_t)k] < 1.0 ? 1 : 0;   // Session.cpp:571
+        CK(ltr_knn_diff_refined(ctx, s.keyframe_scans_static_projected_, s.keyframe_poses_, 0, target_map, P.num_nn_points_within,
+                                P.dist_nn_points_within, s.icp_T16_.data(), s.icp_accepted_.data(), &co, &di));
+    }
     CK(set(&s.scans_knn_coexist_, co, true));
     CK(set(&s.scans_knn_diff_, di, true));
     return LTR_OK;
@@ -669,6 +690,7 @@ int Removerter::run_step3() {
 int Removerter::reset_to_step0() {
     CK(ltr_scan_images_release(ctx, 0));   // their storage stays for the next step's sets
     for (Session* s : {&central_sess_, &query_sess_}) {
+        s->clear_icp_stats();   // Step 2's results
         auto it = saved.find("OriginalNoisy" + s->sess_type_ + "MapGlobal");
         if (!owns(*s)) {   // session-split: everything held of the other session was derived after Step 0
             for (auto& kv : s->cloud_names()) if (*kv.second >= 0) { CK(ltr_cloud_free(ctx, *kv.second)); *kv.second = -1; }
@@ -710,6 +732,7 @@ int Removerter::cascade_promote_updated() {
     for (Session* s : {&central_sess_, &query_sess_}) {
         for (auto& kv : s->cloud_names()) if (*kv.second >= 0) { CK(ltr_cloud_free(ctx, *kv.second)); *kv.second = -1; }
         for (auto& kv : s->scanset_names()) if (*kv.second >= 0) { CK(ltr_scanset_free(ctx, *kv.second)); *kv.second = -1; }
+        s->clear_icp_stats();
     }
     for (auto& kv : saved) CK(ltr_cloud_free(ctx, kv.second));
     saved.clear();
@@ -804,6 +827,29 @@ int ltrh_scanside_removal(ltrh_removerter* r, int32_t map_sess, int32_t scan_ses
     Removerter& R = *r->R;
     R.err.clear();
     return R.scansideRemovalForEachScan(map_sess == 0 ? R.central_sess_ : R.query_sess_, scan_sess == 0 ? R.central_sess_ : R.query_sess_, criterion);
+}
+
+int ltrh_set_icp_refinement(ltrh_removerter* r, int32_t on) {
+    if (!r) return LTR_ERR_INVALID;
+    r->R->useICPrefinement_ = on != 0;
+    return LTR_OK;
+}
+
+int ltrh_icp_stats(ltrh_removerter* r, int32_t sess, int32_t capacity, int32_t* K_out, float* T16, double* fitness, int32_t* iterations,
+                   int32_t* exit_reason, uint8_t* accepted) {
+    if (!r || (sess != 0 && sess != 1) || !K_out) return LTR_ERR_INVALID;
+    const Session& S = sess == 0 ? r->R->central_sess_ : r->R->query_sess_;
+    const int32_t K = (int32_t)S.icp_fitness_.size();
+    *K_out = K;
+    if (capacity < K) return LTR_OK;   // a size query
+    for (int32_t k = 0; k < K; ++k) {
+        if (T16) for (int j = 0; j < 16; ++j) T16[16 * (size_t)k + j] = S.icp_T16_[16 * (size_t)k + j];
+        if (fitness) fitness[k] = S.icp_fitness_[(size_t)k];
+        if (iterations) iterations[k] = S.icp_iterations_[(size_t)k];
+        if (exit_reason) exit_reason[k] = S.icp_exit_[(size_t)k];
+        if (accepted) accepted[k] = S.icp_accepted_[(size_t)k];
+    }
+    return LTR_OK;
 }
 
 int ltrh_stage(ltrh_removerter* r, const char* name) {

@@ -32,6 +32,12 @@ public:
                 keyframe_scans_strong_pd_ = -1, keyframe_scans_strong_nd_ = -1, keyframe_scans_weak_nd_ = -1;
     // scan-side removal of this session's scans (the commented central_/query_scans_{static,dynamic}_ of Removerter.h)
     ltr_scanset scans_static_ = -1, scans_dynamic_ = -1;
+    // ICP refinement of the last extractLowDynPointsViaKnnDiff with useICPrefinement_ on (ltr_icp_refine), per keyframe of this rank
+    std::vector<float> icp_T16_;
+    std::vector<double> icp_fitness_;
+    std::vector<int32_t> icp_iterations_, icp_exit_;
+    std::vector<uint8_t> icp_accepted_;
+    void clear_icp_stats() { icp_T16_.clear(); icp_fitness_.clear(); icp_iterations_.clear(); icp_exit_.clear(); icp_accepted_.clear(); }
     // maps (Session.h:67-87)
     ltr_cloud map_global_orig_ = -1, map_global_curr_ = -1, map_global_curr_static_ = -1, map_global_curr_dynamic_ = -1;
     ltr_cloud map_global_updated_ = -1, map_global_updated_strong_ = -1;
@@ -78,7 +84,7 @@ public:
 
     // ---- Session methods (Session.cpp) ----
     int parseScansViaProjection(Session& s, ltr_cloud map, ltr_scanset* vec_to_store);     // Session.cpp:348-360
-    int extractLowDynPointsViaKnnDiff(Session& s, ltr_cloud target_map);                   // Session.cpp:393-427
+    int extractLowDynPointsViaKnnDiff(Session& s, ltr_cloud target_map);                   // Session.cpp:393-427, 549-584
     int extractHighDynPointsViaKnnDiff(Session& s, ltr_cloud target_map);                  // Session.cpp:487-504
     int constructGlobalNDMap(Session& s);                                                  // Session.cpp:430-435
     int constructGlobalPDMap(Session& s);                                                  // Session.cpp:437-445
@@ -115,6 +121,7 @@ public:
     int fail(int code, const std::string& msg);
 
     ltrh_params P;
+    bool useICPrefinement_ = false;   // Session.cpp:551 (`bool useICPrefinement { false }`), set by ltrh_set_icp_refinement
     ltr_ctx* ctx = nullptr;
     ltr_comm comm{};          // legacy caller-supplied hooks (host-memory tests); superseded by the native transport when nccl_world >= 0
     bool has_comm = false;

@@ -152,8 +152,7 @@ __global__ void __launch_bounds__(128) knn_scan_label_kernel(PtrView scans, cons
     int lo = 0, hi = K;
     while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (off[mid] <= i) lo = mid; else hi = mid; }
     float x = scans.x[i], y = scans.y[i], z = scans.z[i];
-    if (!ext_identity) transform_point(ext, order, x, y, z, &x, &y, &z);                              // utility.cpp:164 with base2lidar (as written)
-    transform_point(poses + (size_t)(pose_offset + lo) * 24 + 12, order, x, y, z, &x, &y, &z);        // utility.cpp:165
+    knn_scan_to_global(poses + (size_t)(pose_offset + lo) * 24 + 12, ext, ext_identity, order, &x, &y, &z);   // utility.cpp:164-165, base2lidar as written
     gx[i] = x; gy[i] = y; gz[i] = z;
     label[i] = small_target.n > 0 ? knn_label_small(s_t, (int)small_target.n, x, y, z, k, thr) : knn_label_dispatch(g, cell_start, sorted, x, y, z, k, thr);
 }
@@ -167,10 +166,7 @@ __global__ void __launch_bounds__(256) knn_relocalise_kernel(const float* __rest
     if (i >= n) return;
     int lo = 0, hi = K;
     while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (off[mid] <= i) lo = mid; else hi = mid; }
-    float x = gx[i], y = gy[i], z = gz[i];
-    transform_point(poses + (size_t)(pose_offset + lo) * 24, order, x, y, z, &x, &y, &z);   // utility.cpp:198
-    if (!ext_identity) transform_point(ext, order, x, y, z, &x, &y, &z);                    // utility.cpp:199
-    ox[i] = x; oy[i] = y; oz[i] = z;
+    map_to_sensor(poses + (size_t)(pose_offset + lo) * 24, ext, ext_identity, order, gx[i], gy[i], gz[i], &ox[i], &oy[i], &oz[i]);   // utility.cpp:198-199
 }
 
 // sm_90a: 32 registers and a 44 B spill (L1-resident) at full occupancy.  __launch_bounds__(128, 12) removes the spill (40 registers)

@@ -159,6 +159,14 @@ LTR_DEV void map_to_sensor(const double* __restrict__ inv_pose, const double* __
     if (!ext_identity) transform_point(ext, order, *lx, *ly, *lz, lx, ly, lz);
 }
 
+// local2global of a scan point as the kNN diff moves it (Session.cpp:545 passes base2lidar; utility.cpp:164-165): the extrinsic unless it is
+// exactly the identity (ext: base2lidar rows 0..2), then the pose (rows 0..2).  Its inverse is map_to_sensor with the inverse pose.
+LTR_DEV void knn_scan_to_global(const double* __restrict__ pose, const double* __restrict__ ext, int ext_identity, int order, float* x, float* y,
+                                float* z) {
+    if (!ext_identity) transform_point(ext, order, *x, *y, *z, x, y, z);
+    transform_point(pose, order, *x, *y, *z, x, y, z);
+}
+
 // FLANN L2_Simple<float> squared distance: ((dx*dx) + dy*dy) + dz*dz with dx = query - point
 LTR_DEV float l2_simple(float qx, float qy, float qz, float px, float py, float pz) {
     const float dx = fs(qx, px), dy = fs(qy, py), dz = fs(qz, pz);

@@ -40,6 +40,7 @@
 #include "ltr_internal.cuh"
 #include "ref_math.cuh"
 #include "device_util.cuh"
+#include "sparse_grid.cuh"
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
@@ -49,14 +50,8 @@ namespace ltr {
 namespace {
 
 constexpr int kMaxK = 16;
-constexpr int kCellBits = 17;                 // per axis: indices < 2^17
-constexpr int kSegShift = 3 * kCellBits;      // 51: segment above the three cell indices
-constexpr int kMaxSegments = 1 << (64 - kSegShift);   // 8192 keyframes per launch
-constexpr int kMaxDim = (1 << kCellBits) - 1;
-constexpr double kCell0 = 0.25;               // finest cell side [m]
-constexpr double kLevelRatio = 4.0;
-constexpr int kMaxLevels = 8;
-constexpr int kFinalDim = 10;                 // a level of at most this many cells per axis is searched without a shell bound
+constexpr int kSegShift = kGridSegShift;
+constexpr int kMaxSegments = kGridMaxSegments;   // 8192 keyframes per launch
 constexpr int kBoundedShells = 2;
 constexpr int64_t kChunkPoints = (int64_t)1 << 24;
 
@@ -64,32 +59,6 @@ int64_t chunk_points() {
     int64_t n = kChunkPoints;
     if (const char* e = std::getenv("LTR_SCANSIDE_CHUNK_POINTS")) if (*e) n = std::min<int64_t>(std::max<int64_t>(std::atoll(e), 1), (int64_t)1 << 30);
     return n;
-}
-
-struct Level {
-    double origin[3];
-    double inv_cell, cell;          // cell = 1 / inv_cell
-    int dim[3];
-    int final_level;
-    const unsigned long long* keys; // sorted unique (segment, cell) keys
-    const uint32_t* start;          // first point of each cell, [ncell] = number of points
-    const float4* pts;              // points in key order
-    const uint32_t* seg_first;      // cells of segment s: [seg_first[s], seg_first[s + 1])
-};
-
-struct LevelBuf {
-    Level L{};
-    void* block = nullptr;
-};
-
-__device__ __forceinline__ unsigned long long cell_key(int seg, long long cx, long long cy, long long cz) {
-    return ((unsigned long long)seg << kSegShift) | ((unsigned long long)cz << (2 * kCellBits)) | ((unsigned long long)cy << kCellBits) |
-           (unsigned long long)cx;
-}
-
-__device__ __forceinline__ long long cell_index(double v, double origin, double inv_cell) {
-    const double t = fmin(fmax((v - origin) * inv_cell, -0x1p40), 0x1p40);
-    return (long long)floor(t);
 }
 
 // ---- level build -------------------------------------------------------------------------------------------------------------------
@@ -121,7 +90,7 @@ __global__ void __launch_bounds__(256) level_compact_kernel(PtrView p, const uns
     if (head[i]) { ukeys[pos[i]] = keys[i]; start[pos[i]] = (uint32_t)i; }
     if (i == n - 1) { const uint32_t m = pos[i] + head[i]; start[m] = (uint32_t)n; *ncell = m; }
     const uint32_t j = idx[i];
-    pts[i] = make_float4(p.x[j], p.y[j], p.z[j], 0.0f);
+    pts[i] = make_float4(p.x[j], p.y[j], p.z[j], __uint_as_float(j));
 }
 
 __global__ void level_segments_kernel(const unsigned long long* __restrict__ ukeys, const uint32_t* __restrict__ ncell, int nseg,
@@ -136,7 +105,9 @@ __global__ void level_segments_kernel(const unsigned long long* __restrict__ uke
     seg_first[s] = lo;
 }
 
-// Grid level of cell side `cell` over the points of p (segments from off, or one segment), box [mn, mx] of p.
+}  // namespace
+
+// sparse_grid.cuh
 int build_level(ltr_ctx* ctx, PtrView p, const int64_t* d_off, int nseg, const float mn[3], const float mx[3], double cell, bool final_level,
                 LevelBuf* out) {
     Level L{};
@@ -192,6 +163,8 @@ int build_level(ltr_ctx* ctx, PtrView p, const int64_t* d_off, int nseg, const f
     blk = nullptr;   // ownership moves to out
     return LTR_OK;
 }
+
+namespace {
 
 // ---- exact k-NN ----------------------------------------------------------------------------------------------------------------------
 template <int K>
@@ -308,37 +281,6 @@ int launch_exact_knn(ltr_ctx* ctx, int k, const Level& L, PtrView q, const int64
     LTR_LAUNCH_CHECK(ctx);
     return LTR_OK;
 }
-
-// The levels of one target, finest first, built as far as some query needs them.
-struct Pyramid {
-    PtrView pts{nullptr, nullptr, nullptr, nullptr, 0};
-    const int64_t* d_off = nullptr;
-    int nseg = 1;
-    float mn[3], mx[3];
-    double cell0 = kCell0;
-    std::vector<LevelBuf> levels;
-
-    void init(PtrView p, const int64_t* off, int ns, const float lo[3], const float hi[3]) {
-        pts = p; d_off = off; nseg = ns;
-        double ext = 0.0;
-        for (int d = 0; d < 3; ++d) { mn[d] = lo[d]; mx[d] = hi[d]; ext = std::max(ext, (double)hi[d] - (double)lo[d]); }
-        cell0 = std::max(kCell0, ext / (double)(kMaxDim - 4));   // indices < 2^17 on the finest level
-    }
-    int get(ltr_ctx* ctx, int l, const Level** out) {
-        while ((int)levels.size() <= l) {
-            const int m = (int)levels.size();
-            const double cell = cell0 * std::pow(kLevelRatio, m);
-            int dmax = 0;
-            for (int d = 0; d < 3; ++d) dmax = std::max(dmax, (int)std::floor(((double)mx[d] - (double)mn[d]) / cell) + 3);
-            LevelBuf b;
-            LTR_TRY(build_level(ctx, pts, d_off, nseg, mn, mx, cell, dmax <= kFinalDim || m == kMaxLevels - 1, &b));
-            levels.push_back(b);
-        }
-        *out = &levels[(size_t)l].L;
-        return LTR_OK;
-    }
-    void release(ltr_ctx* ctx) { for (auto& b : levels) if (b.block) dev_free(ctx, b.block); levels.clear(); }
-};
 
 // avg[i] for every query of q against the target pyramid; *unsettled = queries the bounded pass on the finest level left over.
 int exact_avg_all(ltr_ctx* ctx, Pyramid& T, int k, PtrView q, const int64_t* q_off, int nseg, float* avg, uint32_t* list_a,

@@ -41,7 +41,7 @@ class Comm(ctypes.Structure):
 
 
 HOST_EXPORTS = ["ltrh_params_default", "ltrh_create", "ltrh_destroy", "ltrh_last_error", "ltrh_set_comm", "ltrh_context", "ltrh_comm_init_nccl", "ltrh_owns_session", "ltrh_invert_poses",
-                "ltrh_load_session", "ltrh_load_session_raw", "ltrh_run_step0", "ltrh_run_step12", "ltrh_run_step3", "ltrh_reset_to_step0", "ltrh_cascade_promote_updated", "ltrh_scanside_removal", "ltrh_stage", "ltrh_cloud",
+                "ltrh_load_session", "ltrh_load_session_raw", "ltrh_run_step0", "ltrh_run_step12", "ltrh_run_step3", "ltrh_reset_to_step0", "ltrh_cascade_promote_updated", "ltrh_scanside_removal", "ltrh_set_icp_refinement", "ltrh_icp_stats", "ltrh_stage", "ltrh_cloud",
                 "ltrh_scanset", "ltrh_timing", "ltrh_log_count", "ltrh_log_get", "ltrh_io_last_error", "ltrh_io_read_pcd", "ltrh_io_write_pcd",
                 "ltrh_io_read_poses", "ltrh_io_parse_keyframes", "ltrh_io_parse_keyframes_in_roi", "ltrh_io_voxel_grid", "ltrh_io_voxel_grid_scans", "ltrh_io_yaml_get"]
 
@@ -75,6 +75,8 @@ def host_lib():
     for f in ("ltrh_run_step0", "ltrh_run_step12", "ltrh_run_step3", "ltrh_reset_to_step0", "ltrh_cascade_promote_updated"):
         getattr(L, f).argtypes = [vp]
     L.ltrh_scanside_removal.argtypes = [vp, i32, i32, i32]
+    L.ltrh_set_icp_refinement.argtypes = [vp, i32]
+    L.ltrh_icp_stats.argtypes = [vp, i32, i32, P(i32), vp, vp, vp, vp, vp]
     L.ltrh_stage.argtypes = [vp, ctypes.c_char_p]
     L.ltrh_cloud.argtypes = [vp, ctypes.c_char_p, i32, P(i32)]
     L.ltrh_scanset.argtypes = [vp, ctypes.c_char_p, i32, P(i32)]
@@ -326,6 +328,23 @@ class Removerter:
     def scanside_removal(self, map_sess, scan_sess, criterion=0):
         """scansideRemovalForEachScan (ltrh_scanside_removal): fills the scan sets "scans_static_" / "scans_dynamic_" of scan_sess."""
         self._ck(host_lib().ltrh_scanside_removal(self._h, map_sess, scan_sess, criterion))
+
+    def set_icp_refinement(self, on=True):
+        """Session::partitionLowDynamicPointsOfScanByKnn's ICP refinement for later Step 2 runs (ltrh_set_icp_refinement; off by default)."""
+        self._ck(host_lib().ltrh_set_icp_refinement(self._h, 1 if on else 0))
+
+    def icp_stats(self, sess):
+        """This rank's refinement of session `sess` in the last Step 2 (ltrh_icp_stats): dict of per-keyframe arrays T (K, 4, 4) float32,
+        fitness, iterations, exit (ltr_icp_exit) and accepted (bool); K = 0 when the step ran without refinement."""
+        K = ctypes.c_int32()
+        self._ck(host_lib().ltrh_icp_stats(self._h, sess, 0, ctypes.byref(K), None, None, None, None, None))
+        n = K.value
+        T = np.empty((n, 4, 4), np.float32); fit = np.empty(n, np.float64); it = np.empty(n, np.int32); ex = np.empty(n, np.int32)
+        acc = np.empty(n, np.uint8)
+        if n:
+            self._ck(host_lib().ltrh_icp_stats(self._h, sess, n, ctypes.byref(K), T.ctypes.data, fit.ctypes.data, it.ctypes.data, ex.ctypes.data,
+                                               acc.ctypes.data))
+        return {"T": T, "fitness": fit, "iterations": it, "exit": ex, "accepted": acc.astype(bool)}
 
     def stage(self, name):
         self._ck(host_lib().ltrh_stage(self._h, name.encode()))
