@@ -34,14 +34,11 @@
 // The partition (ltr_knn_diff_refined) then moves scan_global by final in f32 when the caller accepts the keyframe (the reference: fitness
 // < 1.0) and runs ltr_knn_diff's labelling and global2local on it, so a keyframe that is not accepted gives ltr_knn_diff's bytes.
 //
-// Nearest neighbour with index.  tgt goes into the sparse grid levels of scanside.cu (sparse_grid.cuh, one segment, built once per call:
-// the target is fixed across iterations).  A query searches shell by shell; on a level it stops after shell s >= 1 when its current
-// smallest distance D satisfies D <= ((s - 2^-6) c)^2 (1 - 2^-20), or when the block holds every cell.  scanside.cu's header shows that
-// every point outside the block then has a computed distance STRICTLY greater than ((s - 2^-6) c)^2 (1 - 2^-20) >= D, so every point at
-// distance D is inside the block and has been evaluated: the lowest index among them is the lowest index overall.  (scanside.cu's
-// early stop at D = 0 in shell 0 is not used here: an underflowed 0 can sit in the next cell, and its index may be lower.)  Bounded
-// levels give up after kNnShells shells and the query moves to the next, 4x coarser level; the coarsest searches until the rule holds.
-// Which level answers changes the cost only.
+// Nearest neighbour with index.  tgt goes into the sparse grid levels of sparse_grid.cuh (one segment, built once per call: the target is
+// fixed across iterations).  A query searches shell by shell; on a level it stops after shell s >= 1 when its current smallest distance D
+// satisfies D <= ((s - 2^-6) c)^2 (1 - 2^-20), or when the block holds every cell, but not at D = 0 in shell 0.  sparse_grid.cuh's header
+// proves that the lowest index among the points at distance D is then the lowest overall.  Bounded levels give up after kNnShells
+// shells and the query moves to the next, 4x coarser level; the coarsest searches until the rule holds.
 //
 // Memory: the global scans (16 B/point) while the source is voxelised, the 0.4 m source (16 B per source point), tgt's grid levels (28 B
 // per tgt point each), and per launch of at most LTR_ICP_CHUNK_POINTS source points (environment; default 2^24, a keyframe is never
@@ -49,12 +46,10 @@
 // returned before the call ends.
 #include "ltr_internal.cuh"
 #include "ref_math.cuh"
-#include "device_util.cuh"
 #include "sparse_grid.cuh"
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
-#include <cstdlib>
 
 namespace ltr {
 
@@ -65,12 +60,6 @@ constexpr int kJacobiSweeps = 10;
 constexpr int kNnShells = 2;
 constexpr int64_t kChunkPoints = (int64_t)1 << 24;
 constexpr int kExitNoCorrespondences = LTR_ICP_NO_CORRESPONDENCES;
-
-int64_t chunk_points() {
-    int64_t n = kChunkPoints;
-    if (const char* e = std::getenv("LTR_ICP_CHUNK_POINTS")) if (*e) n = std::min<int64_t>(std::max<int64_t>(std::atoll(e), 1), (int64_t)1 << 30);
-    return n;
-}
 
 struct Levels {
     Level L[kGridMaxLevels];
@@ -86,70 +75,23 @@ LTR_DEV double ds(double a, double b) { return __dsub_rn(a, b); }
 LTR_DEV double dd(double a, double b) { return __ddiv_rn(a, b); }
 
 // ---- exact 1-NN with the lowest index on ties (file header) --------------------------------------------------------------------------
-LTR_DEV void nn_row(const Level& L, uint32_t c0, uint32_t c1, long long xa, long long xb, long long y, long long z, float qx, float qy, float qz,
-                    float& bd, uint32_t& bi) {
-    const unsigned long long ka = cell_key(0, xa, y, z), kb = cell_key(0, xb, y, z);
-    uint32_t lo = c0, hi = c1;
-    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (L.keys[mid] < ka) lo = mid + 1; else hi = mid; }
-    for (uint32_t ci = lo; ci < c1 && L.keys[ci] <= kb; ++ci) {
-        const uint32_t e = L.start[ci + 1];
-        for (uint32_t p = L.start[ci]; p < e; ++p) {
-            const float4 t = L.pts[p];
-            const float d = l2_simple(qx, qy, qz, t.x, t.y, t.z);
-            const uint32_t idx = __float_as_uint(t.w);
-            if (d < bd || (d == bd && idx < bi)) { bd = d; bi = idx; }
-        }
+// the shell search's accumulator; its stop rule is in sparse_grid.cuh's header
+struct Nearest {
+    float d;
+    uint32_t i;
+    LTR_DEV void push(float v, const float4& t) {
+        const uint32_t idx = __float_as_uint(t.w);
+        if (v < d || (v == d && idx < i)) { d = v; i = idx; }
     }
-}
-
-// false: not settled within kNnShells shells on a bounded level
-LTR_DEV bool nn_level(const Level& L, float qx, float qy, float qz, float* d_out, uint32_t* i_out) {
-    float bd = __int_as_float(0x7f800000);
-    uint32_t bi = 0xffffffffu;
-    const float q[3] = {qx, qy, qz};
-    long long c[3], s0 = 0, cover = 0;
-#pragma unroll
-    for (int d = 0; d < 3; ++d) {
-        c[d] = cell_index((double)q[d], L.origin[d], L.inv_cell);
-        const long long hi = (long long)L.dim[d] - 1;
-        s0 = max(s0, max(-c[d], c[d] - hi));
-        cover = max(cover, max(c[d], hi - c[d]));
-    }
-    const uint32_t c0 = L.seg_first[0], c1 = L.seg_first[1];
-    for (long long s = s0;; ++s) {
-        if (!L.final_level && s > kNnShells) return false;
-        const long long z0 = max(c[2] - s, 0ll), z1 = min(c[2] + s, (long long)L.dim[2] - 1);
-        const long long y0 = max(c[1] - s, 0ll), y1 = min(c[1] + s, (long long)L.dim[1] - 1);
-        const long long xa = max(c[0] - s, 0ll), xb = min(c[0] + s, (long long)L.dim[0] - 1);
-        for (long long z = z0; z <= z1; ++z) {
-            const bool zface = z == c[2] - s || z == c[2] + s;
-            for (long long y = y0; y <= y1; ++y) {
-                if (zface || y == c[1] - s || y == c[1] + s) {
-                    if (xa <= xb) nn_row(L, c0, c1, xa, xb, y, z, qx, qy, qz, bd, bi);
-                } else {
-                    if (c[0] - s >= 0 && c[0] - s < L.dim[0]) nn_row(L, c0, c1, c[0] - s, c[0] - s, y, z, qx, qy, qz, bd, bi);
-                    if (s > 0 && c[0] + s >= 0 && c[0] + s < L.dim[0]) nn_row(L, c0, c1, c[0] + s, c[0] + s, y, z, qx, qy, qz, bd, bi);
-                }
-            }
-        }
-        if (s >= cover) break;
-        if (bi != 0xffffffffu && s > 0) {
-            const double r = ((double)s - 0x1p-6) * L.cell;
-            if ((double)bd <= r * r * (1.0 - 0x1p-20)) break;
-        }
-    }
-    *d_out = bd;
-    *i_out = bi;
-    return true;
-}
+    LTR_DEV bool settled(long long s, double cell) const { return i != 0xffffffffu && s > 0 && (double)d <= shell_bound(s, cell); }
+};
 
 LTR_DEV void nn1(const Levels& T, float qx, float qy, float qz, float* d, uint32_t* idx) {
-    for (int l = 0; l < T.n; ++l)
-        if (nn_level(T.L[l], qx, qy, qz, d, idx)) return;
+    for (int l = 0; l < T.n; ++l) {
+        Nearest b{__int_as_float(0x7f800000), 0xffffffffu};
+        if (shell_search(T.L[l], 0, qx, qy, qz, kNnShells, b)) { *d = b.d; *idx = b.i; return; }
+    }
 }
-
-// ((m0 x + m1 y) + m2 z) + m3 in f32, m = one row of a row-major float 4x4
-LTR_DEV float frow(const float* m, float x, float y, float z) { return fa(fa(fa(fm(m[0], x), fm(m[1], y)), fm(m[2], z)), m[3]); }
 
 // ---- rigid estimate (file header, step 3) -------------------------------------------------------------------------------------------
 // H[3a + b] = sum (p_a - p_mean_a)(q_b - q_mean_b); writes R (row-major 3x3) and t in double.
@@ -361,38 +303,6 @@ __global__ void __launch_bounds__(kIcpThreads) icp_kernel(Levels T, PtrView tgt,
     }
 }
 
-// local2global as ltr_knn_diff moves a scan (knn.cu, knn_scan_label_kernel): base2lidar as written at Session.cpp:545, then the pose;
-// with refine != null the points of an accepted keyframe are then moved by its float 4x4 in f32 (Session.cpp:565)
-__global__ void __launch_bounds__(256) icp_global_kernel(PtrView in, const int64_t* __restrict__ off, int K, const double* __restrict__ poses,
-                                                         int pose_offset, const double* __restrict__ ext, int ext_identity, int order,
-                                                         const float* __restrict__ T16, const uint8_t* __restrict__ accept, float* __restrict__ gx,
-                                                         float* __restrict__ gy, float* __restrict__ gz) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= in.n) return;
-    const int k = find_kf(off, K, i);
-    float x = in.x[i], y = in.y[i], z = in.z[i];
-    knn_scan_to_global(poses + (size_t)(pose_offset + k) * 24 + 12, ext, ext_identity, order, &x, &y, &z);
-    if (accept && accept[k]) {
-        const float* m = T16 + 16 * (size_t)k;
-        const float nx = frow(m, x, y, z), ny = frow(m + 4, x, y, z), nz = frow(m + 8, x, y, z);
-        x = nx; y = ny; z = nz;
-    }
-    gx[i] = x; gy[i] = y; gz[i] = z;
-}
-
-// global2local of both partitions (Session.cpp:603-604)
-__global__ void __launch_bounds__(256) icp_local_kernel(const float* __restrict__ gx, const float* __restrict__ gy, const float* __restrict__ gz,
-                                                        int64_t n, const int64_t* __restrict__ off, int K, const double* __restrict__ poses,
-                                                        int pose_offset, const double* __restrict__ ext, int ext_identity, int order, DevCloud out) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int k = find_kf(off, K, i);
-    map_to_sensor(poses + (size_t)(pose_offset + k) * 24, ext, ext_identity, order, gx[i], gy[i], gz[i], &out.x()[i], &out.y()[i], &out.z()[i]);
-}
-
-struct ScanSetGuard { ltr_ctx* c; ltr_scanset h = -1; ~ScanSetGuard() { if (h >= 0) ltr_scanset_free(c, h); } };
-struct CloudGuard { ltr_ctx* c; ltr_cloud h = -1; ~CloudGuard() { if (h >= 0) ltr_cloud_free(c, h); } };
-
 int check_scans_poses(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_offset, DevScanSet** sp, DevPoses** pp) {
     LTR_TRY(scanset_get(ctx, scans_h, sp));
     LTR_TRY(poses_get(ctx, poses_h, pp));
@@ -453,15 +363,12 @@ int ltr_icp_refine(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t
         for (int j = 0; j < 16; ++j) hT[16 * (size_t)k + j] = (j % 5 == 0) ? 1.0f : 0.0f;
     if (scans.pts.n > 0) {
         // 1. the global scans and their per-keyframe 0.4 m centroids
-        ScanSetGuard g_glob{ctx}, g_src{ctx};
+        ScanSetOwner g_glob(ctx), g_src(ctx);
         LTR_TRY(scanset_new(ctx, scans.h_off, &g_glob.h));
-        DevCloud g = ctx->scansets[g_glob.h].pts;
-        const int64_t n = scans.pts.n;
-        icp_global_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(view(scans.pts), scans.d_off, K, poses.d, pose_offset, ctx->d_ext,
-                                                                              ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, nullptr, nullptr,
-                                                                              g.x(), g.y(), g.z());
-        LTR_LAUNCH_CHECK(ctx);
-        LTR_CUDA(ctx, cudaMemcpyAsync(g.i(), scans.pts.i(), (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
+        const DevCloud g = ctx->scansets[g_glob.h].pts;
+        // scan_global as ltr_knn_diff moves it: base2lidar, then the pose
+        LTR_TRY(scans_to_global(ctx, scans, 0, scans.pts.n, poses.d + (size_t)pose_offset * 24, ctx->ext_identity ? nullptr : ctx->d_ext, g.x(),
+                                g.y(), g.z(), g.i()));
         {
             float mn[3], mx[3];
             uint32_t nonfinite = 0;
@@ -469,32 +376,23 @@ int ltr_icp_refine(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t
             if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite scan coordinates (%u points)", nonfinite);
         }
         LTR_TRY(ltr_voxel_centroid_per_keyframe(ctx, g_glob.h, P.source_leaf, &g_src.h));
-        ltr_scanset_free(ctx, g_glob.h);
-        g_glob.h = -1;
+        g_glob.reset();
         const DevScanSet src = ctx->scansets[g_src.h];
         // 2. the target's grid levels, all of them: every iteration searches them
-        Pyramid pyr;
-        struct PyrGuard { ltr_ctx* c; Pyramid* p; ~PyrGuard() { p->release(c); } } g_pyr{ctx, &pyr};
+        Pyramid pyr(ctx);
         pyr.init(view(tgt), nullptr, 1, tmn, tmx);
         Levels lv{};
         for (int l = 0;; ++l) {
             const Level* L;
-            LTR_TRY(pyr.get(ctx, l, &L));
+            LTR_TRY(pyr.get(l, &L));
             lv.L[l] = *L;
             lv.n = l + 1;
             if (L->final_level) break;
         }
-        // 3. keyframe chunks of at most chunk_points() source points, one CTA per keyframe
-        const int64_t cap = chunk_points();
-        std::vector<int> kf_cut{0};
-        for (int kf = 0; kf < K;) {
-            int e = kf + 1;
-            while (e < K && src.h_off[e + 1] - src.h_off[kf] <= cap) ++e;
-            kf_cut.push_back(e);
-            kf = e;
-        }
+        // 3. keyframe chunks of at most LTR_ICP_CHUNK_POINTS source points, one CTA per keyframe
         int64_t max_chunk = 0;
-        for (size_t c = 0; c + 1 < kf_cut.size(); ++c) max_chunk = std::max(max_chunk, src.h_off[kf_cut[c + 1]] - src.h_off[kf_cut[c]]);
+        const std::vector<int> kf_cut = plan_keyframe_chunks(src.h_off, env_points("LTR_ICP_CHUNK_POINTS", kChunkPoints, (int64_t)1 << 30), K,
+                                                             &max_chunk);
         if (max_chunk >= ((int64_t)1 << 31)) return fail(ctx, LTR_ERR_UNSUPPORTED, "a keyframe of %lld source points", (long long)max_chunk);
         auto pad = [](size_t v) { return (v + 255) / 256 * 256; };
         const size_t b_work = pad((size_t)std::max<int64_t>(max_chunk, 1) * 16), b_corr = pad((size_t)std::max<int64_t>(max_chunk, 1) * 4);
@@ -542,58 +440,8 @@ int ltr_knn_diff_refined(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, i
     if (!ctx) return LTR_ERR_INVALID;
     DevScanSet* sp;
     DevPoses* pp;
-    DevCloud* tp;
-    LTR_TRY(check_scans_poses(ctx, scans_h, poses_h, pose_offset, &sp, &pp));
-    LTR_TRY(cloud_get(ctx, target_h, &tp));
-    if (k < 1 || k > 16) return fail(ctx, LTR_ERR_UNSUPPORTED, "k = %d outside [1, 16]", k);
-    if (!(thr > 0.0f)) return fail(ctx, LTR_ERR_INVALID, "threshold must be positive");
-    if (tp->n < 1) return fail(ctx, LTR_ERR_UNSUPPORTED, "empty target map (PCL's nearestKSearch asserts on an empty tree)");
-    const DevScanSet scans = *sp;
-    const DevPoses poses = *pp;
-    const DevCloud target = *tp;
-    const int K = scans.K;
-    const int64_t n = scans.pts.n;
-    if (K > 0 && (!T16 || !accepted)) return fail(ctx, LTR_ERR_INVALID, "null transforms or accept mask");
-    if (n == 0) {
-        std::vector<int64_t> off((size_t)K + 1, 0);
-        if (out_coexist) LTR_TRY(scanset_new(ctx, off, out_coexist));
-        if (out_diff) LTR_TRY(scanset_new(ctx, off, out_diff));
-        return LTR_OK;
-    }
-    KnnTarget kt;
-    void* kt_block = nullptr;
-    ScratchGuard g_kt(ctx, &kt_block);
-    LTR_TRY(knn_target_build(ctx, target, k, thr, &kt, &kt_block));
-    void* p = nullptr;
-    ScratchGuard g_p(ctx, &p);
-    const size_t b_g = ((size_t)n * 12 + 255) / 256 * 256, b_T = ((size_t)K * 64 + 255) / 256 * 256;
-    LTR_TRY(dev_alloc(ctx, &p, b_g + b_T + (size_t)K + (size_t)n));
-    float* gx = (float*)p;
-    float* gy = gx + n;
-    float* gz = gy + n;
-    float* dT = (float*)((char*)p + b_g);
-    uint8_t* dacc = (uint8_t*)p + b_g + b_T;
-    uint8_t* label = dacc + K;
-    std::vector<uint8_t> acc((size_t)K);
-    for (int j = 0; j < K; ++j) acc[j] = accepted[j] ? 1 : 0;
-    LTR_CUDA(ctx, cudaMemcpyAsync(dT, T16, (size_t)K * 64, cudaMemcpyHostToDevice, ctx->stream));
-    LTR_CUDA(ctx, cudaMemcpyAsync(dacc, acc.data(), (size_t)K, cudaMemcpyHostToDevice, ctx->stream));
-    const int ext_id = ctx->ext_identity ? 1 : 0, order = ctx->cfg.transform_order;
-    icp_global_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(view(scans.pts), scans.d_off, K, poses.d, pose_offset, ctx->d_ext, ext_id,
-                                                                          order, dT, dacc, gx, gy, gz);
-    LTR_LAUNCH_CHECK(ctx);
-    LTR_TRY(knn_target_label(ctx, kt, PtrView{gx, gy, gz, nullptr, n}, k, thr, label));
-    g_kt.release();
-    CloudGuard g_sc{ctx};
-    LTR_TRY(cloud_new(ctx, n, &g_sc.h));
-    const DevCloud sc = ctx->clouds[g_sc.h];
-    icp_local_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(gx, gy, gz, n, scans.d_off, K, poses.d, pose_offset, ctx->d_ext, ext_id,
-                                                                         order, sc);
-    LTR_LAUNCH_CHECK(ctx);
-    LTR_CUDA(ctx, cudaMemcpyAsync(sc.i(), scans.pts.i(), (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
-    DevScanSet set = scans;
-    set.pts = sc;
-    return split_scanset_by_flag(ctx, set, label, out_coexist, out_diff);
+    LTR_TRY(check_scans_poses(ctx, scans_h, poses_h, pose_offset, &sp, &pp));   // this entry checks the pose range before k and thr
+    return knn_diff(ctx, scans_h, poses_h, pose_offset, target_h, k, thr, true, T16, accepted, out_coexist, out_diff);
 }
 
 }  // extern "C"

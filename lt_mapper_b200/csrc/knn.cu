@@ -13,6 +13,7 @@
 // ((dx*dx) + dy*dy) + dz*dz in f32, dx = query - point, no FMA.
 #include "ltr_internal.cuh"
 #include "ref_math.cuh"
+#include "device_util.cuh"
 #include <algorithm>
 #include <cmath>
 
@@ -138,35 +139,29 @@ __device__ __forceinline__ uint8_t knn_label_dispatch(const Grid& g, const uint3
     }
 }
 
-// scans: local -> (base2lidar as written at Session.cpp:545) -> pose => global query; label
-__global__ void __launch_bounds__(128) knn_scan_label_kernel(PtrView scans, const int64_t* __restrict__ off, int K, const double* __restrict__ poses,
-                                                             int pose_offset, const double* __restrict__ ext, int ext_identity, int order, Grid g,
-                                                             const uint32_t* __restrict__ cell_start, const float4* __restrict__ sorted, int k,
-                                                             float thr, uint8_t* __restrict__ label, float* __restrict__ gx, float* __restrict__ gy,
-                                                             float* __restrict__ gz, PtrView small_target) {
+// scans: local -> (base2lidar as written at Session.cpp:545) -> pose => global query, then, with T16 != null, the points of an accepted
+// keyframe moved by its float 4x4 in f32 (Session.cpp:565); label.  sm_90a: 40 registers, no spill, 12 CTAs per SM.  The minimum of 12
+// CTAs keeps that allocation: with the bare bound ptxas picks 32 registers and a 44 B spill since the kernel carries the refinement.
+__global__ void __launch_bounds__(128, 12) knn_scan_label_kernel(PtrView scans, const int64_t* __restrict__ off, int K, const double* __restrict__ poses,
+                                                             const double* __restrict__ ext, int order, const float* __restrict__ T16,
+                                                             const uint8_t* __restrict__ accept, Grid g, const uint32_t* __restrict__ cell_start,
+                                                             const float4* __restrict__ sorted, int k, float thr, uint8_t* __restrict__ label,
+                                                             float* __restrict__ gx, float* __restrict__ gy, float* __restrict__ gz, PtrView small_target) {
     __shared__ float4 s_t[kMaxK];
     if (small_target.n > 0 && threadIdx.x < small_target.n) s_t[threadIdx.x] = make_float4(small_target.x[threadIdx.x], small_target.y[threadIdx.x], small_target.z[threadIdx.x], 0.0f);
     if (small_target.n > 0) __syncthreads();
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= scans.n) return;
-    int lo = 0, hi = K;
-    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (off[mid] <= i) lo = mid; else hi = mid; }
+    const int kf = find_kf(off, K, i);
     float x = scans.x[i], y = scans.y[i], z = scans.z[i];
-    knn_scan_to_global(poses + (size_t)(pose_offset + lo) * 24 + 12, ext, ext_identity, order, &x, &y, &z);   // utility.cpp:164-165, base2lidar as written
+    scan_to_global(poses + (size_t)kf * 24 + 12, ext, order, &x, &y, &z);
+    if (T16 && accept[kf]) {
+        const float* m = T16 + 16 * (size_t)kf;
+        const float nx = frow(m, x, y, z), ny = frow(m + 4, x, y, z), nz = frow(m + 8, x, y, z);
+        x = nx; y = ny; z = nz;
+    }
     gx[i] = x; gy[i] = y; gz[i] = z;
     label[i] = small_target.n > 0 ? knn_label_small(s_t, (int)small_target.n, x, y, z, k, thr) : knn_label_dispatch(g, cell_start, sorted, x, y, z, k, thr);
-}
-
-// global2local of the partitioned points (Session.cpp:603-604)
-__global__ void __launch_bounds__(256) knn_relocalise_kernel(const float* __restrict__ gx, const float* __restrict__ gy, const float* __restrict__ gz,
-                                                             int64_t n, const int64_t* __restrict__ off, int K, const double* __restrict__ poses,
-                                                             int pose_offset, const double* __restrict__ ext, int ext_identity, int order,
-                                                             float* __restrict__ ox, float* __restrict__ oy, float* __restrict__ oz) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    int lo = 0, hi = K;
-    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (off[mid] <= i) lo = mid; else hi = mid; }
-    map_to_sensor(poses + (size_t)(pose_offset + lo) * 24, ext, ext_identity, order, gx[i], gy[i], gz[i], &ox[i], &oy[i], &oz[i]);   // utility.cpp:198-199
 }
 
 // sm_90a: 32 registers and a 44 B spill (L1-resident) at full occupancy.  __launch_bounds__(128, 12) removes the spill (40 registers)
@@ -258,16 +253,8 @@ int knn_target_label(ltr_ctx* ctx, const KnnTarget& t, PtrView q, int k, float t
     return LTR_OK;
 }
 
-}  // namespace ltr
-
-using namespace ltr;
-
-extern "C" {
-
-int ltr_knn_diff(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_offset, ltr_cloud target_h, int32_t k, float thr,
-                 ltr_scanset* out_coexist, ltr_scanset* out_diff) {
-    ApiTrace tr__(ctx, "ltr_knn_diff");
-    if (!ctx) return LTR_ERR_INVALID;
+int knn_diff(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_offset, ltr_cloud target_h, int32_t k, float thr, bool refined,
+             const float* T16, const uint8_t* accepted, ltr_scanset* out_coexist, ltr_scanset* out_diff) {
     DevScanSet* sp;
     DevPoses* pp;
     DevCloud* tp;
@@ -278,51 +265,61 @@ int ltr_knn_diff(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t p
     if (!(thr > 0.0f)) return fail(ctx, LTR_ERR_INVALID, "threshold must be positive");
     if (pose_offset < 0 || pose_offset + sp->K > pp->K) return fail(ctx, LTR_ERR_INVALID, "pose range [%d,%d) outside [0,%d)", pose_offset, pose_offset + sp->K, pp->K);
     if (tp->n < 1) return fail(ctx, LTR_ERR_UNSUPPORTED, "empty target map (PCL's nearestKSearch asserts on an empty tree)");
-    const bool small = tp->n < k;   // fewer than k target points: all of them are returned and the sum is still divided by k (Session.cpp:592-594)
     const DevScanSet scans = *sp;
+    if (refined && scans.K > 0 && (!T16 || !accepted)) return fail(ctx, LTR_ERR_INVALID, "null transforms or accept mask");
+    const bool small = tp->n < k;   // fewer than k target points: all of them are returned and the sum is still divided by k (Session.cpp:592-594)
     const DevPoses poses = *pp;
     const DevCloud target = *tp;
     const int64_t n = scans.pts.n;
-    GridBuf gb;
-    ScratchGuard g_grid(ctx, &gb.block);
-    void* p = nullptr;
-    ScratchGuard g_p(ctx, &p);
-    uint8_t* label = nullptr;
-    float *gx = nullptr, *gy = nullptr, *gz = nullptr;
+    const int K = scans.K;
+    ScanSplit split(ctx, scans, poses.d + (size_t)pose_offset * 24);
+    LTR_TRY(split.init());
     if (n > 0) {
+        GridBuf gb;
+        ScratchGuard g_grid(ctx, &gb.block);
         PtrView small_view{nullptr, nullptr, nullptr, nullptr, 0};
         if (small) small_view = view(target);
         else LTR_TRY(build_grid(ctx, target, k, thr, &gb));
-        LTR_TRY(dev_alloc(ctx, &p, (size_t)n * (3 * sizeof(float) + 1) + 64));
-        gx = (float*)p; gy = gx + n; gz = gy + n; label = (uint8_t*)(gz + n);
-        knn_scan_label_kernel<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(view(scans.pts), scans.d_off, scans.K, poses.d, pose_offset, ctx->d_ext,
-            ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, gb.g, gb.cell_start, gb.sorted, k, thr, label, gx, gy, gz, small_view);
+        void* p = nullptr;
+        ScratchGuard g_p(ctx, &p);
+        const size_t b_g = ((size_t)n * 12 + 255) / 256 * 256, b_T = T16 ? ((size_t)K * 64 + 255) / 256 * 256 : 0;
+        LTR_TRY(dev_alloc(ctx, &p, b_g + b_T + (T16 ? (size_t)K : 0)));
+        float* gx = (float*)p;
+        float* gy = gx + n;
+        float* gz = gy + n;
+        float* dT = nullptr;
+        uint8_t* dacc = nullptr;
+        if (T16) {
+            dT = (float*)((char*)p + b_g);
+            dacc = (uint8_t*)p + b_g + b_T;
+            std::vector<uint8_t> acc((size_t)K);
+            for (int j = 0; j < K; ++j) acc[j] = accepted[j] ? 1 : 0;
+            LTR_CUDA(ctx, cudaMemcpyAsync(dT, T16, (size_t)K * 64, cudaMemcpyHostToDevice, ctx->stream));
+            LTR_CUDA(ctx, cudaMemcpyAsync(dacc, acc.data(), (size_t)K, cudaMemcpyHostToDevice, ctx->stream));
+        }
+        knn_scan_label_kernel<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(view(scans.pts), scans.d_off, K, poses.d + (size_t)pose_offset * 24,
+            ctx->ext_identity ? nullptr : ctx->d_ext, ctx->cfg.transform_order, dT, dacc, gb.g, gb.cell_start, gb.sorted, k, thr, split.flags,
+            gx, gy, gz, small_view);
         LTR_LAUNCH_CHECK(ctx);
         g_grid.release();
-        // re-localise in place (every point; partitioning afterwards keeps the arithmetic identical to the reference,
-        // which transforms the two partitions separately with the same per-point operations)
-        // NOTE: intensity is carried unchanged.
-        DevCloud tmp = scans.pts;  // reuse layout: write relocalised xyz into a scratch cloud with the same stride
-        ltr_cloud scratch;
-        LTR_TRY(cloud_new(ctx, n, &scratch));
-        struct CloudGuard { ltr_ctx* c; ltr_cloud h; bool armed; ~CloudGuard() { if (armed) ltr_cloud_free(c, h); } } g_scratch{ctx, scratch, true};   // error paths below
-        DevCloud sc = ctx->clouds[scratch];
-        knn_relocalise_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(gx, gy, gz, n, scans.d_off, scans.K, poses.d, pose_offset, ctx->d_ext,
-            ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, sc.x(), sc.y(), sc.z());
-        LTR_LAUNCH_CHECK(ctx);
-        LTR_CUDA(ctx, cudaMemcpyAsync(sc.i(), tmp.i(), (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
-        g_scratch.armed = false;
-        DevScanSet view_set = scans;
-        view_set.pts = sc;
-        const int rc = split_scanset_by_flag(ctx, view_set, label, out_coexist, out_diff);
-        ltr_cloud_free(ctx, scratch);
-        return rc;
+        // every point goes back; partitioning afterwards keeps the arithmetic identical to the reference, which transforms the two
+        // partitions separately with the same per-point operations
+        LTR_TRY(split.relocalise(0, n, gx, gy, gz));
     }
-    // empty input: empty outputs with K keyframes
-    std::vector<int64_t> off((size_t)scans.K + 1, 0);
-    if (out_coexist) LTR_TRY(scanset_new(ctx, off, out_coexist));
-    if (out_diff) LTR_TRY(scanset_new(ctx, off, out_diff));
-    return LTR_OK;
+    return split.finish(out_coexist, out_diff);
+}
+
+}  // namespace ltr
+
+using namespace ltr;
+
+extern "C" {
+
+int ltr_knn_diff(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_offset, ltr_cloud target_h, int32_t k, float thr,
+                 ltr_scanset* out_coexist, ltr_scanset* out_diff) {
+    ApiTrace tr__(ctx, "ltr_knn_diff");
+    if (!ctx) return LTR_ERR_INVALID;
+    return knn_diff(ctx, scans_h, poses_h, pose_offset, target_h, k, thr, false, nullptr, nullptr, out_coexist, out_diff);
 }
 
 int ltr_knn_split_cloud(ltr_ctx* ctx, ltr_cloud query_h, ltr_cloud target_h, int32_t k, float thr, ltr_cloud* out_near, ltr_cloud* out_far) {

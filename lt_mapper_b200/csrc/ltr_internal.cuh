@@ -187,6 +187,20 @@ struct ScratchGuard {
     ScratchGuard& operator=(const ScratchGuard&) = delete;
 };
 
+// Owns an ltr_cloud / ltr_scanset handle (h, -1: none) and frees it on every exit path; reset() frees it now.
+template <int (*Free)(ltr_ctx*, int32_t)>
+struct HandleOwner {
+    ltr_ctx* ctx;
+    int32_t h;
+    explicit HandleOwner(ltr_ctx* c, int32_t handle = -1) : ctx(c), h(handle) {}
+    ~HandleOwner() { reset(); }
+    void reset() { if (h >= 0) { Free(ctx, h); h = -1; } }
+    HandleOwner(const HandleOwner&) = delete;
+    HandleOwner& operator=(const HandleOwner&) = delete;
+};
+using CloudOwner = HandleOwner<ltr_cloud_free>;
+using ScanSetOwner = HandleOwner<ltr_scanset_free>;
+
 int cloud_new(ltr_ctx* ctx, int64_t n, ltr_cloud* out);          // uninitialised cloud of n points
 int cloud_get(ltr_ctx* ctx, ltr_cloud h, DevCloud** c);
 int scanset_new(ltr_ctx* ctx, const std::vector<int64_t>& off, ltr_scanset* out);  // allocates points + uploads offsets
@@ -224,6 +238,39 @@ bool scan_images_have_storage(const ltr_ctx* ctx);
 int segment_counts(ltr_ctx* ctx, const uint8_t* flags, const DevScanSet& s, std::vector<int64_t>* counts);
 int split_scanset_by_flag(ltr_ctx* ctx, const DevScanSet& in, const uint8_t* flags, ltr_scanset* out_unflagged, ltr_scanset* out_flagged);
 
+// The points [base, base + n) of `scans` in the global frame (scan_to_global, ref_math.cuh), written to o*[i - base]; keyframe k's pose
+// rows are poses + 24 k + 12, ext is the extrinsic applied first (null: the identity).  oi (optional) receives the intensity.
+int scans_to_global(ltr_ctx* ctx, const DevScanSet& scans, int64_t base, int64_t n, const double* poses, const double* ext, float* ox,
+                    float* oy, float* oz, float* oi);
+
+// The end of a scan-set split (ltr_knn_diff, ltr_scanside_split).  The caller sets flags[i] (1: second part) for every point and hands
+// over the points' global coordinates, all at once or a keyframe range at a time; relocalise() moves them back to their keyframes'
+// frames (global2local, Session.cpp:603-604: the inverse pose at poses + 24 k, then base2lidar) into a copy of the scans that keeps
+// their intensity, and finish() splits that copy by the flags, order preserved, or gives K empty keyframes when the set has no points.
+// The copy is allocated by the first relocalise(), so a caller that frees its search structures first never holds both.
+class ScanSplit {
+public:
+    uint8_t* flags = nullptr;   // one byte per point, after init()
+    ScanSplit(ltr_ctx* ctx, const DevScanSet& scans, const double* poses) : ctx_(ctx), scans_(scans), poses_(poses), reloc_(ctx) {}
+    ~ScanSplit() { if (flags) dev_free(ctx_, flags); }
+    int init();
+    int relocalise(int64_t base, int64_t n, const float* gx, const float* gy, const float* gz);
+    int finish(ltr_scanset* out0, ltr_scanset* out1);
+    ScanSplit(const ScanSplit&) = delete;
+    ScanSplit& operator=(const ScanSplit&) = delete;
+private:
+    ltr_ctx* ctx_;
+    DevScanSet scans_;
+    const double* poses_;
+    CloudOwner reloc_;
+};
+
+// A launch-size knob: the environment variable `name` clamped to [1, hi], or def when it is unset or empty.
+int64_t env_points(const char* name, int64_t def, int64_t hi);
+// Cuts the keyframes of the offsets off[0..K] into launches [cut[j], cut[j + 1]) of at most max_kf keyframes and at most cap points,
+// except that a keyframe is never split (a larger one goes alone); *max_points = the largest launch's points.
+std::vector<int> plan_keyframe_chunks(const std::vector<int64_t>& off, int64_t cap, int max_kf, int64_t* max_points);
+
 // The thresholded kNN decision of ltr_knn_split_cloud (knn.cu) against one target, built once and applied to any number of query views
 // already in the target's frame (scan-side removal, scanside.cu).  knn_target_build: 1 <= k <= 16, thr > 0, target of >= 1 finite points;
 // the caller returns *block to the allocator.  knn_target_label: label[i] = 1 if |avg| >= thr ("far"), else 0.
@@ -237,5 +284,10 @@ struct KnnTarget {
 };
 int knn_target_build(ltr_ctx* ctx, const DevCloud& target, int k, float thr, KnnTarget* t, void** block);
 int knn_target_label(ltr_ctx* ctx, const KnnTarget& t, PtrView q, int k, float thr, uint8_t* label);
+
+// ltr_knn_diff (T16 = accepted = null) and ltr_knn_diff_refined (knn.cu): with T16 the global points of keyframe k with accepted[k] != 0
+// are moved by T16 + 16 k before they are labelled.  refined: K > 0 keyframes without T16 or accepted are LTR_ERR_INVALID.
+int knn_diff(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_offset, ltr_cloud target_h, int32_t k, float thr, bool refined,
+             const float* T16, const uint8_t* accepted, ltr_scanset* out_coexist, ltr_scanset* out_diff);
 
 }  // namespace ltr

@@ -159,13 +159,17 @@ LTR_DEV void map_to_sensor(const double* __restrict__ inv_pose, const double* __
     if (!ext_identity) transform_point(ext, order, *lx, *ly, *lz, lx, ly, lz);
 }
 
-// local2global of a scan point as the kNN diff moves it (Session.cpp:545 passes base2lidar; utility.cpp:164-165): the extrinsic unless it is
-// exactly the identity (ext: base2lidar rows 0..2), then the pose (rows 0..2).  Its inverse is map_to_sensor with the inverse pose.
-LTR_DEV void knn_scan_to_global(const double* __restrict__ pose, const double* __restrict__ ext, int ext_identity, int order, float* x, float* y,
-                                float* z) {
-    if (!ext_identity) transform_point(ext, order, *x, *y, *z, x, y, z);
+// local2global of a scan point (utility.cpp:164-165): the extrinsic `ext` (3x4 rows), skipped when null because it is exactly the identity,
+// then the pose (rows 0..2).  The reference passes different extrinsics on different paths (DESIGN.md §5.1): base2lidar (ltr_ctx::d_ext)
+// for the kNN diff (Session.cpp:545) and ICP, lidar2base (d_ext + 12) for scan-side removal and mergeScansWithinGlobalCoordUtil.  The
+// paths that move points back all use map_to_sensor with base2lidar (Session.cpp:603-604, utility.cpp:198-199).
+LTR_DEV void scan_to_global(const double* __restrict__ pose, const double* __restrict__ ext, int order, float* x, float* y, float* z) {
+    if (ext) transform_point(ext, order, *x, *y, *z, x, y, z);
     transform_point(pose, order, *x, *y, *z, x, y, z);
 }
+
+// ((m0 x + m1 y) + m2 z) + m3 in f32, m = one row of a row-major float 4x4 (PCL's Matrix4f applied to a point)
+LTR_DEV float frow(const float* m, float x, float y, float z) { return fa(fa(fa(fm(m[0], x), fm(m[1], y)), fm(m[2], z)), m[3]); }
 
 // FLANN L2_Simple<float> squared distance: ((dx*dx) + dy*dy) + dz*dz with dx = query - point
 LTR_DEV float l2_simple(float qx, float qy, float qz, float px, float py, float pz) {

@@ -11,23 +11,10 @@
 //
 // "map" needs only the decision |avg_map| < thr: that is knn.cu's bounded 27-cell grid search (its header has the proof).
 // "scan minus map" needs the exact VALUES of avg_scan and avg_map -- two large averages can differ by less than thr -- so no radius bound
-// applies.  Both averages come from an exact k-NN over sparse grids:
-//   * a grid level sorts its points by the 64-bit key (segment, cz, cy, cx) with the project's radix sort (util.cu) and keeps the sorted
-//     unique keys and each cell's first point.  Segment = keyframe of the launch for the own-scan targets, 0 for the map.  A row of cells
-//     (one segment, cz, cy; consecutive cx) is one contiguous key range: one binary search per row.
-//   * a query searches shell by shell (Chebyshev radius s = 0, 1, ... in cells around its own cell) and stops after shell s when the
-//     block holds every cell of the level, or when its current k-th smallest computed distance D_k satisfies
-//         D_k <= ((s - 2^-6) c)^2 (1 - 2^-20)        (c = 1 / inv_cell, the cell side the indices are computed with), or D_k = 0.
-// Why the stop is exact.  A point p outside the block lies in a cell whose index differs from the query's by >= s + 1 on some axis a.
-// Both indices are floor(fl(fl(v - origin) * inv_cell)) with |.| clamped to 2^40 (a clamp only moves a query's index towards the box, so
-// its true distance is larger still); each evaluation carries a relative error below 3 * 2^-53, i.e. below 2^-11 cells for |index| <= 2^40,
-// so |p_a - q_a| >= (s - 2^-10) c > (s - 2^-6) c in exact arithmetic.  FLANN's L2_Simple in f32 (((dx*dx) + dy*dy) + dz*dz, no FMA):
-// rounding is monotone, so |dx| = |fl(q_a - p_a)| >= fl((s - 2^-6) c) >= (s - 2^-6) c (1 - u), u = 2^-24, fl(dx*dx) >= dx^2 (1 - u), and the
-// two additions of non-negative terms round to no less than fl(dx*dx).  The computed distance of p is therefore
-// >= ((s - 2^-6) c)^2 (1 - u)^3 > ((s - 2^-6) c)^2 (1 - 2^-20) >= D_k: no point outside the block can displace a value of the k smallest
-// (a tie at D_k leaves the multiset unchanged), so the double sum in ascending order, its float rounding and the division by float(k) are
-// final.  D_k = 0 cannot be undercut by any distance.  How many values enter the sum is min(k, points evaluated), never "finite ones":
-// an overflowed +inf distance is summed as FLANN would return it.
+// applies.  Both averages come from an exact k-NN over the sparse grid levels of sparse_grid.cuh (segment = keyframe of the launch for
+// the own-scan targets, 0 for the map): a query searches shell by shell and stops after shell s when the block holds every cell, or when
+// its k-th smallest computed distance D_k satisfies D_k <= ((s - 2^-6) c)^2 (1 - 2^-20), or D_k = 0.  sparse_grid.cuh's header proves
+// the stop exact.
 // Two passes: a bounded pass on the finest level (c0 = 0.25 m, shells 0..2) settles almost every point.  The rest (isolated returns at
 // long range, queries far from the map) are compacted into a list and searched on levels of 4x, 16x, ... the cell side, bounded again
 // except on the coarsest level (at most 10 cells per axis), which searches until the stop rule holds.  A level changes the cost only.
@@ -43,7 +30,6 @@
 #include "sparse_grid.cuh"
 #include <algorithm>
 #include <cmath>
-#include <cstdlib>
 
 namespace ltr {
 
@@ -54,12 +40,6 @@ constexpr int kSegShift = kGridSegShift;
 constexpr int kMaxSegments = kGridMaxSegments;   // 8192 keyframes per launch
 constexpr int kBoundedShells = 2;
 constexpr int64_t kChunkPoints = (int64_t)1 << 24;
-
-int64_t chunk_points() {
-    int64_t n = kChunkPoints;
-    if (const char* e = std::getenv("LTR_SCANSIDE_CHUNK_POINTS")) if (*e) n = std::min<int64_t>(std::max<int64_t>(std::atoll(e), 1), (int64_t)1 << 30);
-    return n;
-}
 
 // ---- level build -------------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) level_key_kernel(PtrView p, const int64_t* __restrict__ off, int nseg, Level L,
@@ -167,6 +147,7 @@ int build_level(ltr_ctx* ctx, PtrView p, const int64_t* d_off, int nseg, const f
 namespace {
 
 // ---- exact k-NN ----------------------------------------------------------------------------------------------------------------------
+// the K smallest computed distances; the shell search's stop rule for them is in sparse_grid.cuh's header
 template <int K>
 struct Best {
     float d[K];
@@ -176,7 +157,7 @@ struct Best {
         for (int j = 0; j < K; ++j) d[j] = __int_as_float(0x7f800000);
         seen = 0;
     }
-    __device__ __forceinline__ void push(float v) {
+    __device__ __forceinline__ void push(float v, const float4&) {
         ++seen;
         if (v < d[K - 1]) {
             d[K - 1] = v;
@@ -185,63 +166,20 @@ struct Best {
                 if (d[j] < d[j - 1]) { const float t = d[j]; d[j] = d[j - 1]; d[j - 1] = t; }
         }
     }
+    __device__ __forceinline__ bool settled(long long s, double cell) const {
+        if (seen < K) return false;
+        const double dk = (double)d[K - 1], b = shell_bound(s, cell);
+        return dk == 0.0 || (s > 0 && dk <= b);
+    }
 };
 
-template <int K>
-__device__ __forceinline__ void scan_row(const Level& L, uint32_t c0, uint32_t c1, int seg, long long xa, long long xb, long long y, long long z,
-                                         float qx, float qy, float qz, Best<K>& b) {
-    const unsigned long long ka = cell_key(seg, xa, y, z), kb = cell_key(seg, xb, y, z);
-    uint32_t lo = c0, hi = c1;
-    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (L.keys[mid] < ka) lo = mid + 1; else hi = mid; }
-    for (uint32_t ci = lo; ci < c1 && L.keys[ci] <= kb; ++ci) {
-        const uint32_t e = L.start[ci + 1];
-        for (uint32_t p = L.start[ci]; p < e; ++p) {
-            const float4 t = L.pts[p];
-            b.push(l2_simple(qx, qy, qz, t.x, t.y, t.z));
-        }
-    }
-}
-
-// Exact mean of the k smallest squared distances from q to the points of segment `seg` (file header).  false: not settled within
-// max_shell shells on a bounded level.
+// Exact mean of the k smallest squared distances from q to the points of segment `seg`.  false: not settled within max_shell shells on a
+// bounded level.
 template <int K>
 __device__ bool knn_exact_avg(const Level& L, int seg, float qx, float qy, float qz, int max_shell, float* avg) {
     Best<K> b;
     b.init();
-    const float q[3] = {qx, qy, qz};
-    long long c[3], s0 = 0, cover = 0;
-#pragma unroll
-    for (int d = 0; d < 3; ++d) {
-        c[d] = cell_index((double)q[d], L.origin[d], L.inv_cell);
-        const long long hi = (long long)L.dim[d] - 1;
-        s0 = max(s0, max(-c[d], c[d] - hi));       // Chebyshev distance from the query's cell to the box: nearer shells are empty
-        cover = max(cover, max(c[d], hi - c[d]));  // from this radius on the block holds every cell
-    }
-    const uint32_t c0 = L.seg_first[seg], c1 = L.seg_first[seg + 1];
-    bool done = c0 == c1;
-    for (long long s = s0; !done; ++s) {
-        if (!L.final_level && s > max_shell) return false;
-        const long long z0 = max(c[2] - s, 0ll), z1 = min(c[2] + s, (long long)L.dim[2] - 1);
-        const long long y0 = max(c[1] - s, 0ll), y1 = min(c[1] + s, (long long)L.dim[1] - 1);
-        const long long xa = max(c[0] - s, 0ll), xb = min(c[0] + s, (long long)L.dim[0] - 1);
-        for (long long z = z0; z <= z1; ++z) {
-            const bool zface = z == c[2] - s || z == c[2] + s;
-            for (long long y = y0; y <= y1; ++y) {
-                if (zface || y == c[1] - s || y == c[1] + s) {
-                    if (xa <= xb) scan_row<K>(L, c0, c1, seg, xa, xb, y, z, qx, qy, qz, b);
-                } else {
-                    if (c[0] - s >= 0 && c[0] - s < L.dim[0]) scan_row<K>(L, c0, c1, seg, c[0] - s, c[0] - s, y, z, qx, qy, qz, b);
-                    if (s > 0 && c[0] + s >= 0 && c[0] + s < L.dim[0]) scan_row<K>(L, c0, c1, seg, c[0] + s, c[0] + s, y, z, qx, qy, qz, b);
-                }
-            }
-        }
-        if (s >= cover) break;
-        if (b.seen >= K) {
-            const double dk = (double)b.d[K - 1];
-            const double r = ((double)s - 0x1p-6) * L.cell;
-            if (dk == 0.0 || (s > 0 && dk <= r * r * (1.0 - 0x1p-20))) done = true;
-        }
-    }
+    if (!shell_search(L, seg, qx, qy, qz, max_shell, b)) return false;
     // accumulate(..., 0.0) in double, ascending (Removerter.cpp:1052, 1097); float(sum) / float(k) (:1053, 1098)
     const int cnt = b.seen < K ? (int)b.seen : K;
     double sum = 0.0;
@@ -290,7 +228,7 @@ int exact_avg_all(ltr_ctx* ctx, Pyramid& T, int k, PtrView q, const int64_t* q_o
     *unsettled = 0;
     for (int l = 0; n > 0; ++l) {
         const Level* L;
-        LTR_TRY(T.get(ctx, l, &L));
+        LTR_TRY(T.get(l, &L));
         uint32_t* next = (list == list_a) ? list_b : list_a;
         LTR_CUDA(ctx, cudaMemsetAsync(d_cnt, 0, sizeof(unsigned int), ctx->stream));
         LTR_TRY(launch_exact_knn(ctx, k, *L, q, q_off, nseg, list, n, avg, next, d_cnt));
@@ -305,37 +243,7 @@ int exact_avg_all(ltr_ctx* ctx, Pyramid& T, int k, PtrView q, const int64_t* q_o
     return LTR_OK;
 }
 
-// ---- transforms and decisions --------------------------------------------------------------------------------------------------------
-// local2global (utility.cpp:164-165): lidar2base, then the pose, f32 rounding after each step
-__global__ void __launch_bounds__(256) scanside_global_kernel(PtrView in, const int64_t* __restrict__ off, int K, int64_t base,
-                                                              const double* __restrict__ poses, int pose_offset, const double* __restrict__ ext,
-                                                              int ext_identity, int order, int64_t n, float* __restrict__ gx,
-                                                              float* __restrict__ gy, float* __restrict__ gz) {
-    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= n) return;
-    const int64_t i = base + t;
-    const int k = find_kf(off, K, i);
-    float x = in.x[i], y = in.y[i], z = in.z[i];
-    if (!ext_identity) transform_point(ext + 12, order, x, y, z, &x, &y, &z);
-    transform_point(poses + (size_t)(pose_offset + k) * 24 + 12, order, x, y, z, &x, &y, &z);
-    gx[t] = x; gy[t] = y; gz[t] = z;
-}
-
-// global2local (utility.cpp:198-199): inverse pose, then base2lidar
-__global__ void __launch_bounds__(256) scanside_local_kernel(const float* __restrict__ gx, const float* __restrict__ gy, const float* __restrict__ gz,
-                                                             const int64_t* __restrict__ off, int K, int64_t base, const double* __restrict__ poses,
-                                                             int pose_offset, const double* __restrict__ ext, int ext_identity, int order,
-                                                             int64_t n, DevCloud out) {
-    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= n) return;
-    const int64_t i = base + t;
-    const int k = find_kf(off, K, i);
-    float x = gx[t], y = gy[t], z = gz[t];
-    transform_point(poses + (size_t)(pose_offset + k) * 24, order, x, y, z, &x, &y, &z);
-    if (!ext_identity) transform_point(ext, order, x, y, z, &x, &y, &z);
-    out.x()[i] = x; out.y()[i] = y; out.z()[i] = z;
-}
-
+// ---- decisions -----------------------------------------------------------------------------------------------------------------------
 // fabsf(avg_scan - avg_map) < thr -> static (Removerter.cpp:1107), the subtraction in f32
 __global__ void __launch_bounds__(256) scanside_diff_kernel(const float* __restrict__ avg_scan, const float* __restrict__ avg_map, int64_t n,
                                                             float thr, uint8_t* __restrict__ flag) {
@@ -383,27 +291,13 @@ int ltr_scanside_split(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int
         if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite map coordinates (%u points)", nonfinite);
     }
     const int64_t n = scans.pts.n;
-    const int ext_id = ctx->ext_identity ? 1 : 0, order = ctx->cfg.transform_order;
-    ltr_cloud reloc_h = -1;
-    struct CloudGuard { ltr_ctx* c; ltr_cloud* h; ~CloudGuard() { if (*h >= 0) ltr_cloud_free(c, *h); } } g_reloc{ctx, &reloc_h};
-    void* flags = nullptr;
-    ScratchGuard g_flags(ctx, &flags);
-    LTR_TRY(dev_alloc(ctx, &flags, (size_t)std::max<int64_t>(n, 1)));
+    const double* pose0 = poses.d + (size_t)pose_offset * 24;
+    ScanSplit split(ctx, scans, pose0);
+    LTR_TRY(split.init());
     if (n > 0) {
-        LTR_TRY(cloud_new(ctx, n, &reloc_h));
-        const DevCloud reloc = ctx->clouds[reloc_h];
-        LTR_CUDA(ctx, cudaMemcpyAsync(reloc.i(), scans.pts.i(), (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
-        // keyframe chunks: at most chunk_points() points (a keyframe is never split) and kMaxSegments keyframes
-        const int64_t cap = chunk_points();
-        std::vector<int> kf_cut{0};
-        for (int kf = 0; kf < scans.K;) {
-            int e = kf + 1;
-            while (e < scans.K && e - kf < kMaxSegments && scans.h_off[e + 1] - scans.h_off[kf] <= cap) ++e;
-            kf_cut.push_back(e);
-            kf = e;
-        }
         int64_t max_chunk = 0;
-        for (size_t c = 0; c + 1 < kf_cut.size(); ++c) max_chunk = std::max(max_chunk, scans.h_off[kf_cut[c + 1]] - scans.h_off[kf_cut[c]]);
+        const std::vector<int> kf_cut = plan_keyframe_chunks(scans.h_off, env_points("LTR_SCANSIDE_CHUNK_POINTS", kChunkPoints, (int64_t)1 << 30),
+                                                             kMaxSegments, &max_chunk);
         if (max_chunk >= ((int64_t)1 << 32)) return fail(ctx, LTR_ERR_UNSUPPORTED, "a keyframe of %lld points", (long long)max_chunk);
         const int64_t ccap = round_cap(max_chunk);
         void* work = nullptr;
@@ -422,8 +316,7 @@ int ltr_scanside_split(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int
         KnnTarget kt;
         void* kt_block = nullptr;
         ScratchGuard g_kt(ctx, &kt_block);
-        Pyramid mapT;
-        struct PyrGuard { ltr_ctx* c; Pyramid* p; ~PyrGuard() { p->release(c); } } g_mapT{ctx, &mapT};
+        Pyramid mapT(ctx);
         if (criterion == LTR_SCANSIDE_MAP) LTR_TRY(knn_target_build(ctx, map, k, thr, &kt, &kt_block));
         else {
             float mn[3], mx[3];
@@ -435,17 +328,15 @@ int ltr_scanside_split(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int
             const int64_t base = scans.h_off[kf0], m = scans.h_off[kf1] - base;
             ctx->scanside_stats[3]++;
             if (m == 0) continue;
-            const unsigned nb = (unsigned)((m + 255) / 256);
-            scanside_global_kernel<<<nb, 256, 0, ctx->stream>>>(view(scans.pts), scans.d_off, scans.K, base, poses.d, pose_offset, ctx->d_ext, ext_id,
-                                                                order, m, g.x(), g.y(), g.z());
-            LTR_LAUNCH_CHECK(ctx);
+            // local2global with lidar2base (file header)
+            LTR_TRY(scans_to_global(ctx, scans, base, m, pose0, ctx->ext_identity ? nullptr : ctx->d_ext + 12, g.x(), g.y(), g.z(), nullptr));
             g.n = m;
             float mn[3], mx[3];
             uint32_t nonfinite = 0;
             LTR_TRY(minmax_xyz(ctx, g, mn, mx, &nonfinite));
             if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite scan coordinates (%u points in keyframes [%d,%d))", nonfinite, kf0, kf1);
             const PtrView q = view(g);
-            uint8_t* fl = (uint8_t*)flags + base;
+            uint8_t* fl = split.flags + base;
             if (criterion == LTR_SCANSIDE_MAP) {
                 // |avg_map| < thr -> static (Removerter.cpp:1056)
                 LTR_TRY(knn_target_label(ctx, kt, q, k, thr, fl));
@@ -455,31 +346,21 @@ int ltr_scanside_split(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int
                 int64_t un = 0;
                 LTR_TRY(exact_avg_all(ctx, mapT, k, q, nullptr, 1, avg_map, list_a, list_b, d_cnt, &un));
                 ctx->scanside_stats[1] += un;
-                Pyramid self;
-                struct PyrGuard2 { ltr_ctx* c; Pyramid* p; ~PyrGuard2() { p->release(c); } } g_self{ctx, &self};
+                Pyramid self(ctx);
                 self.init(q, c_off, nkf, mn, mx);
                 LTR_TRY(exact_avg_all(ctx, self, k, q, c_off, nkf, avg_scan, list_a, list_b, d_cnt, &un));
                 ctx->scanside_stats[2] += un;
-                self.release(ctx);
-                scanside_diff_kernel<<<nb, 256, 0, ctx->stream>>>(avg_scan, avg_map, m, thr, fl);
+                self.release();
+                scanside_diff_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(avg_scan, avg_map, m, thr, fl);
                 LTR_LAUNCH_CHECK(ctx);
             }
-            scanside_local_kernel<<<nb, 256, 0, ctx->stream>>>(g.x(), g.y(), g.z(), scans.d_off, scans.K, base, poses.d, pose_offset, ctx->d_ext,
-                                                               ext_id, order, m, reloc);
-            LTR_LAUNCH_CHECK(ctx);
+            LTR_TRY(split.relocalise(base, m, g.x(), g.y(), g.z()));
         }
-        mapT.release(ctx);
+        mapT.release();
         g_kt.release();
         g_work.release();
-        DevScanSet set = scans;
-        set.pts = reloc;
-        LTR_TRY(split_scanset_by_flag(ctx, set, (const uint8_t*)flags, out_static, out_dynamic));
-        return LTR_OK;
     }
-    std::vector<int64_t> off((size_t)scans.K + 1, 0);
-    if (out_static) LTR_TRY(scanset_new(ctx, off, out_static));
-    if (out_dynamic) LTR_TRY(scanset_new(ctx, off, out_dynamic));
-    return LTR_OK;
+    return split.finish(out_static, out_dynamic);
 }
 
 int ltr_scanside_stats(ltr_ctx* ctx, int64_t* stats4) {

@@ -4,6 +4,7 @@
 #include "device_util.cuh"
 #include <cfloat>
 #include <cmath>
+#include <cstdlib>
 #include <algorithm>
 
 namespace ltr {
@@ -727,9 +728,9 @@ static int voxel_distributed(ltr_ctx* ctx, int comm, const DevCloud& loc, float 
         scount[(size_t)d] += hl[i];
     }
     // 3. group the local points by destination (stable), move them to their owners
-    ltr_cloud send_h;
-    LTR_TRY(cloud_new(ctx, n, &send_h));
-    struct CloudGuard { ltr_ctx* c; ltr_cloud h; ~CloudGuard() { if (h >= 0) ltr_cloud_free(c, h); } } g_send{ctx, send_h}, g_recv{ctx, -1}, g_slice{ctx, -1};
+    CloudOwner g_send(ctx), g_recv(ctx), g_slice(ctx);
+    LTR_TRY(cloud_new(ctx, n, &g_send.h));
+    const ltr_cloud send_h = g_send.h;
     if (n > 0) {
         vox_dest_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(keys0, n, shift, cuts, keys1, idx1);
         LTR_LAUNCH_CHECK(ctx);
@@ -740,7 +741,7 @@ static int voxel_distributed(ltr_ctx* ctx, int comm, const DevCloud& loc, float 
     }
     g_p.release();
     LTR_TRY(nccl_alltoallv_cloud(ctx, comm, ctx->clouds[send_h], scount, &g_recv.h));
-    ltr_cloud_free(ctx, send_h); g_send.h = -1;
+    g_send.reset();
     // 4. my range, with the GLOBAL box
     const DevCloud recv = ctx->clouds[g_recv.h];
     LTR_TRY(cloud_new(ctx, recv.n, &g_slice.h));
@@ -753,17 +754,88 @@ static int voxel_distributed(ltr_ctx* ctx, int comm, const DevCloud& loc, float 
 }
 
 // ------------------------------------------------------------------------------------------------
-// mergeScansWithinGlobalCoordUtil (utility.cpp:170-192): local -> lidar2base -> pose, f32 rounding after each step
+// Frame changes of scan sets: local2global of the points [base, base + n) (utility.cpp:164-165), and global2local back (utility.cpp:198-199)
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) merge_global_kernel(PtrView in, const int64_t* __restrict__ off, int K, const double* __restrict__ poses,
-                                                           const double* __restrict__ ext, int ext_identity, int order, DevCloud out) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= in.n) return;
+__global__ void __launch_bounds__(256) scans_to_global_kernel(PtrView in, const int64_t* __restrict__ off, int K, int64_t base, int64_t n,
+                                                              const double* __restrict__ poses, const double* __restrict__ ext, int order,
+                                                              float* __restrict__ ox, float* __restrict__ oy, float* __restrict__ oz,
+                                                              float* __restrict__ oi) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    const int64_t i = base + t;
     const int k = find_kf(off, K, i);
     float x = in.x[i], y = in.y[i], z = in.z[i];
-    if (!ext_identity) transform_point(ext + 12, order, x, y, z, &x, &y, &z);  // lidar2base
-    transform_point(poses + (size_t)k * 24 + 12, order, x, y, z, &x, &y, &z);  // pose
-    out.x()[i] = x; out.y()[i] = y; out.z()[i] = z; out.i()[i] = in.i[i];
+    scan_to_global(poses + (size_t)k * 24 + 12, ext, order, &x, &y, &z);
+    ox[t] = x; oy[t] = y; oz[t] = z;
+    if (oi) oi[t] = in.i[i];
+}
+
+__global__ void __launch_bounds__(256) global_to_scans_kernel(const float* __restrict__ gx, const float* __restrict__ gy, const float* __restrict__ gz,
+                                                              const int64_t* __restrict__ off, int K, int64_t base, int64_t n,
+                                                              const double* __restrict__ poses, const double* __restrict__ ext, int order,
+                                                              DevCloud out) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    const int64_t i = base + t;
+    const int k = find_kf(off, K, i);
+    map_to_sensor(poses + (size_t)k * 24, ext, ext == nullptr, order, gx[t], gy[t], gz[t], &out.x()[i], &out.y()[i], &out.z()[i]);
+}
+
+int scans_to_global(ltr_ctx* ctx, const DevScanSet& scans, int64_t base, int64_t n, const double* poses, const double* ext, float* ox,
+                    float* oy, float* oz, float* oi) {
+    if (n == 0) return LTR_OK;
+    scans_to_global_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(view(scans.pts), scans.d_off, scans.K, base, n, poses, ext,
+                                                                                ctx->cfg.transform_order, ox, oy, oz, oi);
+    LTR_LAUNCH_CHECK(ctx);
+    return LTR_OK;
+}
+
+int ScanSplit::init() {
+    return scans_.pts.n > 0 ? dev_alloc(ctx_, (void**)&flags, (size_t)scans_.pts.n) : LTR_OK;
+}
+
+int ScanSplit::relocalise(int64_t base, int64_t n, const float* gx, const float* gy, const float* gz) {
+    if (n == 0) return LTR_OK;
+    if (reloc_.h < 0) {
+        LTR_TRY(cloud_new(ctx_, scans_.pts.n, &reloc_.h));
+        LTR_CUDA(ctx_, cudaMemcpyAsync(ctx_->clouds[reloc_.h].i(), scans_.pts.i(), (size_t)scans_.pts.n * sizeof(float), cudaMemcpyDeviceToDevice,
+                                       ctx_->stream));
+    }
+    global_to_scans_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx_->stream>>>(gx, gy, gz, scans_.d_off, scans_.K, base, n, poses_,
+        ctx_->ext_identity ? nullptr : ctx_->d_ext, ctx_->cfg.transform_order, ctx_->clouds[reloc_.h]);
+    LTR_LAUNCH_CHECK(ctx_);
+    return LTR_OK;
+}
+
+int ScanSplit::finish(ltr_scanset* out0, ltr_scanset* out1) {
+    if (scans_.pts.n == 0) {
+        const std::vector<int64_t> off((size_t)scans_.K + 1, 0);
+        if (out0) LTR_TRY(scanset_new(ctx_, off, out0));
+        if (out1) LTR_TRY(scanset_new(ctx_, off, out1));
+        return LTR_OK;
+    }
+    DevScanSet set = scans_;
+    set.pts = ctx_->clouds[reloc_.h];
+    return split_scanset_by_flag(ctx_, set, flags, out0, out1);
+}
+
+int64_t env_points(const char* name, int64_t def, int64_t hi) {
+    if (const char* e = std::getenv(name)) if (*e) return std::min<int64_t>(std::max<int64_t>(std::atoll(e), 1), hi);
+    return def;
+}
+
+std::vector<int> plan_keyframe_chunks(const std::vector<int64_t>& off, int64_t cap, int max_kf, int64_t* max_points) {
+    const int K = (int)off.size() - 1;
+    std::vector<int> cut{0};
+    *max_points = 0;
+    for (int kf = 0; kf < K;) {
+        int e = kf + 1;
+        while (e < K && e - kf < max_kf && off[e + 1] - off[kf] <= cap) ++e;
+        cut.push_back(e);
+        *max_points = std::max(*max_points, off[e] - off[kf]);
+        kf = e;
+    }
+    return cut;
 }
 
 // precleaningKeyframes (Session.cpp:506-533)
@@ -900,12 +972,9 @@ int ltr_merge_scans_global(ltr_ctx* ctx, ltr_scanset scans, ltr_poses poses, ltr
     const DevScanSet ss = *s;
     const DevPoses pp = *p;
     LTR_TRY(cloud_new(ctx, ss.pts.n, out));
-    if (ss.pts.n == 0) return LTR_OK;
-    const int T = 256;
-    merge_global_kernel<<<(unsigned)((ss.pts.n + T - 1) / T), T, 0, ctx->stream>>>(view(ss.pts), ss.d_off, ss.K, pp.d, ctx->d_ext,
-                                                                                ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, ctx->clouds[*out]);
-    LTR_LAUNCH_CHECK(ctx);
-    return LTR_OK;
+    // mergeScansWithinGlobalCoordUtil (utility.cpp:170-192): lidar2base, then the pose
+    const DevCloud o = ctx->clouds[*out];
+    return scans_to_global(ctx, ss, 0, ss.pts.n, pp.d, ctx->ext_identity ? nullptr : ctx->d_ext + 12, o.x(), o.y(), o.z(), o.i());
 }
 
 int ltr_preclean(ltr_ctx* ctx, ltr_scanset scans, float radius, ltr_scanset* out) {

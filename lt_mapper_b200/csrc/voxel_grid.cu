@@ -19,7 +19,6 @@
 #include <cfloat>
 #include <climits>
 #include <cmath>
-#include <cstdlib>
 
 namespace ltr {
 
@@ -33,11 +32,6 @@ constexpr int64_t kVgChunkPoints = (int64_t)64 << 20;   // points per launch: bo
 // Test knob: LTR_VOXEL_GRID_CHUNK_POINTS=n (clamped to [1, kVgChunkPoints]; unset or empty: kVgChunkPoints) takes the place of
 // kVgChunkPoints in voxel_grid_run, so that tests can split small inputs into many launches and check the scratch indexing relative to
 // each launch's first scan.
-static int64_t vg_chunk_points() {
-    int64_t n = kVgChunkPoints;
-    if (const char* e = std::getenv("LTR_VOXEL_GRID_CHUNK_POINTS")) if (*e) n = std::min<int64_t>(std::max<int64_t>(std::atoll(e), 1), kVgChunkPoints);
-    return n;
-}
 
 // x86-64 cvttss2si: NaN and out-of-range values give the "integer indefinite" 0x80000000 (CUDA saturates, and NaN -> 0)
 __device__ __forceinline__ int32_t x86_f2i32(float f) {
@@ -423,11 +417,10 @@ static int voxel_grid_run(ltr_ctx* ctx, const PtrView& src, const std::vector<in
         if (n >= ((int64_t)1 << 31)) return fail(ctx, LTR_ERR_UNSUPPORTED, "voxel grid: scan %d has %lld points (>= 2^31)", k, (long long)n);
         max_chunk = std::max(max_chunk, n);
     }
-    max_chunk = std::max(max_chunk, std::min<int64_t>(off[K], vg_chunk_points()));
+    max_chunk = std::max(max_chunk, std::min<int64_t>(off[K], env_points("LTR_VOXEL_GRID_CHUNK_POINTS", kVgChunkPoints, kVgChunkPoints)));
     void *p_ent = nullptr, *p_pos = nullptr, *p_segs = nullptr, *p_cnt = nullptr, *p_status = nullptr, *p_oo = nullptr;
     ScratchGuard g_ent(ctx, &p_ent), g_pos(ctx, &p_pos), g_segs(ctx, &p_segs), g_cnt(ctx, &p_cnt), g_status(ctx, &p_status), g_oo(ctx, &p_oo);
-    ltr_cloud sc_h = -1;
-    struct CloudGuard { ltr_ctx* c; ltr_cloud* h; ~CloudGuard() { if (*h >= 0) ltr_cloud_free(c, *h); } } g_sc{ctx, &sc_h};
+    CloudOwner g_sc(ctx);
     const size_t nk = (size_t)std::max(K, 1);
     LTR_TRY(dev_alloc(ctx, &p_cnt, nk * sizeof(int64_t)));
     LTR_TRY(dev_alloc(ctx, &p_status, nk * sizeof(int32_t)));
@@ -436,9 +429,9 @@ static int voxel_grid_run(ltr_ctx* ctx, const PtrView& src, const std::vector<in
         LTR_TRY(dev_alloc(ctx, &p_ent, (size_t)max_chunk * sizeof(uint64_t)));
         LTR_TRY(dev_alloc(ctx, &p_pos, (size_t)max_chunk * 2 * sizeof(uint32_t)));
         LTR_TRY(dev_alloc(ctx, &p_segs, (size_t)max_chunk * sizeof(uint64_t)));
-        LTR_TRY(cloud_new(ctx, off[K], &sc_h));
+        LTR_TRY(cloud_new(ctx, off[K], &g_sc.h));
     }
-    const DevCloud sc = sc_h >= 0 ? ctx->clouds[sc_h] : DevCloud();
+    const DevCloud sc = g_sc.h >= 0 ? ctx->clouds[g_sc.h] : DevCloud();
     for (int k0 = 0; k0 < K;) {
         int k1 = k0 + 1;
         while (k1 < K && off[k1 + 1] - off[k0] <= max_chunk) ++k1;
