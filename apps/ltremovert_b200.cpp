@@ -6,6 +6,7 @@
 // 1517-1520, 1600-1601, 1607-1650).  No ROS, no PCL; rviz publishing is dropped (side effect only).
 //
 //   ltremovert_b200 --config params.yaml [--selfremovert] [--pcl110] [--no-split] [--clean-scans[=map|scan-minus-map]] [--icp-refinement]
+//                   [--adaptive-threshold[=c]]
 //     --selfremovert   run selfRemovert over remove_resolution_list (Removerter.cpp:1378-1393) instead of the shipped
 //                      single removeOnce(2.5) (Removerter.cpp:1584, 1587)
 //     --pcl110         PCL >= 1.10 transformPointCloud summation order (ltr_config.transform_order = 1)
@@ -19,6 +20,10 @@
 //                      when its fitness is below 1.0 (partitionLowDynamicPointsOfScanByKnn's `useICPrefinement`, Session.cpp:549-584,
 //                      off in the reference); prints one summary line (keyframes accepted, median iterations).  The output tree keeps
 //                      its layout; the files derived from Step 2 hold the refined results.
+//     --adaptive-threshold  every remove, revert, ND and PD pass flags a pixel when its range diff exceeds fl(c * scan range) instead of
+//                      0.1 m (the range-proportional threshold calcDescrepancyAndParseDynamicPointIdx leaves commented out,
+//                      Removerter.cpp:393-402); c defaults to the reference's 0.05 and must lie in (0, 1).  Prints one summary line; the
+//                      output tree keeps its layout.  There is no yaml key: the reference has none.
 //
 // Multi-GPU: start one process per GPU with RANK / WORLD_SIZE / LOCAL_RANK in the environment (torchrun, mpirun -x, a shell loop);
 // every rank reads the yaml and the pose files, but loads only the scans of ITS keyframe block (even world: ranks < world/2 take the
@@ -124,7 +129,9 @@ int main(int argc, char** argv) {
     bool selfremovert = false, pcl110 = false, no_split = false;
     int clean_scans = -1;   // -1 off, else ltr_scanside_criterion
     bool icp_refinement = false;
-    const char* usage = "usage: %s --config params.yaml [--selfremovert] [--pcl110] [--no-split] [--clean-scans[=map|scan-minus-map]] [--icp-refinement]\n";
+    float adaptive_c = 0.0f;   // 0: the constant threshold
+    const char* usage = "usage: %s --config params.yaml [--selfremovert] [--pcl110] [--no-split] [--clean-scans[=map|scan-minus-map]] [--icp-refinement]"
+                        " [--adaptive-threshold[=c], 0 < c < 1]\n";
     for (int i = 1; i < argc; ++i) {
         if (!std::strcmp(argv[i], "--config") && i + 1 < argc) cfg_path = argv[++i];
         else if (!std::strcmp(argv[i], "--selfremovert")) selfremovert = true;
@@ -133,6 +140,12 @@ int main(int argc, char** argv) {
         else if (!std::strcmp(argv[i], "--clean-scans") || !std::strcmp(argv[i], "--clean-scans=map")) clean_scans = LTR_SCANSIDE_MAP;
         else if (!std::strcmp(argv[i], "--clean-scans=scan-minus-map")) clean_scans = LTR_SCANSIDE_SCAN_MINUS_MAP;
         else if (!std::strcmp(argv[i], "--icp-refinement")) icp_refinement = true;
+        else if (!std::strcmp(argv[i], "--adaptive-threshold")) adaptive_c = 0.05f;
+        else if (!std::strncmp(argv[i], "--adaptive-threshold=", 21)) {
+            char* end = nullptr;
+            adaptive_c = std::strtof(argv[i] + 21, &end);
+            if (end == argv[i] + 21 || *end || !(adaptive_c > 0.0f && adaptive_c < 1.0f)) { std::fprintf(stderr, usage, argv[0]); return 2; }
+        }
         else { std::fprintf(stderr, usage, argv[0]); return 2; }
     }
     if (cfg_path.empty()) { std::fprintf(stderr, usage, argv[0]); return 2; }
@@ -221,6 +234,10 @@ int main(int argc, char** argv) {
             std::fprintf(stderr, "[pcl::VoxelGrid::applyFilter] Leaf size is too small for the input dataset (%d scans returned unchanged)\n", overflow_warnings);
         std::vector<float>().swap(S.xyzi);   // the raw scans now live on the device
     }
+    R.adaptiveThresholdCoeff_ = adaptive_c;   // checked above
+    if (adaptive_c != 0.0f && rank == 0)
+        std::printf(" Adaptive threshold: coefficient %g, a pixel flags when its diff exceeds fl(%g * scan range) in every remove / revert / ND / PD pass\n",
+                    (double)adaptive_c, (double)adaptive_c);
     ck(R.run_step0(), "Step 0");
     R.useICPrefinement_ = icp_refinement;
     ck(R.run_step12(), "Step 1-2");

@@ -153,6 +153,14 @@ int ltr_voxel_grid_per_keyframe(ltr_ctx* ctx, ltr_scanset in, float leaf, ltr_sc
  * (environment: LTR_SCAN_IMAGE_CACHE_MB=n caps them at n MiB; 0 builds the images per launch, without keeping them). */
 int ltr_remove_pass(ltr_ctx* ctx, ltr_cloud map, ltr_scanset scans, ltr_poses poses, int32_t kf_begin, int32_t kf_end,
                     int32_t mode, float res_alpha, float diff_thres, int32_t accumulate, int64_t* n_dynamic);
+/* ltr_remove_pass with the range-adaptive discrepancy threshold the reference leaves commented out in
+ * calcDescrepancyAndParseDynamicPointIdx (Removerter.cpp:393-402, line 396 in place of 398): each pixel of each keyframe compares its
+ * diff (scan - map for HD / revert / PD, map - scan for ND) with t = fl(adaptive_coeff * s), s the keyframe's scan range at the pixel
+ * (10000 without a return), instead of a constant: flagged iff diff < 200 && diff > t.  The winner, the union over keyframes and the
+ * kept scan-side images behave as in ltr_remove_pass.  adaptive_coeff must be finite and in (0, 1) (the reference's value is 0.05),
+ * else LTR_ERR_INVALID. */
+int ltr_remove_pass_adaptive(ltr_ctx* ctx, ltr_cloud map, ltr_scanset scans, ltr_poses poses, int32_t kf_begin, int32_t kf_end,
+                             int32_t mode, float res_alpha, float adaptive_coeff, int32_t accumulate, int64_t* n_dynamic);
 /* Drops the scan-side images ltr_remove_pass keeps; free_storage != 0 also returns their storage to the context's allocator cache. */
 int ltr_scan_images_release(ltr_ctx* ctx, int32_t free_storage);
 /* Device pointer to the N flag bytes of the last ltr_remove_pass on `map` (for an all-reduce hook). */

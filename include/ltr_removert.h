@@ -113,6 +113,12 @@ int ltrh_scanside_removal(ltrh_removerter* r, int32_t map_sess, int32_t scan_ses
  * (ltr_knn_diff_refined): scans_knn_coexist_ / scans_knn_diff_ then hold the registered points.  Multi-GPU: each rank refines its own
  * keyframe block against its replica of the target map; no collective. */
 int ltrh_set_icp_refinement(ltrh_removerter* r, int32_t on);
+/* The range-adaptive discrepancy threshold of calcDescrepancyAndParseDynamicPointIdx (Removerter.cpp:393-402, commented out in the
+ * reference): with c in (0, 1) every later remove, revert, ND and PD pass (removeOnce, revertOnce, iremoveOnceForND, removeOnceForPD)
+ * runs ltr_remove_pass_adaptive with coefficient c, so that a pixel flags when its diff exceeds fl(c * scan range) instead of 0.1 m; the
+ * reference's value is 0.05.  c = 0 (the default) turns it off.  Any other value: LTR_ERR_INVALID.  Multi-GPU: nothing new crosses
+ * ranks (the flag union of each pass is unchanged). */
+int ltrh_set_adaptive_threshold(ltrh_removerter* r, float c);
 /* Per-keyframe results of the last refinement of session `sess` on this rank: *K_out keyframes (0 when the last detectLowDynamicPoints ran
  * without refinement, and after ltrh_reset_to_step0 or ltrh_cascade_promote_updated, which release Step 2's results), and, when capacity >= *K_out, the final float 4x4 (16 per keyframe), fitness, iterations, exit reason (ltr_icp_exit)
  * and the accepted flag (fitness < 1.0).  Any array may be NULL. */

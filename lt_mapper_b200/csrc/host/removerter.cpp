@@ -316,7 +316,10 @@ int Removerter::partitionCurrentMapGeneric(ltr_cloud map, Session& source, ltr_s
     int64_t n_map = 0;
     CK(ltr_cloud_size(ctx, map, &n_map));
     // n_dynamic is taken from the partition below (after the cross-rank flag union), so no count is requested here
-    CK(ltr_remove_pass(ctx, map, scans, source.keyframe_poses_, 0, source.num_keyframes_, mode, res, 0.1f, 0, nullptr));
+    if (adaptiveThresholdCoeff_ != 0.0f)   // Removerter.cpp:396 in place of :398, for every variant
+        CK(ltr_remove_pass_adaptive(ctx, map, scans, source.keyframe_poses_, 0, source.num_keyframes_, mode, res, adaptiveThresholdCoeff_, 0, nullptr));
+    else
+        CK(ltr_remove_pass(ctx, map, scans, source.keyframe_poses_, 0, source.num_keyframes_, mode, res, 0.1f, 0, nullptr));
     CK(reduce_flags(map, source));
     CK(ltr_apply_partition(ctx, map, stat, dyn));
     int64_t n_dyn = 0;
@@ -832,6 +835,12 @@ int ltrh_scanside_removal(ltrh_removerter* r, int32_t map_sess, int32_t scan_ses
 int ltrh_set_icp_refinement(ltrh_removerter* r, int32_t on) {
     if (!r) return LTR_ERR_INVALID;
     r->R->useICPrefinement_ = on != 0;
+    return LTR_OK;
+}
+
+int ltrh_set_adaptive_threshold(ltrh_removerter* r, float c) {
+    if (!r || !(c == 0.0f || (c > 0.0f && c < 1.0f))) return LTR_ERR_INVALID;   // NaN fails every comparison
+    r->R->adaptiveThresholdCoeff_ = c;
     return LTR_OK;
 }
 

@@ -122,6 +122,7 @@ public:
 
     ltrh_params P;
     bool useICPrefinement_ = false;   // Session.cpp:551 (`bool useICPrefinement { false }`), set by ltrh_set_icp_refinement
+    float adaptiveThresholdCoeff_ = 0.0f;   // Removerter.cpp:395-396 (`adaptive_coeff`, commented out); 0: the constant 0.1 (:398), set by ltrh_set_adaptive_threshold
     ltr_ctx* ctx = nullptr;
     ltr_comm comm{};          // legacy caller-supplied hooks (host-memory tests); superseded by the native transport when nccl_world >= 0
     bool has_comm = false;

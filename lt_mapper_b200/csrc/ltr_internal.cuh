@@ -66,8 +66,10 @@ struct ScanImageSet {
     ScanImageKey key;
     uint32_t* rimg = nullptr;     // scan range images, (kf_end - kf_begin) x rows x cols
     float* pyr = nullptr;         // sliding-window maxima of tile culling (project_cull.cuh), built for pyr_shortcut
-    uint32_t* timg = nullptr;     // test image of the scan-minus-map fast path (scan_test_image_kernel), built for timg_shortcut
+    uint32_t* timg = nullptr;     // test image of the scan-minus-map fast path (scan_test_image_kernel), built for timg_shortcut and the
+                                  // threshold coefficient with the bits timg_coeff_bits (0: the constant threshold)
     int pyr_shortcut = -1, timg_shortcut = -1;
+    uint32_t timg_coeff_bits = 0;
     uint64_t last_use = 0;
 };
 

@@ -79,8 +79,11 @@ __global__ void __launch_bounds__(256) scan_rimg_fast_kernel(PtrView scans, cons
 // empty_scan_shortcut_ok).  With pad_g guard rows above and below and pad_c = 1 guard column (FastCfg::pad_*) the guard rows replicate the
 // rows that pixel_index clamps to, so the short elevation path gathers from it without clamping its index, and column 0 and the guard column
 // hold +inf: the pixels next to the azimuth seam, whose pairs map_project_fast_kernel sends to the full exact path.  pad_g = pad_c = 0: plain layout.
+// kAdaptive (pixel threshold fl(c s), Removerter.cpp:396): every other pixel holds fl_up(s - fl(c s)) instead of s -- an upper bound of
+// s - t that the fast kernel tests against 0 (project_fast.cuh); a pixel without a return too, unless the shortcut made it -inf.
+template <bool kAdaptive = false>
 __global__ void __launch_bounds__(256) scan_test_image_kernel(const uint32_t* __restrict__ rimg, uint32_t* __restrict__ test_img, int nb, int rows, int cols,
-                                                              int pad_g, int pad_c, int empty_to_ninf) {
+                                                              int pad_g, int pad_c, int empty_to_ninf, float coeff) {
     const int W = cols + pad_c;
     const int64_t per_kf = (int64_t)(rows + 2 * pad_g) * W, n = nb * per_kf;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -90,16 +93,19 @@ __global__ void __launch_bounds__(256) scan_test_image_kernel(const uint32_t* __
         const int cp = p - rp * W;
         const int r = min(max(rp - pad_g, 0), rows - 1), c = min(cp, cols - 1);
         const uint32_t b = rimg[(size_t)k * rows * cols + (size_t)r * cols + c];
-        test_img[i] = (pad_c && (cp == 0 || cp == cols)) ? 0x7f800000u : (empty_to_ninf && b == kNoPointBits) ? 0xff800000u : b;
+        const uint32_t v = kAdaptive ? __float_as_uint(__fsub_ru(__uint_as_float(b), fm(coeff, __uint_as_float(b)))) : b;
+        test_img[i] = (pad_c && (cp == 0 || cp == cols)) ? 0x7f800000u : (empty_to_ninf && b == kNoPointBits) ? 0xff800000u : v;
     }
 }
 
 // Exact projection of every map point into every keyframe of the batch.
 //   kCandidatesOnly = true  (HD / revert / PD, diff = scan - map): by monotonicity of f32 subtraction the set
-//       {points with scan - range > thres} is a prefix in range order of the pixel's points, so the pixel winner among
+//       {points with scan - range > t} is a prefix in range order of the pixel's points, so the pixel winner among
 //       them equals the global pixel winner whenever any exists; only those points touch the atomic (SURVEY.md §A.2).
+//       The argument needs t constant within a pixel, not across pixels: it holds for the adaptive t = fl(c s) (kAdaptive,
+//       `thres` = c), which only depends on the pixel's scan range s.
 //   kCandidatesOnly = false (ND, visible-point extraction): true per-pixel minimum with a read-before-atomic filter.
-template <bool kCandidatesOnly>
+template <bool kCandidatesOnly, bool kAdaptive = false>
 __global__ void __launch_bounds__(256) map_project_kernel(PtrView map, const double* __restrict__ poses, int kf0, int nb,
                                                           const double* __restrict__ ext, int ext_identity, int order, ImgShape g,
                                                           const uint32_t* __restrict__ scan_rimg, float thres, uint64_t* __restrict__ win) {
@@ -111,11 +117,12 @@ __global__ void __launch_bounds__(256) map_project_kernel(PtrView map, const dou
     const float x = map.x[i], y = map.y[i], z = map.z[i];
     unsigned n_atomics = 0;   // not reported by this kernel
     for (int k = 0; k < nb; ++k)
-        exact_pair<kCandidatesOnly>(x, y, z, (uint32_t)i, (uint32_t)k, s_pose + 12 * k, ext, ext_identity, order, g, scan_rimg, thres, win, 0, &n_atomics);
+        exact_pair<kCandidatesOnly, kAdaptive>(x, y, z, (uint32_t)i, (uint32_t)k, s_pose + 12 * k, ext, ext_identity, order, g, scan_rimg, thres, win, 0, &n_atomics);
 }
 
-// calcDescrepancyAndParseDynamicPointIdx (Removerter.cpp:381-413) over the batch images; also re-arms `win`.
-template <bool kCandidatesOnly>
+// calcDescrepancyAndParseDynamicPointIdx (Removerter.cpp:381-413) over the batch images; also re-arms `win`.  kAdaptive: the threshold
+// is fl(c s) of the pixel's scan range s (Removerter.cpp:396 in place of :398), c in `thres`.
+template <bool kCandidatesOnly, bool kAdaptive = false>
 __global__ void __launch_bounds__(256) resolve_kernel(const uint32_t* __restrict__ scan_rimg, uint64_t* __restrict__ win, int64_t total_px,
                                                       float thres, uint8_t* __restrict__ flags) {
     const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -124,14 +131,14 @@ __global__ void __launch_bounds__(256) resolve_kernel(const uint32_t* __restrict
     if (kCandidatesOnly) {
         if (w == kWinNone) return;
         win[p] = kWinNone;
-        const float mr = __uint_as_float((uint32_t)(w >> 32));
-        const float diff = fs(__uint_as_float(scan_rimg[p]), mr);  // scan - map (Removerter.cpp:572, 459)
-        if (diff < kValidDiffUpperBound && diff > thres) flags[(uint32_t)w] = 1;
+        const float mr = __uint_as_float((uint32_t)(w >> 32)), sr = __uint_as_float(scan_rimg[p]);
+        const float diff = fs(sr, mr);  // scan - map (Removerter.cpp:572, 459)
+        if (diff < kValidDiffUpperBound && diff > pixel_thres<kAdaptive>(thres, sr)) flags[(uint32_t)w] = 1;
     } else {
         if (w != kWinEmpty) win[p] = kWinEmpty;
-        const float mr = __uint_as_float((uint32_t)(w >> 32));
-        const float diff = fs(mr, __uint_as_float(scan_rimg[p]));  // map - scan (Removerter.cpp:516)
-        if (diff < kValidDiffUpperBound && diff > thres) flags[(uint32_t)w] = 1;
+        const float mr = __uint_as_float((uint32_t)(w >> 32)), sr = __uint_as_float(scan_rimg[p]);
+        const float diff = fs(mr, sr);  // map - scan (Removerter.cpp:516)
+        if (diff < kValidDiffUpperBound && diff > pixel_thres<kAdaptive>(thres, sr)) flags[(uint32_t)w] = 1;
     }
 }
 
@@ -371,10 +378,12 @@ using FastKernel = decltype(&map_project_fast_kernel<true, true, false, true>);
 
 // One launch of the map projection over the keyframes [k0, k0 + nb) of `poses` into `win`, timed by an event pair.  rimg: the launch's scan
 // range images (scan-minus-map; unused by the true minimum), test_img: the test image of the scan-minus-map fast path.  amin (fast path,
-// may be null in the deferred mode): the approximate running minimum, reset here.  da: the deferred mode's scratch.
+// may be null in the deferred mode): the approximate running minimum, reset here.  da: the deferred mode's scratch.  adaptive (scan-minus-map
+// only): `thres` is the coefficient c of the pixel threshold fl(c s), and test_img was built for it.
 static int project_map(ltr_ctx* ctx, PassPlan& p, const DevCloud& map, const DevPoses& poses, int k0, int nb, Proj mode, const uint32_t* rimg,
-                       const uint32_t* test_img, float thres, uint64_t* win, uint32_t* amin, const CullArgs& ca, const DeferredArgs& da) {
+                       const uint32_t* test_img, float thres, bool adaptive, uint64_t* win, uint32_t* amin, const CullArgs& ca, const DeferredArgs& da) {
     const bool cand = mode == Proj::kScanMinusMap;
+    adaptive = adaptive && cand;
     if (amin) {
         fill_u32_kernel<<<grid_for(nb * p.npx, 256, ctx->sm_count * 8), 256, 0, ctx->stream>>>(amin, 0x7f800000u, nb * p.npx);
         LTR_LAUNCH_CHECK(ctx);
@@ -382,7 +391,7 @@ static int project_map(ltr_ctx* ctx, PassPlan& p, const DevCloud& map, const Dev
     prof_begin(ctx);
     p.units.push_back(nb);
     if (!p.use_fast) {
-        const auto kern = cand ? map_project_kernel<true> : map_project_kernel<false>;
+        const auto kern = adaptive ? map_project_kernel<true, true> : cand ? map_project_kernel<true> : map_project_kernel<false>;
         kern<<<(unsigned)((map.n + 255) / 256), 256, (size_t)nb * 12 * sizeof(double), ctx->stream>>>(view(map), poses.d, k0, nb, ctx->d_ext,
             ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, p.g, rimg, thres, win);
     } else {
@@ -393,11 +402,11 @@ static int project_map(ltr_ctx* ctx, PassPlan& p, const DevCloud& map, const Dev
             LTR_CUDA(ctx, cudaMemsetAsync(da.best, 0xff, (size_t)nb * p.npx * sizeof(unsigned long long), ctx->stream));   // "no pair yet"
             LTR_CUDA(ctx, cudaMemsetAsync(da.count, 0, sizeof(unsigned int), ctx->stream));
         }
-        // template arguments <candidates only, short elevation path, deferred, guard-padded test image>
-        const FastKernel kern = (cand && p.fc.pad_ok) ? map_project_fast_kernel<true, true, false, true>
-            : with_el_direct(p.fc, [mode](auto el) -> FastKernel {
+        // template arguments <candidates only, short elevation path, deferred, guard-padded test image, adaptive threshold>
+        const FastKernel kern = (cand && p.fc.pad_ok) ? (adaptive ? map_project_fast_kernel<true, true, false, true, true> : map_project_fast_kernel<true, true, false, true>)
+            : with_el_direct(p.fc, [mode, adaptive](auto el) -> FastKernel {
                   constexpr bool kEl = decltype(el)::value;
-                  return mode == Proj::kScanMinusMap ? map_project_fast_kernel<true, kEl, false>
+                  return mode == Proj::kScanMinusMap ? (adaptive ? map_project_fast_kernel<true, kEl, false, false, true> : map_project_fast_kernel<true, kEl, false>)
                        : mode == Proj::kTrueMin      ? map_project_fast_kernel<false, kEl, false>
                                                      : map_project_fast_kernel<false, kEl, true>;
               });
@@ -466,12 +475,13 @@ static int deferred_alloc(ltr_ctx* ctx, int B, int64_t npx, void** block, Deferr
 // Scan-side images of a remove pass for the keyframes [k0, k0 + nb) of `scans`, keyframe-major:
 //   rimg  the scan range image (scan2RangeImg), built here when make_rimg, else read;
 //   pyr   (if non-null) its sliding-window maxima for tile culling; an empty scan pixel is -inf with the shortcut, else +inf;
-//   timg  (if non-null) the test image of the scan-minus-map fast path, guard-padded when `pad`, empty pixels -inf with the shortcut.
+//   timg  (if non-null) the test image of the scan-minus-map fast path, guard-padded when `pad`, empty pixels -inf with the shortcut;
+//         coeff != 0: the one of the adaptive threshold fl(coeff s) (scan_test_image_kernel).
 // The shortcut is the plan's FastCfg::empty_scan_shortcut.  None of them reads the map.  Launches cover at most kImageChunk keyframes (the
 // window-maximum grid's z extent).
 constexpr int kImageChunk = 1024;
 static int build_scan_images(ltr_ctx* ctx, const PassPlan& p, const DevScanSet& scans, int k0, int nb, bool make_rimg, uint32_t* rimg, float* pyr,
-                             uint32_t* timg, bool pad) {
+                             uint32_t* timg, bool pad, float coeff) {
     const ImgShape& g = p.g;
     const int64_t npx = p.npx;
     const int shortcut = p.fc.empty_scan_shortcut;
@@ -489,8 +499,9 @@ static int build_scan_images(ltr_ctx* ctx, const PassPlan& p, const DevScanSet& 
             LTR_LAUNCH_CHECK(ctx);
         }
         if (timg) {
-            scan_test_image_kernel<<<grid_for(n * timg_px, 256, fill_blocks), 256, 0, ctx->stream>>>(ri, timg + (size_t)c0 * timg_px, n, g.rows, g.cols,
-                                                                                                    pad ? p.fc.pad_g : 0, pad ? 1 : 0, shortcut);
+            const auto kern = coeff != 0.0f ? scan_test_image_kernel<true> : scan_test_image_kernel<false>;
+            kern<<<grid_for(n * timg_px, 256, fill_blocks), 256, 0, ctx->stream>>>(ri, timg + (size_t)c0 * timg_px, n, g.rows, g.cols, pad ? p.fc.pad_g : 0,
+                                                                                  pad ? 1 : 0, shortcut, coeff);
             LTR_LAUNCH_CHECK(ctx);
         }
     }
@@ -503,6 +514,7 @@ static void scan_image_set_drop(ScanImageSet& s) {
     s.valid = false;
     s.rimg = nullptr; s.pyr = nullptr; s.timg = nullptr;
     s.pyr_shortcut = s.timg_shortcut = -1;
+    s.timg_coeff_bits = 0;
 }
 
 void scan_images_release(ltr_ctx* ctx, uint64_t serial, bool free_storage) {
@@ -537,11 +549,12 @@ struct ScanImagesPin {
 };
 
 // The kept set with the scan images of a pass over [kf_begin, kf_end) -- found, completed or built, in launches over the whole range.
+// The test image is the one of `coeff` (0: the constant threshold); the range image and the window table do not depend on it.
 // A new set goes into an empty slot or the least recently used one, preferring a slot whose storage is already large enough; storage only
 // grows.  *out = nullptr when the sets are off or the storage would exceed the budget: the pass then builds its images per launch.  The
 // caller holds a ScanImagesPin.
 static int scan_images_get(ltr_ctx* ctx, const PassPlan& p, const DevScanSet& scans, const DevPoses& poses, int kf_begin, int kf_end, bool need_pyr,
-                           bool need_timg, bool pad, ScanImageSet** out) {
+                           bool need_timg, bool pad, float coeff, ScanImageSet** out) {
     *out = nullptr;
     size_t budget = 0;
     if (!scan_image_cache_on(&budget)) return LTR_OK;
@@ -590,16 +603,18 @@ static int scan_images_get(ltr_ctx* ctx, const PassPlan& p, const DevScanSet& sc
     char* base = (char*)s->block;
     const bool make_rimg = !s->valid;
     const bool make_pyr = need_pyr && s->pyr_shortcut != shortcut;
-    const bool make_timg = need_timg && s->timg_shortcut != shortcut;
+    uint32_t coeff_bits;
+    std::memcpy(&coeff_bits, &coeff, sizeof(coeff_bits));
+    const bool make_timg = need_timg && (s->timg_shortcut != shortcut || s->timg_coeff_bits != coeff_bits);
     s->rimg = (uint32_t*)base;
     s->timg = s->cap >= timg_off + timg_bytes ? (uint32_t*)(base + timg_off) : nullptr;
     s->pyr = s->cap >= pyr_off + pyr_bytes ? (float*)(base + pyr_off) : nullptr;
     if (make_rimg || make_pyr || make_timg) {
         s->valid = false;   // until the build is enqueued
-        LTR_TRY(build_scan_images(ctx, p, scans, kf_begin, K, make_rimg, s->rimg, make_pyr ? s->pyr : nullptr, make_timg ? s->timg : nullptr, pad));
+        LTR_TRY(build_scan_images(ctx, p, scans, kf_begin, K, make_rimg, s->rimg, make_pyr ? s->pyr : nullptr, make_timg ? s->timg : nullptr, pad, coeff));
         s->valid = true;
         if (make_pyr) s->pyr_shortcut = shortcut;
-        if (make_timg) s->timg_shortcut = shortcut;
+        if (make_timg) { s->timg_shortcut = shortcut; s->timg_coeff_bits = coeff_bits; }
     }
     s->last_use = ++ctx->scan_images_tick;
     *out = s;
@@ -629,9 +644,13 @@ int ltr_scan_images_release(ltr_ctx* ctx, int32_t free_storage) {
     return LTR_OK;
 }
 
+// adaptive_c != 0: the pixel threshold is fl(adaptive_c s) (ltr_remove_pass_adaptive) and diff_thres is not used.
 static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end,
-                            int32_t mode, float res_alpha, float diff_thres, int32_t accumulate, int64_t* n_dynamic, bool allow_deferred, bool* overflowed) {
+                            int32_t mode, float res_alpha, float diff_thres, float adaptive_c, int32_t accumulate, int64_t* n_dynamic, bool allow_deferred,
+                            bool* overflowed) {
     *overflowed = false;
+    const bool adaptive = adaptive_c != 0.0f;
+    const float thres = adaptive ? adaptive_c : diff_thres;   // the kernels' `thres`: the constant, or the coefficient
     DevCloud* map;
     DevScanSet* scans;
     DevPoses* poses;
@@ -665,14 +684,16 @@ static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, 
     const bool use_cull = p.use_fast && cand && ctx->cfg.fast_path >= 2 && B <= 32 && map->n >= kTilePts && map->n >= npx;
     void *p_tiles = nullptr, *p_pyr = nullptr;
     ScratchGuard g_tiles(ctx, &p_tiles), g_pyr(ctx, &p_pyr);
-    // scan-minus-map with the short elevation path and a 360 degree field of view: the test image is guard-padded (FastCfg::pad_*) and always built
+    // scan-minus-map with the short elevation path and a 360 degree field of view: the test image is guard-padded (FastCfg::pad_*) and always built;
+    // so is the adaptive threshold's (scan_test_image_kernel)
     const bool pad = p.use_fast && cand && p.fc.pad_ok;
-    const bool need_timg = p.use_fast && cand && (shortcut || pad);
+    const float timg_coeff = cand ? adaptive_c : 0.0f;
+    const bool need_timg = p.use_fast && cand && (shortcut || pad || adaptive);
     const int64_t timg_px = pad ? (int64_t)p.fc.pad_npx : npx;
     // the scan-side images come from a kept set built over the whole range (scan_images_get) or, without one, are built per launch
     ScanImagesPin pin(ctx);
     ScanImageSet* set = nullptr;
-    if (run) LTR_TRY(scan_images_get(ctx, p, *scans, *poses, kf_begin, kf_end, use_cull, need_timg, pad, &set));
+    if (run) LTR_TRY(scan_images_get(ctx, p, *scans, *poses, kf_begin, kf_end, use_cull, need_timg, pad, timg_coeff, &set));
     if (use_cull) {
         ca.enabled = 1;
         ca.ntiles = (map->n + kTilePts - 1) / kTilePts;
@@ -707,15 +728,15 @@ static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, 
                 test_img = need_timg ? set->timg + j * timg_px : rimg;
                 if (use_cull) ca.pyr = set->pyr + j * ca.pyr_stride;
             } else {
-                LTR_TRY(build_scan_images(ctx, p, *scans, k0, nb, true, l_rimg, use_cull ? (float*)p_pyr : nullptr, l_timg, pad));
+                LTR_TRY(build_scan_images(ctx, p, *scans, k0, nb, true, l_rimg, use_cull ? (float*)p_pyr : nullptr, l_timg, pad, timg_coeff));
                 rimg = l_rimg;
                 test_img = need_timg ? l_timg : l_rimg;
                 if (use_cull) ca.pyr = (const float*)p_pyr;
             }
-            LTR_TRY(project_map(ctx, p, *map, *poses, k0, nb, proj, rimg, test_img, diff_thres, win, amin, ca, da));
+            LTR_TRY(project_map(ctx, p, *map, *poses, k0, nb, proj, rimg, test_img, thres, adaptive, win, amin, ca, da));
             const unsigned rb = (unsigned)((nb * npx + 255) / 256);
-            if (cand) resolve_kernel<true><<<rb, 256, 0, ctx->stream>>>(rimg, win, nb * npx, diff_thres, map->flags);
-            else resolve_kernel<false><<<rb, 256, 0, ctx->stream>>>(rimg, win, nb * npx, diff_thres, map->flags);
+            const auto resolve = cand ? (adaptive ? resolve_kernel<true, true> : resolve_kernel<true>) : (adaptive ? resolve_kernel<false, true> : resolve_kernel<false>);
+            resolve<<<rb, 256, 0, ctx->stream>>>(rimg, win, nb * npx, thres, map->flags);
             LTR_LAUNCH_CHECK(ctx);
         }
     }
@@ -739,7 +760,19 @@ int ltr_remove_pass(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, ltr_pose
     // ND (true per-pixel minimum) runs in the deferred mode of project_fast.cuh unless the flags accumulate into earlier ones (a run whose
     // overflow list filled up would have to be undone)
     return with_deferred_retry([&](bool allow_deferred, bool* overflowed) {
-        return remove_pass_impl(ctx, map_h, scans_h, poses_h, kf_begin, kf_end, mode, res_alpha, diff_thres, accumulate, n_dynamic,
+        return remove_pass_impl(ctx, map_h, scans_h, poses_h, kf_begin, kf_end, mode, res_alpha, diff_thres, 0.0f, accumulate, n_dynamic,
+                                allow_deferred && !accumulate, overflowed);
+    });
+}
+
+int ltr_remove_pass_adaptive(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end,
+                             int32_t mode, float res_alpha, float adaptive_coeff, int32_t accumulate, int64_t* n_dynamic) {
+    ApiTrace tr__(ctx, "ltr_remove_pass_adaptive");
+    if (!ctx) return LTR_ERR_INVALID;
+    // NaN fails both comparisons
+    if (!(adaptive_coeff > 0.0f && adaptive_coeff < 1.0f)) return fail(ctx, LTR_ERR_INVALID, "adaptive coefficient %g outside (0, 1)", (double)adaptive_coeff);
+    return with_deferred_retry([&](bool allow_deferred, bool* overflowed) {
+        return remove_pass_impl(ctx, map_h, scans_h, poses_h, kf_begin, kf_end, mode, res_alpha, 0.0f, adaptive_coeff, accumulate, n_dynamic,
                                 allow_deferred && !accumulate, overflowed);
     });
 }
@@ -809,7 +842,7 @@ static int parse_projected_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_poses poses_h
                 da.order = (const unsigned long long*)sorted;
             }
             LTR_TRY(project_map(ctx, p, mapc, posc, kf_begin + k0, nb, use_deferred ? Proj::kTrueMinDeferred : Proj::kTrueMin, nullptr, nullptr, 0.0f,
-                                win, amin, no_cull, da));
+                                false, win, amin, no_cull, da));
             parse_count_kernel<<<dim3((unsigned)nchunk, (unsigned)nb), 1024, 0, ctx->stream>>>(win, (int)npx, nchunk, chunk_cnt);
             LTR_LAUNCH_CHECK(ctx);
             parse_compact_kernel<<<dim3((unsigned)nchunk, (unsigned)nb), 1024, 0, ctx->stream>>>(win, (int)npx, nchunk, chunk_cnt, (uint32_t*)p_list + (size_t)k0 * npx,

@@ -96,6 +96,12 @@ __global__ void __launch_bounds__(256) scan_window_max_kernel(const uint32_t* __
 
 // true iff no point of the tile can be a candidate in keyframe k (kf = its fast constants).  Every comparison is written so
 // that NaN / degenerate geometry yields "false" (keep the tile).
+// kAdaptive (`thres` = c, pixel threshold t = fl(c s)): a pair is a candidate only if s - rho > t (fl(s - rho) > t for a float t).
+// Round to nearest gives t >= c s (1 - u), u = 2^-24, so s - t <= s (1 - c (1 - u)), which is non-decreasing in s (c < 1): every pixel
+// of the rectangle has s - t <= smax (1 - c (1 - u)).  With c' = fl_down(c (1 - u)) <= c (1 - u) and k1 = fl_up(1 - c') >= 1 - c (1 - u):
+//     fl_up(smax k1) <= fl_down(rmin - 1 mm)   =>   s - t <= smax k1 <= rmin - 1 mm < rho   for every point of the tile,
+// so no pair is a candidate.  The window table of s is the one of the constant threshold.
+template <bool kAdaptive = false>
 LTR_DEV bool tile_culled(const float* __restrict__ kf, float4 tile, const FastCfg& fc, const ImgShape& g, const CullArgs& ca, int k, float thres) {
     if (kf[15] == 0.0f) return false;
     const FastProj f = fast_project(kf, tile.x, tile.y, tile.z);   // f.r = |c - o|, f.rho_inv_r = 1 / cos(elevation of c)
@@ -133,6 +139,10 @@ LTR_DEV bool tile_culled(const float* __restrict__ kf, float4 tile, const FastCf
         if (r + s - 1 >= r1) break;
     }
     const float rmin = __fsub_rn(__fsub_rn(__fmul_rn(d, 0.999996f), tile.w), 1.0e-4f);
+    if (kAdaptive) {
+        const float k1 = __fsub_ru(1.0f, __fmul_rd(thres, 0.99999994f));        // 0.99999994f == 1 - 2^-24 exactly
+        return __fmul_ru(smax, k1) <= __fsub_rd(rmin, 1.0e-3f);
+    }
     return smax <= __fsub_rn(__fadd_rn(rmin, thres), 1.0e-3f);                 // scan - range <= thres - 1 mm for every point of the tile
 }
 

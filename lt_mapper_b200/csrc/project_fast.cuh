@@ -204,24 +204,30 @@ constexpr uint32_t kNoPointBitsF = 0x461C4000u;  // 10000.0f
 // queue entry: [63:32] map index | [31:14] pixel (row * cols + col, < 2^18) | [13:0] keyframe within the batch
 LTR_DEV uint64_t q_pack(uint32_t i, uint32_t px, uint32_t k) { return ((uint64_t)i << 32) | (px << 14) | k; }
 
-// Offers the exact key (range r, map index i) to pixel px of the winner image.  kCandidatesOnly: only a candidate (scan - r > thres) enters,
-// and with the empty-scan shortcut a pixel without a scan return turns every pair away (diff > 200 for every map point there).  A key that
-// is not below the pixel's current one skips the atomic.
-template <bool kCandidatesOnly>
+// The discrepancy threshold of a pixel whose scan range is s (calcDescrepancyAndParseDynamicPointIdx, Removerter.cpp:393-398): the constant
+// `thres`, or with kAdaptive the range-proportional fl(c s) of the reference's commented-out line 396, the coefficient c passed in `thres`.
+template <bool kAdaptive>
+LTR_DEV float pixel_thres(float thres, float s) { return kAdaptive ? fm(thres, s) : thres; }
+
+// Offers the exact key (range r, map index i) to pixel px of the winner image.  kCandidatesOnly: only a candidate (scan - r > t, t the
+// pixel's threshold, pixel_thres) enters, and with the empty-scan shortcut a pixel without a scan return turns every pair away (diff > 200
+// for every map point there, whatever t is).  A key that is not below the pixel's current one skips the atomic.
+template <bool kCandidatesOnly, bool kAdaptive = false>
 LTR_DEV void offer(uint64_t* __restrict__ win, size_t px, float r, uint32_t i, const uint32_t* __restrict__ scan_rimg, float thres, int shortcut,
                    unsigned* n_atomics) {
     const uint64_t packed = ((uint64_t)__float_as_uint(r) << 32) | i;
     if (kCandidatesOnly) {
         const uint32_t sb = scan_rimg[px];
         if (shortcut && sb == kNoPointBitsF && r < 9000.0f) return;
-        if (!(fs(__uint_as_float(sb), r) > thres)) return;
+        const float s = __uint_as_float(sb);
+        if (!(fs(s, r) > pixel_thres<kAdaptive>(thres, s))) return;
     }
     if (packed < win[px]) { atomicMin((unsigned long long*)&win[px], (unsigned long long)packed); ++*n_atomics; }
 }
 
 // The reference arithmetic of one pair: map point i at (x, y, z) projected into keyframe k of the launch (inv_pose: its inverse pose) and
 // offered at its pixel.
-template <bool kCandidatesOnly>
+template <bool kCandidatesOnly, bool kAdaptive = false>
 LTR_DEV void exact_pair(float x, float y, float z, uint32_t i, uint32_t k, const double* __restrict__ inv_pose, const double* __restrict__ ext,
                         int ext_identity, int order, const ImgShape& g, const uint32_t* __restrict__ scan_rimg, float thres,
                         uint64_t* __restrict__ win, int shortcut, unsigned* n_atomics) {
@@ -230,11 +236,11 @@ LTR_DEV void exact_pair(float x, float y, float z, uint32_t i, uint32_t k, const
     const Sph s = cart2sph(lx, ly, lz);
     int r, c;
     pixel_index(s, g, &r, &c);
-    offer<kCandidatesOnly>(win, (size_t)k * g.rows * g.cols + (size_t)r * g.cols + c, s.r, i, scan_rimg, thres, shortcut, n_atomics);
+    offer<kCandidatesOnly, kAdaptive>(win, (size_t)k * g.rows * g.cols + (size_t)r * g.cols + c, s.r, i, scan_rimg, thres, shortcut, n_atomics);
 }
 
 // Kind A: pixel index known to be right, only the exact range is needed (double transform + sqrt): ~60 instructions.
-template <bool kCandidatesOnly>
+template <bool kCandidatesOnly, bool kAdaptive = false>
 LTR_DEV void exact_range_pair(const PtrView& map, uint64_t e, const double* __restrict__ poses, int kf0, const double* __restrict__ ext,
                               int ext_identity, int order, uint32_t npx, const uint32_t* __restrict__ scan_rimg, float thres,
                               uint64_t* __restrict__ win, int shortcut, unsigned* n_atomics) {
@@ -242,18 +248,18 @@ LTR_DEV void exact_range_pair(const PtrView& map, uint64_t e, const double* __re
     float lx, ly, lz;
     map_to_sensor(poses + (size_t)(kf0 + k) * 24, ext, ext_identity, order, map.x[i], map.y[i], map.z[i], &lx, &ly, &lz);
     const float r = __fsqrt_rn(fa(fa(fm(lx, lx), fm(ly, ly)), fm(lz, lz)));   // == cart2sph().r
-    offer<kCandidatesOnly>(win, (size_t)k * npx + pxl, r, i, scan_rimg, thres, shortcut, n_atomics);
+    offer<kCandidatesOnly, kAdaptive>(win, (size_t)k * npx + pxl, r, i, scan_rimg, thres, shortcut, n_atomics);
 }
 
 // Kind B: nothing is known (pixel near a rounding boundary, degenerate geometry, keyframe without fast constants): the full reference
 // arithmetic, as in map_project_kernel.
-template <bool kCandidatesOnly>
+template <bool kCandidatesOnly, bool kAdaptive = false>
 __device__ __noinline__ void exact_full_pair(const PtrView& map, uint64_t e, const double* __restrict__ poses, int kf0,
                                              const double* __restrict__ ext, int ext_identity, int order, const ImgShape& g,
                                              const uint32_t* __restrict__ scan_rimg, float thres, uint64_t* __restrict__ win, int shortcut,
                                              unsigned* n_atomics) {
     const uint32_t i = (uint32_t)(e >> 32), k = (uint32_t)e & 0x3fffu;
-    exact_pair<kCandidatesOnly>(map.x[i], map.y[i], map.z[i], i, k, poses + (size_t)(kf0 + k) * 24, ext, ext_identity, order, g, scan_rimg, thres,
+    exact_pair<kCandidatesOnly, kAdaptive>(map.x[i], map.y[i], map.z[i], i, k, poses + (size_t)(kf0 + k) * 24, ext, ext_identity, order, g, scan_rimg, thres,
                                 win, shortcut, n_atomics);
 }
 
@@ -280,6 +286,10 @@ struct KfBatch { float kf[kFastMaxBatch][16]; };
 // `test_img` (u32 per pixel, float bits):
 //   kCandidatesOnly: the scan range image with "no return" pixels replaced by -inf when FastCfg::empty_scan_shortcut (built by
 //       scan_test_image_kernel): a pair can only matter if  scan - range > thres  for SOME range within the margin.
+//       kAdaptive (threshold t = fl(c s) per pixel, c in `thres`): the image holds v = fl_up(s - fl(c s)) >= s - t instead of s, and the
+//       certainty threshold is 0.  A candidate has fl(s - rho) > t, hence s - rho > t (t is a float and rounding is monotone), hence
+//       v - rho > 0: the test of the constant threshold with (v, 0) in place of (s, thres) keeps every candidate.  Rounding v up makes
+//       the rounding bound delta of fl(s - t) zero, for every pixel: a pixel without a return (s = 10000, no shortcut) included.
 //   otherwise: the running minimum `approx_min` itself.
 // `approx_min` (u32 per pixel, float bits, initialised to +inf): running minimum of the APPROXIMATE ranges of the pairs that were queued
 // for the pixel.  A pair whose approximate range exceeds it by more than twice the range margin is provably farther than an
@@ -312,7 +322,7 @@ struct DeferredArgs {
     const unsigned long long* order;   // tile claim order (low 32 bits: tile index), or nullptr: map order
 };
 
-template <bool kCandidatesOnly, bool kElDirect, bool kDeferred = false, bool kPad = false>
+template <bool kCandidatesOnly, bool kElDirect, bool kDeferred = false, bool kPad = false, bool kAdaptive = false>
 __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFastCtasPerSm) map_project_fast_kernel(PtrView map, const __grid_constant__ KfBatch kb, const double* __restrict__ poses,
                                                                         int kf0, int nb, const double* __restrict__ ext, int ext_identity, int order,
                                                                         ImgShape g, const __grid_constant__ FastCfg fc, const uint32_t* __restrict__ scan_rimg,
@@ -323,6 +333,7 @@ __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFast
     // kPad (scan-minus-map, short elevation path, 360 degree field of view): the test image is guard-padded (FastCfg::pad_*), so the
     // gather needs no index clamp
     static_assert(!kPad || (kCandidatesOnly && kElDirect && !kDeferred), "the padded test image exists for the scan-minus-map short path only");
+    static_assert(!kAdaptive || (kCandidatesOnly && !kDeferred), "the true minimum does not depend on the threshold");
     extern __shared__ uint64_t s_queues[];
     const int warp = threadIdx.x >> 5;
     uint64_t* s_qa = s_queues + warp * (2 * kQueueCap);
@@ -336,7 +347,8 @@ __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFast
     const uint32_t npx = (uint32_t)(g.rows * g.cols);
     const int hi_c = g.cols - 1, hi_r = g.rows - 1;
     const float kMagic = 12582912.0f;            // 1.5 * 2^23: v + kMagic has the nearest integer in its low mantissa bits
-    const float thr_lo = thres - fc.m_r_abs;
+    // kAdaptive: `thres` is the coefficient c, and the test image holds an upper bound of s - fl(c s), so that the certainty threshold is 0
+    const float thr_lo = (kAdaptive ? 0.0f : thres) - fc.m_r_abs;
     unsigned n_atomics = 0;
 #ifdef LTR_PROBE_NOMAYBE
     unsigned n_nomaybe = 0;
@@ -367,7 +379,7 @@ __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFast
     unsigned cull_mask = 0u;
     if (kCandidatesOnly && ca.enabled) {
         const float4 t = ca.tiles[tile];
-        const bool c = ((int)lane < nb) && tile_culled(kb.kf[lane], t, fc, g, ca, (int)lane, thres);
+        const bool c = ((int)lane < nb) && tile_culled<kAdaptive>(kb.kf[lane], t, fc, g, ca, (int)lane, thres);
         cull_mask = __ballot_sync(0xffffffffu, c);
         if (lane == 0) s_stat[warp][2] += __popc(cull_mask);
     }
@@ -518,13 +530,13 @@ __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFast
             while (qa >= 32) {
                 qa -= 32;
                 const uint64_t e = s_qa[qa + lane];
-                exact_range_pair<kCandidatesOnly>(map, e, poses, kf0, ext, ext_identity, order, npx, scan_rimg, thres, win, fc.empty_scan_shortcut, &n_atomics);
+                exact_range_pair<kCandidatesOnly, kAdaptive>(map, e, poses, kf0, ext, ext_identity, order, npx, scan_rimg, thres, win, fc.empty_scan_shortcut, &n_atomics);
                 if (lane == 0) s_stat[warp][0] += 32;
             }
             while (qb >= 32) {
                 qb -= 32;
                 const uint64_t e = s_qb[qb + lane];
-                exact_full_pair<kCandidatesOnly>(map, e, poses, kf0, ext, ext_identity, order, g, scan_rimg, thres, win, fc.empty_scan_shortcut, &n_atomics);
+                exact_full_pair<kCandidatesOnly, kAdaptive>(map, e, poses, kf0, ext, ext_identity, order, g, scan_rimg, thres, win, fc.empty_scan_shortcut, &n_atomics);
                 if (lane == 0) s_stat[warp][1] += 32;
             }
             __syncwarp();
@@ -535,10 +547,10 @@ __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFast
     }  // persistent tile loop
     const int qa = *(volatile int*)&s_cnt[warp][0], qb = *(volatile int*)&s_cnt[warp][1];
     if ((int)lane < qa) {
-        exact_range_pair<kCandidatesOnly>(map, s_qa[lane], poses, kf0, ext, ext_identity, order, npx, scan_rimg, thres, win, fc.empty_scan_shortcut, &n_atomics);
+        exact_range_pair<kCandidatesOnly, kAdaptive>(map, s_qa[lane], poses, kf0, ext, ext_identity, order, npx, scan_rimg, thres, win, fc.empty_scan_shortcut, &n_atomics);
     }
     if ((int)lane < qb) {
-        exact_full_pair<kCandidatesOnly>(map, s_qb[lane], poses, kf0, ext, ext_identity, order, g, scan_rimg, thres, win, fc.empty_scan_shortcut, &n_atomics);
+        exact_full_pair<kCandidatesOnly, kAdaptive>(map, s_qb[lane], poses, kf0, ext, ext_identity, order, g, scan_rimg, thres, win, fc.empty_scan_shortcut, &n_atomics);
     }
     // statistics: [0] pairs through the exact-range path (deferred mode: deferred_resolve_kernel adds the list entries), [1] atomics on
     // the winner image (deferred mode: plus those on `best`), [2] pairs through the full exact path, [3] culled pairs
