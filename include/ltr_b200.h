@@ -163,7 +163,7 @@ int ltr_remove_pass_adaptive(ltr_ctx* ctx, ltr_cloud map, ltr_scanset scans, ltr
                              int32_t mode, float res_alpha, float adaptive_coeff, int32_t accumulate, int64_t* n_dynamic);
 /* Drops the scan-side images ltr_remove_pass keeps; free_storage != 0 also returns their storage to the context's allocator cache. */
 int ltr_scan_images_release(ltr_ctx* ctx, int32_t free_storage);
-/* Device pointer to the N flag bytes of the last ltr_remove_pass on `map` (for an all-reduce hook). */
+/* Device pointer to the N flag bytes of the last ltr_remove_pass on `map` (for a caller's own all-reduce). */
 int ltr_flags_device_ptr(ltr_ctx* ctx, ltr_cloud map, uint8_t** flags, int64_t* n);
 int ltr_flags_download(ltr_ctx* ctx, ltr_cloud map, uint8_t* flags, int64_t capacity);
 int ltr_flags_upload(ltr_ctx* ctx, ltr_cloud map, const uint8_t* flags, int64_t n);

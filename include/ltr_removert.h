@@ -8,10 +8,10 @@
  * memory in the form the reference holds them after Session::loadKeyframes (Session.cpp:266-302):
  * per keyframe a cloud of x, y, z, intensity floats plus a pose and its inverse.
  *
- * Multi-GPU: one process per GPU, each owning a contiguous block of keyframes of both sessions; maps are
- * replicated.  The two exchange points of the path (per-pass dynamic-flag union, rank-ordered gather of
- * merged clouds) are expressed as the ltr_comm hooks below so that the caller chooses the transport
- * (torch.distributed/NCCL in bench.py; any NCCL communicator natively).
+ * Multi-GPU: one process per GPU, each owning a contiguous block of keyframes of one or both sessions; maps
+ * are replicated on the ranks that own a session.  What crosses ranks (per-pass dynamic-flag union,
+ * rank-ordered gather and distributed voxelisation of merged clouds, maps handed between the two session
+ * groups) goes through the native NCCL transport of ltr_b200.h (ltr_nccl_*), set up by ltrh_comm_init_nccl.
  */
 #ifndef LTR_REMOVERT_H_
 #define LTR_REMOVERT_H_
@@ -45,25 +45,10 @@ typedef struct ltrh_params {
     int32_t keyframe_batch, fast_path;           /* see ltr_config */
 } ltrh_params;
 
-/* Collective hooks; NULL pointers (or world == 1) mean single process.  Device pointers belong to the
- * context's GPU; the orchestrator synchronises its stream before calling a hook and expects the hook to
- * return after the data is in place (or ordered on the default stream and synchronised). */
-typedef struct ltr_comm {
-    int32_t rank, world;
-    void* user;
-    /* in-place max-reduction of n bytes across ranks (logical OR of the per-rank dynamic flags) */
-    int (*allreduce_max_u8)(void* user, uint8_t* dev, int64_t n);
-    /* all-gather of one int64 per rank into out[world] (host memory) */
-    int (*allgather_i64)(void* user, int64_t local, int64_t* out);
-    /* rank-ordered variable all-gather of float arrays: dst[displs[r] .. displs[r]+counts[r]) = rank r's src[0..counts[r]) */
-    int (*allgatherv_f32)(void* user, const float* dev_src, int64_t n_local, float* dev_dst, const int64_t* counts, const int64_t* displs);
-} ltr_comm;
-
 void ltrh_params_default(ltrh_params* p);
 int ltrh_create(ltrh_removerter** out, const ltrh_params* p);
 void ltrh_destroy(ltrh_removerter* r);
 const char* ltrh_last_error(const ltrh_removerter* r);
-int ltrh_set_comm(ltrh_removerter* r, const ltr_comm* comm);
 ltr_ctx* ltrh_context(ltrh_removerter* r);
 /* Native multi-GPU transport (ltr_nccl_* of ltr_b200.h; NCCL on the context's stream, no host code in the loop).  id128 = the 128 bytes
  * of ltr_nccl_unique_id() taken on one rank and shared with the others by the launcher.  split_sessions != 0 with an even world:

@@ -8,6 +8,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <cstdio>
+#include <utility>
 
 namespace ltremovert_b200 {
 
@@ -48,7 +49,6 @@ std::map<std::string, ltr_scanset*> Session::scanset_names() {
 Removerter::Removerter(const ltrh_params& p) : P(p) {
     central_sess_.sess_type_ = "Central"; central_sess_.id = 0;
     query_sess_.sess_type_ = "Query"; query_sess_.id = 1;
-    comm.rank = 0; comm.world = 1;
 }
 
 Removerter::~Removerter() {
@@ -125,14 +125,13 @@ int Removerter::save(const std::string& name, ltr_cloud c) {
 //   * Keyframe sharding: the ranks that own a session hold contiguous keyframe blocks of it (scans + poses) in rank order; every
 //     per-keyframe loop of the reference runs on the owner.  Maps are replicated on those ranks; after a pass the per-rank flag
 //     arrays are OR-ed (reduce_flags) and every rank applies the same partition / voxelisation, so replicas stay bit-identical.
-//     Clouds merged over all keyframes are concatenated in rank == keyframe order (gather_clouds).
+//     Clouds merged over all keyframes are concatenated in rank == keyframe order (gather_cloud).
 //   * Session split (world even, split_sessions): ranks [0, world/2) own the central session, the others the query session.
 //     Step 1 of the two sessions (Removerter.cpp:1584 / 1587) and the two halves of Step 2 are independent, so the two groups
 //     run them concurrently and the replicated per-pass work (partition, voxelisation) is done once per group, not once per
 //     rank.  A map crosses groups exactly where the reference reads the other session's member: rank r hands it to rank
 //     r + world/2 (exchange_with_partner), one peer-to-peer transfer per rank pair.
 // Transport: the native NCCL entry points of libltr_b200.so (ltr_nccl_*), on the context's stream, no host code in the loop.
-// The legacy ltr_comm hooks remain for host-memory tests of the exchange logic (no session split).
 // ---------------------------------------------------------------------------------------------------------------
 int Removerter::comm_init_nccl(const uint8_t* id128, int rank_, int world_, int split_sessions) {
     if (world_ < 1 || rank_ < 0 || rank_ >= world_) return fail(LTR_ERR_INVALID, "bad rank / world");
@@ -152,49 +151,15 @@ int Removerter::comm_init_nccl(const uint8_t* id128, int rank_, int world_, int 
 }
 
 int Removerter::reduce_flags(ltr_cloud map, const Session& over) {
-    if (nccl_world >= 0) {
-        if (group_world <= 1) return LTR_OK;
-        return ltr_nccl_allreduce_flags(ctx, nccl_group[over.id], map) == LTR_OK ? LTR_OK : fail(LTR_ERR_CUDA, ltr_last_error(ctx));
-    }
-    if (!has_comm || comm.world <= 1) return LTR_OK;
-    uint8_t* p; int64_t n;
-    CK(ltr_flags_device_ptr(ctx, map, &p, &n));
-    CK(ltr_synchronize(ctx));
-    if (n > 0 && comm.allreduce_max_u8(comm.user, p, n) != 0) return fail(LTR_ERR_CUDA, "allreduce_max_u8 hook failed");
-    return LTR_OK;
+    if (!sharded()) return LTR_OK;
+    return ltr_nccl_allreduce_flags(ctx, nccl_group[over.id], map) == LTR_OK ? LTR_OK : fail(LTR_ERR_CUDA, ltr_last_error(ctx));
 }
 
-int Removerter::gather_clouds(const Session& over, int n, ltr_cloud** clouds) {
-    if (nccl_world >= 0) {
-        if (group_world <= 1) return LTR_OK;
-        ltr_cloud local[16] = {0}, out[16] = {0};
-        if (n > 16) return fail(LTR_ERR_INVALID, "too many clouds in one gather");
-        for (int i = 0; i < n; ++i) local[i] = *clouds[i];
-        CK(ltr_nccl_allgather_clouds(ctx, nccl_group[over.id], n, local, out));
-        for (int i = 0; i < n; ++i) CK(set(clouds[i], out[i]));
-        return LTR_OK;
-    }
-    if (!has_comm || comm.world <= 1) return LTR_OK;
-    for (int i = 0; i < n; ++i) {
-        ltr_cloud* cloud = clouds[i];
-        float *sx, *sy, *sz, *si; int64_t m;
-        CK(ltr_cloud_device_ptrs(ctx, *cloud, &sx, &sy, &sz, &si, &m));
-        std::vector<int64_t> counts((size_t)comm.world), displs((size_t)comm.world);
-        if (comm.allgather_i64(comm.user, m, counts.data()) != 0) return fail(LTR_ERR_CUDA, "allgather_i64 hook failed");
-        int64_t total = 0;
-        for (int r = 0; r < comm.world; ++r) { displs[r] = total; total += counts[r]; }
-        ltr_cloud g;
-        CK(ltr_cloud_alloc(ctx, total, &g));
-        float *dx, *dy, *dz, *di; int64_t mm;
-        CK(ltr_cloud_device_ptrs(ctx, g, &dx, &dy, &dz, &di, &mm));
-        CK(ltr_synchronize(ctx));
-        const float* src[4] = {sx, sy, sz, si};
-        float* dst[4] = {dx, dy, dz, di};
-        for (int c = 0; c < 4; ++c)
-            if (comm.allgatherv_f32(comm.user, src[c], m, dst[c], counts.data(), displs.data()) != 0) return fail(LTR_ERR_CUDA, "allgatherv_f32 hook failed");
-        CK(set(cloud, g));
-    }
-    return LTR_OK;
+int Removerter::gather_cloud(const Session& over, ltr_cloud* cloud) {
+    if (!sharded()) return LTR_OK;
+    ltr_cloud g;
+    CK(ltr_nccl_allgather_clouds(ctx, nccl_group[over.id], 1, cloud, &g));
+    return set(cloud, g);
 }
 
 int Removerter::exchange_with_partner(int n_send, const ltr_cloud* send, int n_recv, ltr_cloud* recv) {
@@ -203,25 +168,25 @@ int Removerter::exchange_with_partner(int n_send, const ltr_cloud* send, int n_r
 }
 
 int Removerter::load_session(int sess, const float* xyzi, const int64_t* offsets, const double* poses, const double* inv_poses, int K) {
-    Session& S = sess == 0 ? central_sess_ : query_sess_;
-    ltr_scanset ss; ltr_poses ps;
+    ltr_scanset ss;
     CK(ltr_scanset_upload(ctx, xyzi, offsets, K, &ss));
-    CK(ltr_poses_upload(ctx, poses, inv_poses, K, &ps));
-    CK(set(&S.keyframe_scans_, ss, true));
-    if (S.keyframe_poses_ >= 0) CK(ltr_poses_free(ctx, S.keyframe_poses_));
-    S.keyframe_poses_ = ps;
-    S.num_keyframes_ = K;
-    return LTR_OK;
+    return load_session_scans(sess, ss, poses, inv_poses, K);
 }
 
 int Removerter::load_session_raw(int sess, const float* xyzi, const int64_t* offsets, const double* poses, const double* inv_poses, int K,
                                  int32_t* n_overflowed) {
-    Session& S = sess == 0 ? central_sess_ : query_sess_;
-    ltr_scanset raw, ss; ltr_poses ps;
+    ltr_scanset raw, ss;
     CK(ltr_scanset_upload(ctx, xyzi, offsets, K, &raw));
     const int rc = ltr_voxel_grid_per_keyframe(ctx, raw, P.downsample_voxel_size, &ss, n_overflowed);   // Session.cpp:284-289
     ltr_scanset_free(ctx, raw);
     CK(rc);
+    return load_session_scans(sess, ss, poses, inv_poses, K);
+}
+
+// the common tail of both loads: the device scan set `ss` and the uploaded poses become the session's keyframes
+int Removerter::load_session_scans(int sess, ltr_scanset ss, const double* poses, const double* inv_poses, int K) {
+    Session& S = sess == 0 ? central_sess_ : query_sess_;
+    ltr_poses ps;
     CK(ltr_poses_upload(ctx, poses, inv_poses, K, &ps));
     CK(set(&S.keyframe_scans_, ss, true));
     if (S.keyframe_poses_ >= 0) CK(ltr_poses_free(ctx, S.keyframe_poses_));
@@ -239,7 +204,7 @@ int Removerter::octreeDownsampling(ltr_cloud* cloud, float leaf) {
 int Removerter::octreeDownsamplingAppended(ltr_cloud* cloud, float leaf) {
     int64_t n = 0;
     CK(ltr_cloud_size(ctx, *cloud, &n));
-    if (!(nccl_world >= 0 && group_world > 1) || n < dist_voxel_min) return octreeDownsampling(cloud, leaf);
+    if (!sharded() || n < dist_voxel_min) return octreeDownsampling(cloud, leaf);
     const int g = nccl_group[0];            // the rank's own group (both entries are the same communicator)
     int32_t r = 0, w = 1;
     CK(ltr_nccl_info(ctx, g, &r, &w));
@@ -251,29 +216,17 @@ int Removerter::octreeDownsamplingAppended(ltr_cloud* cloud, float leaf) {
     return set(cloud, v);
 }
 
-int Removerter::mergeScansWithinGlobalCoordUtil(Session& s, ltr_scanset scans, ltr_cloud* out) {
-    ltr_cloud m;
-    CK(ltr_merge_scans_global(ctx, scans, s.keyframe_poses_, &m));
-    CK(gather_cloud(s, &m));  // keyframe order == rank order (contiguous keyframe blocks)
-    *out = m;
+int Removerter::voxeliseMerged(Session& s, ltr_cloud merged, float leaf, ltr_cloud* out) {
+    CK(sharded() ? ltr_nccl_voxel_centroid_merged(ctx, nccl_group[s.id], merged, leaf, out) : ltr_voxel_centroid(ctx, merged, leaf, out));
     return LTR_OK;
 }
 
 int Removerter::mergeAndDownsample(Session& s, ltr_scanset scans, float leaf, ltr_cloud* out) {
-    if (nccl_world >= 0 && group_world > 1) {
-        ltr_cloud m, v;
-        CK(ltr_merge_scans_global(ctx, scans, s.keyframe_poses_, &m));      // this rank's keyframes only
-        const int rc = ltr_nccl_voxel_centroid_merged(ctx, nccl_group[s.id], m, leaf, &v);
-        ltr_cloud_free(ctx, m);
-        if (rc != LTR_OK) return fail(rc, ltr_last_error(ctx));
-        *out = v;
-        return LTR_OK;
-    }
     ltr_cloud m;
-    CK(mergeScansWithinGlobalCoordUtil(s, scans, &m));
-    CK(octreeDownsampling(&m, leaf));
-    *out = m;
-    return LTR_OK;
+    CK(ltr_merge_scans_global(ctx, scans, s.keyframe_poses_, &m));      // this rank's keyframes
+    const int rc = voxeliseMerged(s, m, leaf, out);
+    ltr_cloud_free(ctx, m);
+    return rc;
 }
 
 int Removerter::precleaningKeyframes(float radius) {
@@ -287,19 +240,13 @@ int Removerter::precleaningKeyframes(float radius) {
 }
 
 int Removerter::makeGlobalMap(Session& s) {
+    // with several ranks the voxelised map comes from the distributed voxeliser (each rank sorts its key range of the ~10^8 raw points);
+    // map_global_orig_ keeps its meaning (the merged raw cloud of ALL keyframes) through a gather afterwards, in keyframe == rank order
     ltr_cloud orig, curr;
-    if (nccl_world >= 0 && group_world > 1) {
-        // several ranks: the voxelised map comes from the distributed voxeliser (each rank sorts its key range of the ~10^8 raw points);
-        // map_global_orig_ keeps its meaning (the merged raw cloud of ALL keyframes) through a plain gather afterwards
-        CK(ltr_merge_scans_global(ctx, s.keyframe_scans_, s.keyframe_poses_, &orig));       // _sess.mergeScansWithinGlobalCoord() (:218), this rank's keyframes
-        if (ltr_nccl_voxel_centroid_merged(ctx, nccl_group[s.id], orig, P.downsample_voxel_size, &curr) != LTR_OK) return fail(LTR_ERR_CUDA, ltr_last_error(ctx));   // :225
-        CK(gather_cloud(s, &orig));
-        CK(set(&s.map_global_orig_, orig));
-    } else {
-        CK(mergeScansWithinGlobalCoordUtil(s, s.keyframe_scans_, &orig));       // _sess.mergeScansWithinGlobalCoord() (:218)
-        CK(set(&s.map_global_orig_, orig));
-        CK(ltr_voxel_centroid(ctx, s.map_global_orig_, P.downsample_voxel_size, &curr));  // :225
-    }
+    CK(ltr_merge_scans_global(ctx, s.keyframe_scans_, s.keyframe_poses_, &orig));   // _sess.mergeScansWithinGlobalCoord() (:218), this rank's keyframes
+    CK(voxeliseMerged(s, orig, P.downsample_voxel_size, &curr));                    // :225
+    CK(gather_cloud(s, &orig));
+    CK(set(&s.map_global_orig_, orig));
     CK(set(&s.map_global_curr_, curr));
     CK(save("OriginalNoisy" + s.sess_type_ + "MapGlobal", s.map_global_curr_));       // :231
     return LTR_OK;
@@ -310,78 +257,61 @@ int Removerter::makeGlobalMap() {
     return LTR_OK;
 }
 
-// partitionCurrentMap / ForND / ForPD (:801-828, 771-799, 740-768)
-int Removerter::partitionCurrentMapGeneric(ltr_cloud map, Session& source, ltr_scanset scans, int mode, float res, const char* what,
-                                           ltr_cloud* stat, ltr_cloud* dyn) {
+// partitionCurrentMap / ForND / ForPD (:801-828, 771-799, 740-768) and the statements of removeOnce / revertOnce / iremoveOnceForND /
+// removeOnceForPD that follow it: the kept side (dynamic for revertOnce, static for the others) replaces its slot, is voxelised and becomes
+// the new *map; the other side is appended to its slot and voxelised.  Only the HD passes' appended maps go through the distributed voxeliser.
+int Removerter::partitionCurrentMapGeneric(ltr_cloud* map, Session& source, ltr_scanset scans, int mode, float res, const char* what,
+                                           bool keep_dynamic, ltr_cloud* stat, ltr_cloud* dyn) {
     int64_t n_map = 0;
-    CK(ltr_cloud_size(ctx, map, &n_map));
+    CK(ltr_cloud_size(ctx, *map, &n_map));
     // n_dynamic is taken from the partition below (after the cross-rank flag union), so no count is requested here
     if (adaptiveThresholdCoeff_ != 0.0f)   // Removerter.cpp:396 in place of :398, for every variant
-        CK(ltr_remove_pass_adaptive(ctx, map, scans, source.keyframe_poses_, 0, source.num_keyframes_, mode, res, adaptiveThresholdCoeff_, 0, nullptr));
+        CK(ltr_remove_pass_adaptive(ctx, *map, scans, source.keyframe_poses_, 0, source.num_keyframes_, mode, res, adaptiveThresholdCoeff_, 0, nullptr));
     else
-        CK(ltr_remove_pass(ctx, map, scans, source.keyframe_poses_, 0, source.num_keyframes_, mode, res, 0.1f, 0, nullptr));
-    CK(reduce_flags(map, source));
-    CK(ltr_apply_partition(ctx, map, stat, dyn));
+        CK(ltr_remove_pass(ctx, *map, scans, source.keyframe_poses_, 0, source.num_keyframes_, mode, res, 0.1f, 0, nullptr));
+    CK(reduce_flags(*map, source));
+    ltr_cloud st, dy;
+    CK(ltr_apply_partition(ctx, *map, &st, &dy));
     int64_t n_dyn = 0;
-    CK(ltr_cloud_size(ctx, *dyn, &n_dyn));
+    CK(ltr_cloud_size(ctx, dy, &n_dyn));
     log.push_back(PassLog{what, n_map, n_dyn, -1, -1});
+
+    ltr_cloud *kept_slot = stat, *appended_slot = dyn;
+    ltr_cloud kept = st, appended = dy;
+    if (keep_dynamic) { std::swap(kept_slot, appended_slot); std::swap(kept, appended); }
+    CK(set(kept_slot, kept));
+    CK(octreeDownsampling(kept_slot, 0.05f));
+    CK(assign(map, *kept_slot));
+    CK(append(appended_slot, appended));
+    CK(ltr_cloud_free(ctx, appended));
+    CK(mode == LTR_MODE_HD ? octreeDownsamplingAppended(appended_slot, 0.05f) : octreeDownsampling(appended_slot, 0.05f));
+    CK(ltr_cloud_size(ctx, *stat, &log.back().n_static_after));
+    CK(ltr_cloud_size(ctx, *dyn, &log.back().n_dynamic_after));
     return LTR_OK;
 }
 
+// keep static :894-895, voxelise :896, map :899-900, append dynamic :902, voxelise :903
 int Removerter::removeOnce(Session& t, Session& s, float res) {
-    ltr_cloud st, dy;
-    CK(partitionCurrentMapGeneric(t.map_global_curr_, s, s.keyframe_scans_, LTR_MODE_HD, res, "removeOnce", &st, &dy));
-    CK(set(&t.map_global_curr_static_, st));                       // :894-895
-    CK(octreeDownsampling(&t.map_global_curr_static_, 0.05f));     // :896
-    CK(assign(&t.map_global_curr_, t.map_global_curr_static_));    // :899-900
-    CK(append(&t.map_global_curr_dynamic_, dy));                   // :902
-    CK(ltr_cloud_free(ctx, dy));
-    CK(octreeDownsamplingAppended(&t.map_global_curr_dynamic_, 0.05f));    // :903
-    CK(ltr_cloud_size(ctx, t.map_global_curr_static_, &log.back().n_static_after));
-    CK(ltr_cloud_size(ctx, t.map_global_curr_dynamic_, &log.back().n_dynamic_after));
-    return LTR_OK;
+    return partitionCurrentMapGeneric(&t.map_global_curr_, s, s.keyframe_scans_, LTR_MODE_HD, res, "removeOnce", false,
+                                      &t.map_global_curr_static_, &t.map_global_curr_dynamic_);
 }
 
+// keep dynamic :919-920, voxelise :921, map :924-925, append static :927, voxelise :928
 int Removerter::revertOnce(Session& t, Session& s, float res) {
-    ltr_cloud st, dy;
-    CK(partitionCurrentMapGeneric(t.map_global_curr_, s, s.keyframe_scans_, LTR_MODE_HD, res, "revertOnce", &st, &dy));
-    CK(set(&t.map_global_curr_dynamic_, dy));                      // :919-920
-    CK(octreeDownsampling(&t.map_global_curr_dynamic_, 0.05f));    // :921
-    CK(assign(&t.map_global_curr_, t.map_global_curr_dynamic_));   // :924-925
-    CK(append(&t.map_global_curr_static_, st));                    // :927
-    CK(ltr_cloud_free(ctx, st));
-    CK(octreeDownsamplingAppended(&t.map_global_curr_static_, 0.05f));     // :928
-    CK(ltr_cloud_size(ctx, t.map_global_curr_static_, &log.back().n_static_after));
-    CK(ltr_cloud_size(ctx, t.map_global_curr_dynamic_, &log.back().n_dynamic_after));
-    return LTR_OK;
+    return partitionCurrentMapGeneric(&t.map_global_curr_, s, s.keyframe_scans_, LTR_MODE_HD, res, "revertOnce", true,
+                                      &t.map_global_curr_static_, &t.map_global_curr_dynamic_);
 }
 
+// keep strong :843-844, voxelise :845, map :848-849, append weak :851, voxelise :852
 int Removerter::iremoveOnceForND(Session& t, Session& s, float res) {
-    ltr_cloud st, dy;
-    CK(partitionCurrentMapGeneric(t.map_global_nd_, s, s.keyframe_scans_static_projected_, LTR_MODE_ND, res, "iremoveOnceForND", &st, &dy));
-    CK(set(&t.map_global_nd_strong_, st));                         // :843-844
-    CK(octreeDownsampling(&t.map_global_nd_strong_, 0.05f));       // :845
-    CK(assign(&t.map_global_nd_, t.map_global_nd_strong_));        // :848-849
-    CK(append(&t.map_global_nd_weak_, dy));                        // :851
-    CK(ltr_cloud_free(ctx, dy));
-    CK(octreeDownsampling(&t.map_global_nd_weak_, 0.05f));         // :852
-    CK(ltr_cloud_size(ctx, t.map_global_nd_strong_, &log.back().n_static_after));
-    CK(ltr_cloud_size(ctx, t.map_global_nd_weak_, &log.back().n_dynamic_after));
-    return LTR_OK;
+    return partitionCurrentMapGeneric(&t.map_global_nd_, s, s.keyframe_scans_static_projected_, LTR_MODE_ND, res, "iremoveOnceForND", false,
+                                      &t.map_global_nd_strong_, &t.map_global_nd_weak_);
 }
 
+// keep strong :868-869, voxelise :870, map :873-874, append weak :876, voxelise :878
 int Removerter::removeOnceForPD(Session& t, Session& s, float res) {
-    ltr_cloud st, dy;
-    CK(partitionCurrentMapGeneric(t.map_global_pd_, s, s.keyframe_scans_static_projected_, LTR_MODE_PD, res, "removeOnceForPD", &st, &dy));
-    CK(set(&t.map_global_pd_strong_, st));                         // :868-869
-    CK(octreeDownsampling(&t.map_global_pd_strong_, 0.05f));       // :870
-    CK(assign(&t.map_global_pd_, t.map_global_pd_strong_));        // :873-874
-    CK(append(&t.map_global_pd_weak_, dy));                        // :876
-    CK(ltr_cloud_free(ctx, dy));
-    CK(octreeDownsampling(&t.map_global_pd_weak_, 0.05f));         // :878
-    CK(ltr_cloud_size(ctx, t.map_global_pd_strong_, &log.back().n_static_after));
-    CK(ltr_cloud_size(ctx, t.map_global_pd_weak_, &log.back().n_dynamic_after));
-    return LTR_OK;
+    return partitionCurrentMapGeneric(&t.map_global_pd_, s, s.keyframe_scans_static_projected_, LTR_MODE_PD, res, "removeOnceForPD", false,
+                                      &t.map_global_pd_strong_, &t.map_global_pd_weak_);
 }
 
 int Removerter::resetCurrrentMapAsDynamic(Session& s, bool as_dynamic) {
@@ -789,14 +719,6 @@ int ltrh_create(ltrh_removerter** out, const ltrh_params* p) {
 }
 void ltrh_destroy(ltrh_removerter* r) { if (r) { delete r->R; delete r; } }
 const char* ltrh_last_error(const ltrh_removerter* r) { return r ? r->R->err.c_str() : g_err.c_str(); }
-int ltrh_set_comm(ltrh_removerter* r, const ltr_comm* comm) {
-    if (!r) return LTR_ERR_INVALID;
-    if (!comm) { r->R->has_comm = false; return LTR_OK; }
-    if (comm->world > 1 && (!comm->allreduce_max_u8 || !comm->allgather_i64 || !comm->allgatherv_f32)) { r->R->err = "comm hooks missing"; return LTR_ERR_INVALID; }
-    r->R->comm = *comm;
-    r->R->has_comm = true;
-    return LTR_OK;
-}
 ltr_ctx* ltrh_context(ltrh_removerter* r) { return r ? r->R->ctx : nullptr; }
 int ltrh_comm_init_nccl(ltrh_removerter* r, const uint8_t* id128, int32_t rank, int32_t world, int32_t split_sessions) {
     if (!r || !id128) return LTR_ERR_INVALID;

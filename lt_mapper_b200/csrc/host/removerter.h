@@ -89,13 +89,15 @@ public:
     int constructGlobalNDMap(Session& s);                                                  // Session.cpp:430-435
     int constructGlobalPDMap(Session& s);                                                  // Session.cpp:437-445
     int removeWeakNDMapPointsHavingStrongNDInNear(Session& s);                             // Session.cpp:452-484
-    int mergeScansWithinGlobalCoordUtil(Session& s, ltr_scanset scans, ltr_cloud* out);    // utility.cpp:170-192 (+ rank gather)
     int octreeDownsampling(ltr_cloud* cloud, float leaf);                                  // utility.cpp:204-219, in place
     // the same for a freshly appended cloud ("*a += *b", never in octree order): with several ranks every rank contributes its slice of
     // the (replicated) cloud to the distributed voxeliser, so each sorts 1/G of it instead of all of it
     int octreeDownsamplingAppended(ltr_cloud* cloud, float leaf);
-    // mergeScansWithinGlobalCoordUtil followed by octreeDownsampling of the result (the only way the path consumes a merged cloud):
-    // with several ranks the raw merged cloud is never gathered (ltr_nccl_voxel_centroid_merged)
+    // octreeDownsampling of the cloud merged over ALL keyframes of s, given this rank's part `merged` (not consumed): with several
+    // ranks the parts are voxelised together without being gathered (ltr_nccl_voxel_centroid_merged)
+    int voxeliseMerged(Session& s, ltr_cloud merged, float leaf, ltr_cloud* out);
+    // mergeScansWithinGlobalCoordUtil (utility.cpp:170-192) followed by octreeDownsampling of the result, the only way the path
+    // consumes a merged cloud apart from map_global_orig_
     int mergeAndDownsample(Session& s, ltr_scanset scans, float leaf, ltr_cloud* out);
 
     // ---- plumbing ----
@@ -112,11 +114,11 @@ public:
     // ---- multi-GPU (SURVEY.md section 8e; see "Parallel decomposition" in removerter.cpp) ----
     int comm_init_nccl(const uint8_t* id128, int rank, int world, int split_sessions);   // native NCCL transport (ltr_nccl_*)
     bool owns(const Session& s) const { return !split || (rank < world / 2) == (s.id == 0); }
-    bool multi() const { return world > 1; }
+    // the session(s) this rank owns are sharded over more than one rank: flags, merged clouds and appended maps cross ranks
+    bool sharded() const { return group_world > 1; }
     int partner() const { return (rank + world / 2) % world; }
     int reduce_flags(ltr_cloud map, const Session& over);               // OR of the dynamic flags over the ranks that own `over`'s keyframes
-    int gather_clouds(const Session& over, int n, ltr_cloud** clouds);  // each *clouds[i] <- rank-ordered concatenation over those ranks
-    int gather_cloud(const Session& over, ltr_cloud* cloud) { ltr_cloud* one[1] = {cloud}; return gather_clouds(over, 1, one); }
+    int gather_cloud(const Session& over, ltr_cloud* cloud);            // *cloud <- rank-ordered concatenation over those ranks
     int exchange_with_partner(int n_send, const ltr_cloud* send, int n_recv, ltr_cloud* recv);   // split mode only
     int fail(int code, const std::string& msg);
 
@@ -124,13 +126,11 @@ public:
     bool useICPrefinement_ = false;   // Session.cpp:551 (`bool useICPrefinement { false }`), set by ltrh_set_icp_refinement
     float adaptiveThresholdCoeff_ = 0.0f;   // Removerter.cpp:395-396 (`adaptive_coeff`, commented out); 0: the constant 0.1 (:398), set by ltrh_set_adaptive_threshold
     ltr_ctx* ctx = nullptr;
-    ltr_comm comm{};          // legacy caller-supplied hooks (host-memory tests); superseded by the native transport when nccl_world >= 0
-    bool has_comm = false;
     int rank = 0, world = 1;
     bool split = false;       // session-split: ranks [0, world/2) own the central keyframes, the others the query keyframes
     int nccl_world = -1;      // ltr_nccl communicator handles: everyone, ...
     int nccl_group[2] = {-1, -1};   // ... and the ranks that own session s
-    int group_world = 1;
+    int group_world = 1;      // size of this rank's owner group (1 until comm_init_nccl)
     // appended (replicated) clouds of at least this many points go through the distributed voxeliser, every rank contributing a slice.
     // Off by default: on 4 NVLinked ranks the two size exchanges + the exchange + the gather of a ~10 M point cloud cost more than sorting it on
     // every rank; LTR_DIST_VOXEL_MIN turns it on (the multi-rank tests do).
@@ -142,8 +142,9 @@ public:
     std::string err;
 
 private:
-    int partitionCurrentMapGeneric(ltr_cloud map, Session& source, ltr_scanset scans, int mode, float res, const char* what,
-                                   ltr_cloud* stat, ltr_cloud* dyn);
+    int load_session_scans(int sess, ltr_scanset ss, const double* poses, const double* inv_poses, int K);
+    int partitionCurrentMapGeneric(ltr_cloud* map, Session& source, ltr_scanset scans, int mode, float res, const char* what,
+                                   bool keep_dynamic, ltr_cloud* stat, ltr_cloud* dyn);
 };
 
 }  // namespace ltremovert_b200

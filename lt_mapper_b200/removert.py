@@ -2,8 +2,8 @@
 
 `Removerter` mirrors ltremovert::Removerter (ltremovert/src/Removerter.cpp:1653-1678): load two sessions,
 run Step 0 / Step 1+2 / Step 3, read back named clouds.  All work happens in the C++ orchestrator and the
-CUDA library underneath; this module only moves numpy arrays across the C-ABI and, for multi-GPU runs,
-provides the collective hooks on top of torch.distributed (NCCL).
+CUDA library underneath; this module only moves numpy arrays across the C-ABI.  Multi-GPU runs use the
+library's native NCCL transport (`Removerter.init_nccl`).
 """
 import ctypes
 import os
@@ -29,18 +29,7 @@ class Params(ctypes.Structure):
                 ("transform_order", ctypes.c_int32), ("keyframe_batch", ctypes.c_int32), ("fast_path", ctypes.c_int32)]
 
 
-_ALLREDUCE = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64)
-_ALLGATHER_I64 = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.c_int64, ctypes.POINTER(ctypes.c_int64))
-_ALLGATHERV = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
-                               ctypes.POINTER(ctypes.c_int64), ctypes.POINTER(ctypes.c_int64))
-
-
-class Comm(ctypes.Structure):
-    _fields_ = [("rank", ctypes.c_int32), ("world", ctypes.c_int32), ("user", ctypes.c_void_p),
-                ("allreduce_max_u8", _ALLREDUCE), ("allgather_i64", _ALLGATHER_I64), ("allgatherv_f32", _ALLGATHERV)]
-
-
-HOST_EXPORTS = ["ltrh_params_default", "ltrh_create", "ltrh_destroy", "ltrh_last_error", "ltrh_set_comm", "ltrh_context", "ltrh_comm_init_nccl", "ltrh_owns_session", "ltrh_invert_poses",
+HOST_EXPORTS = ["ltrh_params_default", "ltrh_create", "ltrh_destroy", "ltrh_last_error", "ltrh_context", "ltrh_comm_init_nccl", "ltrh_owns_session", "ltrh_invert_poses",
                 "ltrh_load_session", "ltrh_load_session_raw", "ltrh_run_step0", "ltrh_run_step12", "ltrh_run_step3", "ltrh_reset_to_step0", "ltrh_cascade_promote_updated", "ltrh_scanside_removal", "ltrh_set_icp_refinement", "ltrh_set_adaptive_threshold", "ltrh_icp_stats", "ltrh_stage", "ltrh_cloud",
                 "ltrh_scanset", "ltrh_timing", "ltrh_log_count", "ltrh_log_get", "ltrh_io_last_error", "ltrh_io_read_pcd", "ltrh_io_write_pcd",
                 "ltrh_io_read_poses", "ltrh_io_parse_keyframes", "ltrh_io_parse_keyframes_in_roi", "ltrh_io_voxel_grid", "ltrh_io_voxel_grid_scans", "ltrh_io_yaml_get"]
@@ -63,7 +52,6 @@ def host_lib():
     L.ltrh_destroy.restype = None
     L.ltrh_last_error.argtypes = [vp]
     L.ltrh_last_error.restype = ctypes.c_char_p
-    L.ltrh_set_comm.argtypes = [vp, P(Comm)]
     L.ltrh_context.argtypes = [vp]
     L.ltrh_context.restype = vp
     L.ltrh_comm_init_nccl.argtypes = [vp, vp, i32, i32, i32]
@@ -101,104 +89,6 @@ def host_lib():
     return L
 
 
-class _DevArray:
-    """Minimal __cuda_array_interface__ wrapper so torch can alias raw device memory without a copy."""
-
-    def __init__(self, ptr, n, typestr):
-        self.__cuda_array_interface__ = {"shape": (int(n),), "typestr": typestr, "data": (int(ptr), False), "version": 2}
-
-
-class TorchDistComm:
-    """ltr_comm hooks on top of torch.distributed (NCCL for CUDA tensors; gloo works through host staging in tests)."""
-
-    def __init__(self, group=None):
-        import torch
-        import torch.distributed as dist
-        self.torch, self.dist, self.group = torch, dist, group
-        self.rank, self.world = dist.get_rank(group), dist.get_world_size(group)
-        self.backend = dist.get_backend(group)
-        self.device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
-        self.trace = os.environ.get("LTR_COMM_TRACE") == "1"
-        self.stats = {"allreduce": [0, 0.0, 0], "allgather_i64": [0, 0.0, 0], "allgatherv": [0, 0.0, 0]}   # calls, seconds, bytes
-        self._cb = (_ALLREDUCE(self._timed("allreduce", self._allreduce)), _ALLGATHER_I64(self._timed("allgather_i64", self._allgather_i64)),
-                    _ALLGATHERV(self._timed("allgatherv", self._allgatherv)))
-        self.struct = Comm(self.rank, self.world, None, *self._cb)
-
-    def _timed(self, name, fn):
-        import time
-
-        def wrapped(*a):
-            t0 = time.perf_counter()
-            rc = fn(*a)
-            st = self.stats[name]
-            st[0] += 1
-            st[1] += time.perf_counter() - t0
-            st[2] += int(a[2]) * (1 if name == "allreduce" else 4) if name != "allgather_i64" else 8
-            return rc
-        return wrapped
-
-    def _tensor(self, ptr, n, typestr, dtype):
-        if self.device.type == "cuda":
-            return self.torch.as_tensor(_DevArray(ptr, n, typestr), device=self.device)
-        # host memory (gloo tests of the hook logic): alias the buffer through numpy
-        ct = ctypes.c_uint8 if typestr == "|u1" else ctypes.c_float
-        arr = np.ctypeslib.as_array(ctypes.cast(ctypes.c_void_p(ptr), ctypes.POINTER(ct)), shape=(int(n),))
-        return self.torch.from_numpy(arr)
-
-    def _sync(self):
-        if self.device.type == "cuda":
-            self.torch.cuda.synchronize()
-
-    def _allreduce(self, user, dev, n):
-        try:
-            t = self._tensor(dev, n, "|u1", self.torch.uint8)
-            self.dist.all_reduce(t, op=self.dist.ReduceOp.MAX, group=self.group)
-            self._sync()
-            return 0
-        except Exception as e:  # noqa: BLE001 -- must not propagate through the C frame
-            print("allreduce hook failed:", e)
-            return 1
-
-    def _allgather_i64(self, user, local, out):
-        try:
-            t = self.torch.tensor([local], dtype=self.torch.int64, device=self.device)
-            g = [self.torch.zeros_like(t) for _ in range(self.world)]
-            self.dist.all_gather(g, t, group=self.group)
-            for r in range(self.world):
-                out[r] = int(g[r].item())
-            return 0
-        except Exception as e:  # noqa: BLE001
-            print("allgather_i64 hook failed:", e)
-            return 1
-
-    def _allgatherv(self, user, src, n_local, dst, counts, displs):
-        try:
-            torch = self.torch
-            cnt = [int(counts[r]) for r in range(self.world)]
-            total = sum(cnt)
-            if total == 0:
-                return 0
-            mx = max(cnt)
-            send = torch.zeros(mx, dtype=torch.float32, device=self.device)
-            if n_local > 0:
-                send[:n_local] = self._tensor(src, n_local, "<f4", torch.float32)
-            recv = torch.empty(mx * self.world, dtype=torch.float32, device=self.device)
-            if self.backend == "gloo":
-                self.dist.all_gather(list(recv.view(self.world, mx).unbind(0)), send, group=self.group)
-            else:
-                self.dist.all_gather_into_tensor(recv, send, group=self.group)
-            out = self._tensor(dst, total, "<f4", torch.float32)
-            for r in range(self.world):
-                if cnt[r]:
-                    d = int(displs[r])
-                    out[d:d + cnt[r]] = recv[r * mx:r * mx + cnt[r]]
-            self._sync()
-            return 0
-        except Exception as e:  # noqa: BLE001
-            print("allgatherv hook failed:", e)
-            return 1
-
-
 def inverse_poses(poses):
     """Inverse keyframe poses as the reference computes them (general 4x4 cofactor inverse, Session.cpp:110); np.linalg.inv differs in the
     last bits, which is enough to move a few emitted coordinates by one ulp."""
@@ -229,7 +119,7 @@ def selfremovert_schedule(resolutions):
 class Removerter:
     def __init__(self, device=0, vfov=50.0, hfov=360.0, lidar2base=None, num_knn=2, knn_thr=0.01, voxel=0.05,
                  schedule=((OP_REMOVE, 2.5),), extract_high_dyn_knn=True, transform_order=0, keyframe_batch=0,
-                 fast_path=True, cull=True, comm=None):
+                 fast_path=True, cull=True):
         L = host_lib()
         p = Params()
         L.ltrh_params_default(ctypes.byref(p))
@@ -252,20 +142,14 @@ class Removerter:
             msg = L.ltrh_last_error(None).decode()
             self._h = None
             raise binding.LtrError(rc, msg)
-        self._comm = comm
-        if comm is not None:
-            self._ck(L.ltrh_set_comm(self._h, ctypes.byref(comm.struct)))
         # a binding.Context view that shares the orchestrator's ltr_ctx (not owned)
         self.ctx = binding.Context.__new__(binding.Context)
         self.ctx._h = ctypes.c_void_p(L.ltrh_context(self._h))
         self.K = [0, 0]
-        self.rank, self.world, self.split = 0, 1, False
 
     def init_nccl(self, id128, rank, world, split_sessions=True):
         """Native multi-GPU transport (ltrh_comm_init_nccl): every rank passes the same 128-byte id (nccl_unique_id() of one rank)."""
         self._ck(host_lib().ltrh_comm_init_nccl(self._h, id128, rank, world, 1 if split_sessions else 0))
-        self.rank, self.world = rank, world
-        self.split = bool(split_sessions) and world >= 2 and world % 2 == 0
 
     def owns(self, sess):
         return bool(host_lib().ltrh_owns_session(self._h, sess))
@@ -292,23 +176,21 @@ class Removerter:
         if rc != 0:
             raise binding.LtrError(rc, host_lib().ltrh_last_error(self._h).decode())
 
-    def load_session(self, sess, xyzi, offsets, poses, inv_poses):
+    def _load(self, fn, sess, xyzi, offsets, poses, inv_poses):
         x = np.ascontiguousarray(xyzi, np.float32)
         o = np.ascontiguousarray(offsets, np.int64)
         p = np.ascontiguousarray(poses, np.float64)
         ip = np.ascontiguousarray(inv_poses, np.float64)
-        self._ck(host_lib().ltrh_load_session(self._h, sess, x.ctypes.data, o.ctypes.data, p.ctypes.data, ip.ctypes.data, len(o) - 1))
+        self._ck(fn(self._h, sess, x.ctypes.data, o.ctypes.data, p.ctypes.data, ip.ctypes.data, len(o) - 1))
         self.K[sess] = len(o) - 1
+
+    def load_session(self, sess, xyzi, offsets, poses, inv_poses):
+        self._load(host_lib().ltrh_load_session, sess, xyzi, offsets, poses, inv_poses)
 
     def load_session_raw(self, sess, xyzi, offsets, poses, inv_poses):
         """load_session from the scans as read from disk: the load-time VoxelGrid at `voxel` runs on the device first
         (ltrh_load_session_raw, Session::loadKeyframes)."""
-        x = np.ascontiguousarray(xyzi, np.float32)
-        o = np.ascontiguousarray(offsets, np.int64)
-        p = np.ascontiguousarray(poses, np.float64)
-        ip = np.ascontiguousarray(inv_poses, np.float64)
-        self._ck(host_lib().ltrh_load_session_raw(self._h, sess, x.ctypes.data, o.ctypes.data, p.ctypes.data, ip.ctypes.data, len(o) - 1))
-        self.K[sess] = len(o) - 1
+        self._load(host_lib().ltrh_load_session_raw, sess, xyzi, offsets, poses, inv_poses)
 
     def run_step0(self):
         self._ck(host_lib().ltrh_run_step0(self._h))

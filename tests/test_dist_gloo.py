@@ -1,86 +1,42 @@
-"""World-size-2 gloo tests (CPU) of the N > 1 path's host logic: contiguous keyframe blocks, per-pass flag union,
-rank-ordered variable all-gather.  The arithmetic engine here is the oracle (no GPU in this container); what is under
-test is the sharding/collective logic that lt_mapper_b200.removert.TorchDistComm implements for the real library."""
+"""CPU tests (no GPU, no process group) of the multi-GPU keyframe decomposition: each rank owns a contiguous keyframe block, clouds
+merged over all keyframes are the rank-ordered concatenation of the per-block merges, and a pass's dynamic flags are the OR of the
+per-block flags.  The arithmetic engine here is the oracle; what is under test is the decomposition the NCCL transport relies on."""
 import os
-import socket
 import sys
 
 import numpy as np
 import pytest
-import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
-def _worker(rank, world, port, q):
+def test_two_keyframe_blocks_merge_and_flag_union_equal_the_full_pass():
+    """Two ranks of two keyframes each: (1) the rank-ordered concatenation of the per-block merged clouds equals the keyframe-order merge of
+    all keyframes (what ltr_nccl_allgather_clouds assembles); (2) the OR of the per-block flags of an HD pass equals the single-process
+    pass's flags, and neither block alone reaches it (what ltr_nccl_allreduce_flags computes)."""
     sys.path.insert(0, ROOT)
-    # the hooks get host buffers here: with a visible GPU, TorchDistComm would take them for device memory
-    os.environ["CUDA_VISIBLE_DEVICES"] = ""
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    try:
-        import ctypes
-        import oracle
-        import synth
-        from lt_mapper_b200 import removert
-        K = 4
-        full = synth.make_session(0, K, beams=12, az_steps=300)
-        blk = K // world
-        mine = synth.make_session(0, blk, beams=12, az_steps=300, k0=rank * blk)   # this rank's contiguous keyframe block
-        assert np.array_equal(mine.xyzi, full.subset(rank * blk, (rank + 1) * blk).xyzi)
-        comm = removert.TorchDistComm()
-        assert (comm.rank, comm.world) == (rank, world)
-        # (1) rank-ordered variable all-gather of the merged clouds == keyframe-order concatenation
-        local = np.concatenate([oracle.transform(mine.scan(k), mine.poses[k]) for k in range(blk)])
-        counts = (ctypes.c_int64 * world)()
-        assert comm._allgather_i64(None, len(local), counts) == 0
-        cnt = [int(c) for c in counts]
-        displs = (ctypes.c_int64 * world)(*np.concatenate([[0], np.cumsum(cnt)[:-1]]).astype(np.int64))
-        gathered = np.empty((sum(cnt), 4), np.float32)
-        for comp in range(4):
-            src = np.ascontiguousarray(local[:, comp]); dst = np.empty(sum(cnt), np.float32)
-            assert comm._allgatherv(None, src.ctypes.data, len(src), dst.ctypes.data, counts, displs) == 0
-            gathered[:, comp] = dst
-        expect = np.concatenate([oracle.transform(full.scan(k), full.poses[k]) for k in range(K)])
-        assert np.array_equal(gathered, expect)
-        # (2) per-pass flag union: OR of per-rank flags over keyframe blocks == flags of the single-process pass
-        m = oracle.voxel(expect, 0.05)
-        inv = oracle.inverse_poses(full.poses)
-        f_local = oracle.remove_pass(m, mine.xyzi, mine.offsets, inv[rank * blk:(rank + 1) * blk], oracle.MODE_HD, 2.5, threads=1)
-        buf = f_local.copy()
-        assert comm._allreduce(None, buf.ctypes.data, len(buf)) == 0
-        f_full = oracle.remove_pass(m, full.xyzi, full.offsets, inv, oracle.MODE_HD, 2.5, threads=1)
-        assert np.array_equal(buf, f_full)
-        assert f_local.sum() < f_full.sum()   # the union really needed both ranks
-        q.put((rank, "ok"))
-    except Exception as e:  # noqa: BLE001
-        import traceback
-        q.put((rank, "FAIL " + repr(e) + traceback.format_exc()))
-    finally:
-        dist.destroy_process_group()
-
-
-@pytest.mark.timeout(300)
-def test_two_rank_sharding_and_collectives():
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, 2, port, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = [q.get(timeout=240) for _ in procs]
-    for p in procs:
-        p.join(timeout=60)
-    assert sorted(res) == [(0, "ok"), (1, "ok")], res
+    import oracle
+    import synth
+    K, world = 4, 2
+    blk = K // world
+    full = synth.make_session(0, K, beams=12, az_steps=300)
+    blocks = [synth.make_session(0, blk, beams=12, az_steps=300, k0=r * blk) for r in range(world)]   # each rank's contiguous block
+    for r, mine in enumerate(blocks):
+        assert np.array_equal(mine.xyzi, full.subset(r * blk, (r + 1) * blk).xyzi)
+    # (1) rank-ordered concatenation of the merged clouds == keyframe-order merge
+    local = [np.concatenate([oracle.transform(mine.scan(k), mine.poses[k]) for k in range(blk)]) for mine in blocks]
+    expect = np.concatenate([oracle.transform(full.scan(k), full.poses[k]) for k in range(K)])
+    assert np.array_equal(np.concatenate(local), expect)
+    # (2) per-pass flag union: OR of the per-block flags == flags of the single-process pass
+    m = oracle.voxel(expect, 0.05)
+    inv = oracle.inverse_poses(full.poses)
+    f_full = oracle.remove_pass(m, full.xyzi, full.offsets, inv, oracle.MODE_HD, 2.5, threads=1)
+    union = np.zeros_like(f_full)
+    for r, mine in enumerate(blocks):
+        f_local = oracle.remove_pass(m, mine.xyzi, mine.offsets, inv[r * blk:(r + 1) * blk], oracle.MODE_HD, 2.5, threads=1)
+        assert f_local.sum() < f_full.sum()   # the union really needs both blocks
+        union = np.maximum(union, f_local)
+    assert np.array_equal(union, f_full)
 
 
 @pytest.mark.parametrize("world,split", [(1, False), (2, True), (2, False), (4, True), (8, True), (3, False), (8, False)])
