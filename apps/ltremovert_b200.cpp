@@ -6,7 +6,7 @@
 // 1517-1520, 1600-1601, 1607-1650).  No ROS, no PCL; rviz publishing is dropped (side effect only).
 //
 //   ltremovert_b200 --config params.yaml [--selfremovert] [--pcl110] [--no-split] [--clean-scans[=map|scan-minus-map]] [--icp-refinement]
-//                   [--adaptive-threshold[=c]]
+//                   [--adaptive-threshold[=c]] [--map-ball[=R]]
 //     --selfremovert   run selfRemovert over remove_resolution_list (Removerter.cpp:1378-1393) instead of the shipped
 //                      single removeOnce(2.5) (Removerter.cpp:1584, 1587)
 //     --pcl110         PCL >= 1.10 transformPointCloud summation order (ltr_config.transform_order = 1)
@@ -24,6 +24,10 @@
 //                      0.1 m (the range-proportional threshold calcDescrepancyAndParseDynamicPointIdx leaves commented out,
 //                      Removerter.cpp:393-402); c defaults to the reference's 0.05 and must lie in (0, 1).  Prints one summary line; the
 //                      output tree keeps its layout.  There is no yaml key: the reference has none.
+//     --map-ball       every removeOnce / revertOnce projects, per keyframe, only the map points within R m of the keyframe's pose (the
+//                      reference's kUseSubsetMapCloud / kBallSize, Removerter.h:46-48, off there; takeGlobalMapSubsetWithinBall,
+//                      Removerter.cpp:415-427); R defaults to the reference's 80 and must be finite and > 0.  The ND / PD filter passes and
+//                      Step 3 keep the full map.  Prints one summary line; the output tree keeps its layout.
 //
 // Multi-GPU: start one process per GPU with RANK / WORLD_SIZE / LOCAL_RANK in the environment (torchrun, mpirun -x, a shell loop);
 // every rank reads the yaml and the pose files, but loads only the scans of ITS keyframe block (even world: ranks < world/2 take the
@@ -130,8 +134,9 @@ int main(int argc, char** argv) {
     int clean_scans = -1;   // -1 off, else ltr_scanside_criterion
     bool icp_refinement = false;
     float adaptive_c = 0.0f;   // 0: the constant threshold
+    float ball_r = 0.0f;       // 0: the full map
     const char* usage = "usage: %s --config params.yaml [--selfremovert] [--pcl110] [--no-split] [--clean-scans[=map|scan-minus-map]] [--icp-refinement]"
-                        " [--adaptive-threshold[=c], 0 < c < 1]\n";
+                        " [--adaptive-threshold[=c], 0 < c < 1] [--map-ball[=R], R > 0]\n";
     for (int i = 1; i < argc; ++i) {
         if (!std::strcmp(argv[i], "--config") && i + 1 < argc) cfg_path = argv[++i];
         else if (!std::strcmp(argv[i], "--selfremovert")) selfremovert = true;
@@ -141,6 +146,12 @@ int main(int argc, char** argv) {
         else if (!std::strcmp(argv[i], "--clean-scans=scan-minus-map")) clean_scans = LTR_SCANSIDE_SCAN_MINUS_MAP;
         else if (!std::strcmp(argv[i], "--icp-refinement")) icp_refinement = true;
         else if (!std::strcmp(argv[i], "--adaptive-threshold")) adaptive_c = 0.05f;
+        else if (!std::strcmp(argv[i], "--map-ball")) ball_r = 80.0f;
+        else if (!std::strncmp(argv[i], "--map-ball=", 11)) {
+            char* end = nullptr;
+            ball_r = std::strtof(argv[i] + 11, &end);
+            if (end == argv[i] + 11 || *end || !(ball_r > 0.0f && ball_r <= 3.4028235e38f)) { std::fprintf(stderr, usage, argv[0]); return 2; }
+        }
         else if (!std::strncmp(argv[i], "--adaptive-threshold=", 21)) {
             char* end = nullptr;
             adaptive_c = std::strtof(argv[i] + 21, &end);
@@ -238,6 +249,9 @@ int main(int argc, char** argv) {
     if (adaptive_c != 0.0f && rank == 0)
         std::printf(" Adaptive threshold: coefficient %g, a pixel flags when its diff exceeds fl(%g * scan range) in every remove / revert / ND / PD pass\n",
                     (double)adaptive_c, (double)adaptive_c);
+    R.mapBallRadius_ = ball_r;   // checked above
+    if (ball_r != 0.0f && rank == 0)
+        std::printf(" Map ball: radius %g m, each removeOnce / revertOnce keyframe projects only the map points within it\n", (double)ball_r);
     ck(R.run_step0(), "Step 0");
     R.useICPrefinement_ = icp_refinement;
     ck(R.run_step12(), "Step 1-2");

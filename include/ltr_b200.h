@@ -161,6 +161,18 @@ int ltr_remove_pass(ltr_ctx* ctx, ltr_cloud map, ltr_scanset scans, ltr_poses po
  * else LTR_ERR_INVALID. */
 int ltr_remove_pass_adaptive(ltr_ctx* ctx, ltr_cloud map, ltr_scanset scans, ltr_poses poses, int32_t kf_begin, int32_t kf_end,
                              int32_t mode, float res_alpha, float adaptive_coeff, int32_t accumulate, int64_t* n_dynamic);
+/* ltr_remove_pass (adaptive_coeff = 0, constant diff_thres) or ltr_remove_pass_adaptive (adaptive_coeff in (0, 1), diff_thres unused) in
+ * which keyframe k sees only its ball subset of the map: the points i with d2 < r2, d2 = fl(fl(dx*dx + dy*dy) + dz*dz) in f32 without
+ * contraction, dx = fl(x_i - c_k.x), c_k the f32-rounded translation column of poses[k] (not the inverse), r2 = (float)(R*R) in double
+ * (takeGlobalMapSubsetWithinBall, Removerter.cpp:415-427, behind kUseSubsetMapCloud / kBallSize, Removerter.h:46-48; FLANN's L2_Simple
+ * distance and strict radius test).  A point with a non-finite coordinate is in no ball.  The flags are the OR over k of the
+ * single-keyframe pass on the subset, on map indices; the subset keeps map order, so ties between equal ranges in a pixel go to the lowest
+ * map index as in ltr_remove_pass.  Modes HD / ND / PD.  ball_radius must be finite and > 0, and adaptive_coeff 0 or in (0, 1), else
+ * LTR_ERR_INVALID.  ltr_last_pass_stats counts the pairs outside the balls in [1] (settled without exact arithmetic) and, where a whole
+ * 128-point tile is outside a ball, in [6] with the culled pairs; [0] stays K * N. */
+int ltr_remove_pass_ball(ltr_ctx* ctx, ltr_cloud map, ltr_scanset scans, ltr_poses poses, int32_t kf_begin, int32_t kf_end,
+                         int32_t mode, float res_alpha, float diff_thres, float adaptive_coeff, float ball_radius,
+                         int32_t accumulate, int64_t* n_dynamic);
 /* Drops the scan-side images ltr_remove_pass keeps; free_storage != 0 also returns their storage to the context's allocator cache. */
 int ltr_scan_images_release(ltr_ctx* ctx, int32_t free_storage);
 /* Device pointer to the N flag bytes of the last ltr_remove_pass on `map` (for a caller's own all-reduce). */

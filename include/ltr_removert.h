@@ -104,6 +104,13 @@ int ltrh_set_icp_refinement(ltrh_removerter* r, int32_t on);
  * reference's value is 0.05.  c = 0 (the default) turns it off.  Any other value: LTR_ERR_INVALID.  Multi-GPU: nothing new crosses
  * ranks (the flag union of each pass is unchanged). */
 int ltrh_set_adaptive_threshold(ltrh_removerter* r, float c);
+/* The reference's ball subset of the map (kUseSubsetMapCloud / kBallSize, Removerter.h:46-48, off there; takeGlobalMapSubsetWithinBall,
+ * Removerter.cpp:415-427, called from the HD pass at :617-624): with radius R > 0 every later removeOnce / revertOnce (the selfRemovert
+ * schedule of ltrh_run_step12, cascade runs) runs ltr_remove_pass_ball with radius R, so that each keyframe projects only the map points
+ * within R of its pose's translation; the adaptive threshold applies when set.  The ND / PD filter passes, the visible-point extraction and
+ * Step 3 keep the full map, as the reference does.  The reference's value is 80.  R = 0 (the default) turns it off; any value that is not
+ * finite and > 0: LTR_ERR_INVALID.  Multi-GPU: each rank's keyframe block uses its own poses; nothing new crosses ranks. */
+int ltrh_set_map_ball(ltrh_removerter* r, float radius);
 /* Per-keyframe results of the last refinement of session `sess` on this rank: *K_out keyframes (0 when the last detectLowDynamicPoints ran
  * without refinement, and after ltrh_reset_to_step0 or ltrh_cascade_promote_updated, which release Step 2's results), and, when capacity >= *K_out, the final float 4x4 (16 per keyframe), fitness, iterations, exit reason (ltr_icp_exit)
  * and the accepted flag (fitness < 1.0).  Any array may be NULL. */

@@ -42,7 +42,7 @@ EXPORTS = [
     "ltr_cloud_upload", "ltr_cloud_size", "ltr_cloud_download", "ltr_cloud_free", "ltr_cloud_copy", "ltr_cloud_concat", "ltr_cloud_slice",
     "ltr_cloud_device_ptrs", "ltr_cloud_alloc", "ltr_scanset_upload", "ltr_scanset_info", "ltr_scanset_download",
     "ltr_scanset_free", "ltr_scanset_concat_per_keyframe", "ltr_scanset_flatten", "ltr_poses_upload", "ltr_poses_free",
-    "ltr_preclean", "ltr_merge_scans_global", "ltr_voxel_centroid", "ltr_voxel_centroid_per_keyframe", "ltr_voxel_grid", "ltr_voxel_grid_per_keyframe", "ltr_remove_pass", "ltr_remove_pass_adaptive", "ltr_scan_images_release",
+    "ltr_preclean", "ltr_merge_scans_global", "ltr_voxel_centroid", "ltr_voxel_centroid_per_keyframe", "ltr_voxel_grid", "ltr_voxel_grid_per_keyframe", "ltr_remove_pass", "ltr_remove_pass_adaptive", "ltr_remove_pass_ball", "ltr_scan_images_release",
     "ltr_flags_device_ptr", "ltr_flags_download", "ltr_flags_upload", "ltr_apply_partition", "ltr_parse_projected",
     "ltr_knn_diff", "ltr_knn_split_cloud", "ltr_scanside_split", "ltr_scanside_stats", "ltr_icp_params_default", "ltr_icp_refine", "ltr_knn_diff_refined", "ltr_debug_pixel_index", "ltr_debug_scan_rimg", "ltr_debug_fast_project", "ltr_debug_atan_sweep", "ltr_debug_margins", "ltr_reset_rimg_size", "ltr_last_pass_stats", "ltr_profile_get", "ltr_profile_reset", "ltr_timer_start", "ltr_timer_stop", "ltr_trace_dump",
     "ltr_pinned_alloc", "ltr_pinned_free", "ltr_nccl_unique_id", "ltr_nccl_init", "ltr_nccl_split", "ltr_nccl_info", "ltr_nccl_destroy", "ltr_nccl_version", "ltr_nccl_allreduce_flags",
@@ -99,6 +99,7 @@ def lib():
     L.ltr_voxel_grid_per_keyframe.argtypes = [vp, i32, f32, P(i32), P(i32)]
     L.ltr_remove_pass.argtypes = [vp, i32, i32, i32, i32, i32, i32, f32, f32, i32, P(i64)]
     L.ltr_remove_pass_adaptive.argtypes = [vp, i32, i32, i32, i32, i32, i32, f32, f32, i32, P(i64)]
+    L.ltr_remove_pass_ball.argtypes = [vp, i32, i32, i32, i32, i32, i32, f32, f32, f32, f32, i32, P(i64)]
     L.ltr_scan_images_release.argtypes = [vp, i32]
     L.ltr_flags_device_ptr.argtypes = [vp, i32, P(vp), P(i64)]
     L.ltr_flags_download.argtypes = [vp, i32, vp, i64]
@@ -334,6 +335,17 @@ class Context:
         n = ctypes.c_int64()
         self._ck(lib().ltr_remove_pass_adaptive(self._h, map_, scans, poses, kf_begin, kf_end, mode, res_alpha, coeff,
                                                 1 if accumulate else 0, ctypes.byref(n)))
+        return n.value
+
+    def remove_pass_ball(self, map_, scans, poses, mode, res_alpha, radius, diff_thres=0.1, adaptive_coeff=0.0, kf_begin=0, kf_end=None,
+                         accumulate=False):
+        """remove_pass in which each keyframe sees only the map points within `radius` of its pose's translation (ltr_remove_pass_ball);
+        adaptive_coeff != 0 takes the range-adaptive threshold instead of diff_thres."""
+        if kf_end is None:
+            kf_end = self.scanset_info(scans)[0]
+        n = ctypes.c_int64()
+        self._ck(lib().ltr_remove_pass_ball(self._h, map_, scans, poses, kf_begin, kf_end, mode, res_alpha, diff_thres, adaptive_coeff, radius,
+                                            1 if accumulate else 0, ctypes.byref(n)))
         return n.value
 
     def scan_images_release(self, free_storage=True):

@@ -265,7 +265,10 @@ int Removerter::partitionCurrentMapGeneric(ltr_cloud* map, Session& source, ltr_
     int64_t n_map = 0;
     CK(ltr_cloud_size(ctx, *map, &n_map));
     // n_dynamic is taken from the partition below (after the cross-rank flag union), so no count is requested here
-    if (adaptiveThresholdCoeff_ != 0.0f)   // Removerter.cpp:396 in place of :398, for every variant
+    if (mapBallRadius_ != 0.0f && mode == LTR_MODE_HD)   // removeOnce / revertOnce on the ball subsets (Removerter.cpp:617-624, commented out)
+        CK(ltr_remove_pass_ball(ctx, *map, scans, source.keyframe_poses_, 0, source.num_keyframes_, mode, res, 0.1f, adaptiveThresholdCoeff_,
+                                mapBallRadius_, 0, nullptr));
+    else if (adaptiveThresholdCoeff_ != 0.0f)   // Removerter.cpp:396 in place of :398, for every variant
         CK(ltr_remove_pass_adaptive(ctx, *map, scans, source.keyframe_poses_, 0, source.num_keyframes_, mode, res, adaptiveThresholdCoeff_, 0, nullptr));
     else
         CK(ltr_remove_pass(ctx, *map, scans, source.keyframe_poses_, 0, source.num_keyframes_, mode, res, 0.1f, 0, nullptr));
@@ -763,6 +766,12 @@ int ltrh_set_icp_refinement(ltrh_removerter* r, int32_t on) {
 int ltrh_set_adaptive_threshold(ltrh_removerter* r, float c) {
     if (!r || !(c == 0.0f || (c > 0.0f && c < 1.0f))) return LTR_ERR_INVALID;   // NaN fails every comparison
     r->R->adaptiveThresholdCoeff_ = c;
+    return LTR_OK;
+}
+
+int ltrh_set_map_ball(ltrh_removerter* r, float radius) {
+    if (!r || !(radius == 0.0f || (radius > 0.0f && radius <= 3.4028235e38f))) return LTR_ERR_INVALID;   // NaN fails every comparison
+    r->R->mapBallRadius_ = radius;
     return LTR_OK;
 }
 

@@ -125,6 +125,7 @@ public:
     ltrh_params P;
     bool useICPrefinement_ = false;   // Session.cpp:551 (`bool useICPrefinement { false }`), set by ltrh_set_icp_refinement
     float adaptiveThresholdCoeff_ = 0.0f;   // Removerter.cpp:395-396 (`adaptive_coeff`, commented out); 0: the constant 0.1 (:398), set by ltrh_set_adaptive_threshold
+    float mapBallRadius_ = 0.0f;   // Removerter.h:46-48 (`kUseSubsetMapCloud` off, `kBallSize` 80 m); 0: the full map, set by ltrh_set_map_ball
     ltr_ctx* ctx = nullptr;
     int rank = 0, world = 1;
     bool split = false;       // session-split: ranks [0, world/2) own the central keyframes, the others the query keyframes

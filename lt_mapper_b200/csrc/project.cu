@@ -105,10 +105,12 @@ __global__ void __launch_bounds__(256) scan_test_image_kernel(const uint32_t* __
 //       The argument needs t constant within a pixel, not across pixels: it holds for the adaptive t = fl(c s) (kAdaptive,
 //       `thres` = c), which only depends on the pixel's scan range s.
 //   kCandidatesOnly = false (ND, visible-point extraction): true per-pixel minimum with a read-before-atomic filter.
-template <bool kCandidatesOnly, bool kAdaptive = false>
+//   kBall: keyframe k of the launch sees only the points of its ball (ball_member with ball_c[k], ball_r2), every pair tested.
+template <bool kCandidatesOnly, bool kAdaptive = false, bool kBall = false>
 __global__ void __launch_bounds__(256) map_project_kernel(PtrView map, const double* __restrict__ poses, int kf0, int nb,
                                                           const double* __restrict__ ext, int ext_identity, int order, ImgShape g,
-                                                          const uint32_t* __restrict__ scan_rimg, float thres, uint64_t* __restrict__ win) {
+                                                          const uint32_t* __restrict__ scan_rimg, float thres, uint64_t* __restrict__ win,
+                                                          const float4* __restrict__ ball_c, float ball_r2) {
     extern __shared__ double s_pose[];  // nb * 12: inverse poses of the batch
     for (int t = threadIdx.x; t < nb * 12; t += blockDim.x) s_pose[t] = poses[(size_t)(kf0 + t / 12) * 24 + (t % 12)];
     __syncthreads();
@@ -116,8 +118,10 @@ __global__ void __launch_bounds__(256) map_project_kernel(PtrView map, const dou
     if (i >= map.n) return;
     const float x = map.x[i], y = map.y[i], z = map.z[i];
     unsigned n_atomics = 0;   // not reported by this kernel
-    for (int k = 0; k < nb; ++k)
+    for (int k = 0; k < nb; ++k) {
+        if (kBall && !ball_member(x, y, z, ball_c[k], ball_r2)) continue;
         exact_pair<kCandidatesOnly, kAdaptive>(x, y, z, (uint32_t)i, (uint32_t)k, s_pose + 12 * k, ext, ext_identity, order, g, scan_rimg, thres, win, 0, &n_atomics);
+    }
 }
 
 // calcDescrepancyAndParseDynamicPointIdx (Removerter.cpp:381-413) over the batch images; also re-arms `win`.  kAdaptive: the threshold
@@ -379,11 +383,24 @@ using FastKernel = decltype(&map_project_fast_kernel<true, true, false, true>);
 // One launch of the map projection over the keyframes [k0, k0 + nb) of `poses` into `win`, timed by an event pair.  rimg: the launch's scan
 // range images (scan-minus-map; unused by the true minimum), test_img: the test image of the scan-minus-map fast path.  amin (fast path,
 // may be null in the deferred mode): the approximate running minimum, reset here.  da: the deferred mode's scratch.  adaptive (scan-minus-map
-// only): `thres` is the coefficient c of the pixel threshold fl(c s), and test_img was built for it.
+// only): `thres` is the coefficient c of the pixel threshold fl(c s), and test_img was built for it.  ball (nullptr or args.centre nullptr:
+// the full map): keyframe k sees only the points of its ball (args.centre[k], args.r2); on the fast path through the tile list of the
+// launch, which ball_tile_list_kernel builds here from the tile spheres and non-finite flags into `scratch` (3 ntiles words: out masks,
+// in masks, list).
+struct BallLaunch {
+    BallArgs args;                     // centre and r2 set by the caller; the rest is filled here
+    const float4* tiles = nullptr;
+    const uint8_t* nonfinite = nullptr;
+    long long ntiles = 0;
+    uint32_t* scratch = nullptr;
+};
+
 static int project_map(ltr_ctx* ctx, PassPlan& p, const DevCloud& map, const DevPoses& poses, int k0, int nb, Proj mode, const uint32_t* rimg,
-                       const uint32_t* test_img, float thres, bool adaptive, uint64_t* win, uint32_t* amin, const CullArgs& ca, const DeferredArgs& da) {
+                       const uint32_t* test_img, float thres, bool adaptive, uint64_t* win, uint32_t* amin, const CullArgs& ca, const DeferredArgs& da,
+                       const BallLaunch* ball = nullptr) {
     const bool cand = mode == Proj::kScanMinusMap;
     adaptive = adaptive && cand;
+    const bool use_ball = ball && ball->args.centre;
     if (amin) {
         fill_u32_kernel<<<grid_for(nb * p.npx, 256, ctx->sm_count * 8), 256, 0, ctx->stream>>>(amin, 0x7f800000u, nb * p.npx);
         LTR_LAUNCH_CHECK(ctx);
@@ -391,9 +408,11 @@ static int project_map(ltr_ctx* ctx, PassPlan& p, const DevCloud& map, const Dev
     prof_begin(ctx);
     p.units.push_back(nb);
     if (!p.use_fast) {
-        const auto kern = adaptive ? map_project_kernel<true, true> : cand ? map_project_kernel<true> : map_project_kernel<false>;
+        const auto kern = use_ball ? (adaptive ? map_project_kernel<true, true, true> : cand ? map_project_kernel<true, false, true> : map_project_kernel<false, false, true>)
+                        : adaptive ? map_project_kernel<true, true> : cand ? map_project_kernel<true> : map_project_kernel<false>;
         kern<<<(unsigned)((map.n + 255) / 256), 256, (size_t)nb * 12 * sizeof(double), ctx->stream>>>(view(map), poses.d, k0, nb, ctx->d_ext,
-            ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, p.g, rimg, thres, win);
+            ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, p.g, rimg, thres, win, use_ball ? ball->args.centre : nullptr,
+            use_ball ? ball->args.r2 : 0.0f);
     } else {
         unsigned int* work = (unsigned int*)(ctx->d_counters + 4);
         LTR_CUDA(ctx, cudaMemsetAsync(work, 0, sizeof(unsigned int), ctx->stream));
@@ -402,8 +421,27 @@ static int project_map(ltr_ctx* ctx, PassPlan& p, const DevCloud& map, const Dev
             LTR_CUDA(ctx, cudaMemsetAsync(da.best, 0xff, (size_t)nb * p.npx * sizeof(unsigned long long), ctx->stream));   // "no pair yet"
             LTR_CUDA(ctx, cudaMemsetAsync(da.count, 0, sizeof(unsigned int), ctx->stream));
         }
-        // template arguments <candidates only, short elevation path, deferred, guard-padded test image, adaptive threshold>
-        const FastKernel kern = (cand && p.fc.pad_ok) ? (adaptive ? map_project_fast_kernel<true, true, false, true, true> : map_project_fast_kernel<true, true, false, true>)
+        BallArgs ba{};
+        if (use_ball) {   // the launch's tile list; its count lives in counters[5], never read by the host
+            ba = ball->args;
+            uint32_t* s = ball->scratch;
+            unsigned int* count = (unsigned int*)(ctx->d_counters + 5);
+            ba.out_mask = s; ba.in_mask = s + ball->ntiles; ba.list = s + 2 * ball->ntiles; ba.count = count;
+            LTR_CUDA(ctx, cudaMemsetAsync(count, 0, sizeof(unsigned int), ctx->stream));
+            ball_tile_list_kernel<<<(unsigned)((ball->ntiles * 32 + 255) / 256), 256, 0, ctx->stream>>>(ball->tiles, ball->nonfinite, ball->ntiles, ba, nb,
+                s, s + ball->ntiles, s + 2 * ball->ntiles, count, ctx->d_counters);
+            LTR_LAUNCH_CHECK(ctx);
+        }
+        // template arguments <candidates only, short elevation path, deferred, guard-padded test image, adaptive threshold, ball subset>
+        const FastKernel kern = use_ball
+            ? ((cand && p.fc.pad_ok) ? (adaptive ? map_project_fast_kernel<true, true, false, true, true, true> : map_project_fast_kernel<true, true, false, true, false, true>)
+               : with_el_direct(p.fc, [mode, adaptive](auto el) -> FastKernel {
+                     constexpr bool kEl = decltype(el)::value;
+                     return mode == Proj::kScanMinusMap ? (adaptive ? map_project_fast_kernel<true, kEl, false, false, true, true> : map_project_fast_kernel<true, kEl, false, false, false, true>)
+                          : mode == Proj::kTrueMin      ? map_project_fast_kernel<false, kEl, false, false, false, true>
+                                                        : map_project_fast_kernel<false, kEl, true, false, false, true>;
+                 }))
+            : (cand && p.fc.pad_ok) ? (adaptive ? map_project_fast_kernel<true, true, false, true, true> : map_project_fast_kernel<true, true, false, true>)
             : with_el_direct(p.fc, [mode, adaptive](auto el) -> FastKernel {
                   constexpr bool kEl = decltype(el)::value;
                   return mode == Proj::kScanMinusMap ? (adaptive ? map_project_fast_kernel<true, kEl, false, false, true> : map_project_fast_kernel<true, kEl, false>)
@@ -411,7 +449,7 @@ static int project_map(ltr_ctx* ctx, PassPlan& p, const DevCloud& map, const Dev
                                                      : map_project_fast_kernel<false, kEl, true>;
               });
         kern<<<fast_grid(ctx, map.n), kFastThreads, fast_smem_bytes(), ctx->stream>>>(view(map), make_kf_batch(poses, k0, nb), poses.d, k0, nb, ctx->d_ext,
-            ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, p.g, p.fc, rimg, cand ? test_img : amin, thres, win, amin, ca, ctx->d_counters, work, da);
+            ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, p.g, p.fc, rimg, cand ? test_img : amin, thres, win, amin, ca, ctx->d_counters, work, da, ba);
         if (deferred) {
             LTR_LAUNCH_CHECK(ctx);
             deferred_resolve_kernel<<<grid_for(nb * p.npx, 256, ctx->sm_count * 16), 256, 0, ctx->stream>>>(view(map), poses.d, k0, nb, ctx->d_ext,
@@ -645,9 +683,11 @@ int ltr_scan_images_release(ltr_ctx* ctx, int32_t free_storage) {
 }
 
 // adaptive_c != 0: the pixel threshold is fl(adaptive_c s) (ltr_remove_pass_adaptive) and diff_thres is not used.
+// ball_r2 != 0: keyframe k sees only the map points within the ball of squared radius ball_r2 around its pose's f32 translation
+// (ltr_remove_pass_ball; a negative value: no point is in any ball).
 static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end,
-                            int32_t mode, float res_alpha, float diff_thres, float adaptive_c, int32_t accumulate, int64_t* n_dynamic, bool allow_deferred,
-                            bool* overflowed) {
+                            int32_t mode, float res_alpha, float diff_thres, float adaptive_c, float ball_r2, int32_t accumulate, int64_t* n_dynamic,
+                            bool allow_deferred, bool* overflowed) {
     *overflowed = false;
     const bool adaptive = adaptive_c != 0.0f;
     const float thres = adaptive ? adaptive_c : diff_thres;   // the kernels' `thres`: the constant, or the coefficient
@@ -704,6 +744,45 @@ static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, 
         tile_sphere_kernel<<<(unsigned)((ca.ntiles * 32 + 255) / 256), 256, 0, ctx->stream>>>(view(*map), (float4*)p_tiles, ca.ntiles);
         LTR_LAUNCH_CHECK(ctx);
     }
+    // ball subset: the centres of the pass's keyframes and, on the fast path, the tile spheres (shared with culling), a non-finite flag per
+    // tile and the per-launch tile classification (BallLaunch)
+    BallLaunch bl;
+    void *p_ball = nullptr;
+    ScratchGuard g_ball(ctx, &p_ball);
+    std::vector<float4> centre;   // outlives the copy below: the pass synchronises before it returns
+    if (ball_r2 != 0.0f && run) {
+        const int K = kf_end - kf_begin;
+        const long long ntiles = (map->n + kTilePts - 1) / kTilePts;
+        centre.resize((size_t)K);
+        for (int k = 0; k < K; ++k) {   // the pose's translation column (pose rows at 12..23 of DevPoses::h), rounded to f32
+            const double* T = &poses->h[(size_t)(kf_begin + k) * 24 + 12];
+            centre[(size_t)k] = make_float4((float)T[3], (float)T[7], (float)T[11], 0.0f);
+        }
+        const size_t c_bytes = ((size_t)K * sizeof(float4) + 255) / 256 * 256;
+        const size_t w_bytes = p.use_fast ? ((size_t)ntiles * 3 * sizeof(uint32_t) + 255) / 256 * 256 : 0;
+        const size_t t_bytes = (p.use_fast && !use_cull) ? (size_t)ntiles * sizeof(float4) : 0;
+        const size_t f_bytes = p.use_fast ? (size_t)ntiles : 0;
+        LTR_TRY(dev_alloc(ctx, &p_ball, c_bytes + w_bytes + t_bytes + f_bytes));
+        char* b = (char*)p_ball;
+        LTR_CUDA(ctx, cudaMemcpyAsync(b, centre.data(), (size_t)K * sizeof(float4), cudaMemcpyHostToDevice, ctx->stream));
+        bl.args.centre = (const float4*)b;
+        bl.args.r2 = ball_r2;
+        if (p.use_fast) {
+            bl.ntiles = ntiles;
+            bl.scratch = (uint32_t*)(b + c_bytes);
+            float4* tiles = use_cull ? (float4*)p_tiles : (float4*)(b + c_bytes + w_bytes);
+            if (!use_cull) {
+                tile_sphere_kernel<<<(unsigned)((ntiles * 32 + 255) / 256), 256, 0, ctx->stream>>>(view(*map), tiles, ntiles);
+                LTR_LAUNCH_CHECK(ctx);
+            }
+            uint8_t* nonfinite = (uint8_t*)(b + c_bytes + w_bytes + t_bytes);
+            LTR_CUDA(ctx, cudaMemsetAsync(nonfinite, 0, (size_t)ntiles, ctx->stream));
+            tile_nonfinite_kernel<<<(unsigned)((map->n + 255) / 256), 256, 0, ctx->stream>>>(view(*map), nonfinite);
+            LTR_LAUNCH_CHECK(ctx);
+            bl.tiles = tiles;
+            bl.nonfinite = nonfinite;
+        }
+    }
     LTR_TRY(pass_begin(ctx, p));
     if (run) {
         void *p_rimg = nullptr, *p_win = nullptr;
@@ -733,7 +812,9 @@ static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, 
                 test_img = need_timg ? l_timg : l_rimg;
                 if (use_cull) ca.pyr = (const float*)p_pyr;
             }
-            LTR_TRY(project_map(ctx, p, *map, *poses, k0, nb, proj, rimg, test_img, thres, adaptive, win, amin, ca, da));
+            BallLaunch* blk = nullptr;
+            if (bl.args.centre) { blk = &bl; bl.args.centre = (const float4*)p_ball + (k0 - kf_begin); }
+            LTR_TRY(project_map(ctx, p, *map, *poses, k0, nb, proj, rimg, test_img, thres, adaptive, win, amin, ca, da, blk));
             const unsigned rb = (unsigned)((nb * npx + 255) / 256);
             const auto resolve = cand ? (adaptive ? resolve_kernel<true, true> : resolve_kernel<true>) : (adaptive ? resolve_kernel<false, true> : resolve_kernel<false>);
             resolve<<<rb, 256, 0, ctx->stream>>>(rimg, win, nb * npx, thres, map->flags);
@@ -742,6 +823,7 @@ static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, 
     }
     g_tiles.release();
     g_pyr.release();
+    g_ball.release();
     LTR_CUDA(ctx, cudaEventRecord(ctx->ev1, ctx->stream));
     if (n_dynamic) LTR_TRY(count_flags(ctx, map->flags, map->n, n_dynamic));
     unsigned int h_over = 0;
@@ -760,7 +842,7 @@ int ltr_remove_pass(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, ltr_pose
     // ND (true per-pixel minimum) runs in the deferred mode of project_fast.cuh unless the flags accumulate into earlier ones (a run whose
     // overflow list filled up would have to be undone)
     return with_deferred_retry([&](bool allow_deferred, bool* overflowed) {
-        return remove_pass_impl(ctx, map_h, scans_h, poses_h, kf_begin, kf_end, mode, res_alpha, diff_thres, 0.0f, accumulate, n_dynamic,
+        return remove_pass_impl(ctx, map_h, scans_h, poses_h, kf_begin, kf_end, mode, res_alpha, diff_thres, 0.0f, 0.0f, accumulate, n_dynamic,
                                 allow_deferred && !accumulate, overflowed);
     });
 }
@@ -772,7 +854,24 @@ int ltr_remove_pass_adaptive(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h,
     // NaN fails both comparisons
     if (!(adaptive_coeff > 0.0f && adaptive_coeff < 1.0f)) return fail(ctx, LTR_ERR_INVALID, "adaptive coefficient %g outside (0, 1)", (double)adaptive_coeff);
     return with_deferred_retry([&](bool allow_deferred, bool* overflowed) {
-        return remove_pass_impl(ctx, map_h, scans_h, poses_h, kf_begin, kf_end, mode, res_alpha, 0.0f, adaptive_coeff, accumulate, n_dynamic,
+        return remove_pass_impl(ctx, map_h, scans_h, poses_h, kf_begin, kf_end, mode, res_alpha, 0.0f, adaptive_coeff, 0.0f, accumulate, n_dynamic,
+                                allow_deferred && !accumulate, overflowed);
+    });
+}
+
+int ltr_remove_pass_ball(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end,
+                         int32_t mode, float res_alpha, float diff_thres, float adaptive_coeff, float ball_radius, int32_t accumulate, int64_t* n_dynamic) {
+    ApiTrace tr__(ctx, "ltr_remove_pass_ball");
+    if (!ctx) return LTR_ERR_INVALID;
+    // NaN fails every comparison
+    if (!(ball_radius > 0.0f && ball_radius <= 3.4028235e38f)) return fail(ctx, LTR_ERR_INVALID, "ball radius %g is not finite and > 0", (double)ball_radius);
+    if (adaptive_coeff != 0.0f && !(adaptive_coeff > 0.0f && adaptive_coeff < 1.0f))
+        return fail(ctx, LTR_ERR_INVALID, "adaptive coefficient %g outside (0, 1)", (double)adaptive_coeff);
+    // PCL's radiusSearch hands FLANN radius^2 as a float; an r2 that rounds to 0 admits no point (-1 stands for it: 0 means "no ball")
+    float r2 = (float)((double)ball_radius * (double)ball_radius);
+    if (r2 == 0.0f) r2 = -1.0f;
+    return with_deferred_retry([&](bool allow_deferred, bool* overflowed) {
+        return remove_pass_impl(ctx, map_h, scans_h, poses_h, kf_begin, kf_end, mode, res_alpha, diff_thres, adaptive_coeff, r2, accumulate, n_dynamic,
                                 allow_deferred && !accumulate, overflowed);
     });
 }

@@ -322,18 +322,80 @@ struct DeferredArgs {
     const unsigned long long* order;   // tile claim order (low 32 bits: tile index), or nullptr: map order
 };
 
-template <bool kCandidatesOnly, bool kElDirect, bool kDeferred = false, bool kPad = false, bool kAdaptive = false>
+// Ball subset of the map (ltr_remove_pass_ball, DESIGN.md 4.3): keyframe k of a launch sees only the map points with
+// fl(fl(dx dx + dy dy) + dz dz) < r2, d = fl(p - c_k), c_k the f32 translation of its pose.  Per launch, ball_tile_list_kernel classifies
+// every 128-point tile against every keyframe of the launch (`out`: no point of the tile is a member, `in`: every point is) and lists
+// the tiles that are not `out` in all of them; map_project_fast_kernel<..., kBall> claims only the listed tiles.
+struct BallArgs {
+    const float4* centre;      // [keyframes in launch]: c_k (w unused); nullptr: no ball
+    const uint32_t* out_mask;  // [tile]: bit k = no point of the tile is in ball k
+    const uint32_t* in_mask;   // [tile]: bit k = every point of the tile is in ball k
+    const uint32_t* list;      // tiles to project, in any order
+    const unsigned int* count; // number of listed tiles (device-side, written by ball_tile_list_kernel)
+    float r2;
+};
+
+// the exact membership test of the contract: FLANN's L2_Simple distance in f32 without contraction, strictly below r2 (NaN: not a member)
+LTR_DEV bool ball_member(float x, float y, float z, float4 c, float r2) {
+    const float dx = __fsub_rn(x, c.x), dy = __fsub_rn(y, c.y), dz = __fsub_rn(z, c.z);
+    return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)) < r2;
+}
+
+// One warp per tile, lane k against ball k of the launch (DESIGN.md 4.3 derives the slack).  With the tile sphere (c, rho) and
+// D = |c - c_k| evaluated in double, every point p of the tile has D - rho <= |p - c_k| <= D + rho, and the f32 d2 of the contract is
+// within 5u (u = 2^-24) relative of |p - c_k|^2 (no underflow matters once r2 >= 2^-100).  The double evaluation is within 1e-15 relative.
+//   out: D - rho > 0 and (D - rho)^2 >= r2 (1 + 2^-20)  =>  d2 >= r2 (1 + 2^-20)(1 - 5u - 1e-15) > r2
+//   in : (D + rho)^2 <= r2 (1 - 2^-20), every point of the tile finite  =>  d2 <= r2 (1 - 2^-20)(1 + 5u + 1e-15) < r2
+// Outside r2 in [2^-100, FLT_MAX] nothing is classified, and every point takes the exact test.  Listed: every tile whose `out` mask is not
+// all nb keyframes; the pairs of its `out` bits are counted as culled pairs (counters[3]), those of an unlisted tile too.
+__global__ void __launch_bounds__(256) ball_tile_list_kernel(const float4* __restrict__ tiles, const uint8_t* __restrict__ tile_nonfinite,
+                                                             long long ntiles, BallArgs ba, int nb, uint32_t* __restrict__ out_mask,
+                                                             uint32_t* __restrict__ in_mask, uint32_t* __restrict__ list,
+                                                             unsigned int* __restrict__ count, unsigned long long* __restrict__ counters) {
+    const long long tile = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (tile >= ntiles) return;
+    const unsigned lane = threadIdx.x & 31;
+    bool out = false, in = false;
+    const double r2 = (double)ba.r2;
+    if ((int)lane < nb && r2 >= 0x1p-100 && r2 <= 3.4028234663852886e38) {
+        const float4 t = tiles[tile], c = ba.centre[lane];
+        const double dx = (double)t.x - (double)c.x, dy = (double)t.y - (double)c.y, dz = (double)t.z - (double)c.z;
+        const double D = sqrt(dx * dx + dy * dy + dz * dz), rho = (double)t.w;
+        const double lo = D - rho, hi = D + rho;
+        out = lo > 0.0 && lo * lo >= r2 * (1.0 + 0x1p-20);   // NaN: false
+        in = !tile_nonfinite[tile] && hi * hi <= r2 * (1.0 - 0x1p-20);
+    }
+    const unsigned om = __ballot_sync(0xffffffffu, out), im = __ballot_sync(0xffffffffu, in);
+    if (lane == 0) {
+        out_mask[tile] = om;
+        in_mask[tile] = im;
+        const unsigned all = nb >= 32 ? 0xffffffffu : (1u << nb) - 1u;
+        if (om != all) list[atomicAdd(count, 1u)] = (uint32_t)tile;
+        if (om && counters) atomicAdd(&counters[3], (unsigned long long)__popc(om) * (unsigned long long)kTilePts);
+    }
+}
+
+// 1 per tile that holds a non-finite coordinate (such a point is never a ball member, and the tile sphere does not bound it); zeroed before
+__global__ void __launch_bounds__(256) tile_nonfinite_kernel(PtrView map, uint8_t* __restrict__ tile_nonfinite) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= map.n) return;
+    if (!(isfinite(map.x[i]) && isfinite(map.y[i]) && isfinite(map.z[i]))) tile_nonfinite[i / kTilePts] = 1;
+}
+
+template <bool kCandidatesOnly, bool kElDirect, bool kDeferred = false, bool kPad = false, bool kAdaptive = false, bool kBall = false>
 __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFastCtasPerSm) map_project_fast_kernel(PtrView map, const __grid_constant__ KfBatch kb, const double* __restrict__ poses,
                                                                         int kf0, int nb, const double* __restrict__ ext, int ext_identity, int order,
                                                                         ImgShape g, const __grid_constant__ FastCfg fc, const uint32_t* __restrict__ scan_rimg,
                                                                         const uint32_t* __restrict__ test_img, float thres,
                                                                         uint64_t* __restrict__ win, uint32_t* __restrict__ approx_min,
                                                                         CullArgs ca, unsigned long long* __restrict__ counters,
-                                                                        unsigned int* __restrict__ work_counter, DeferredArgs da) {
+                                                                        unsigned int* __restrict__ work_counter, DeferredArgs da, BallArgs ba) {
     // kPad (scan-minus-map, short elevation path, 360 degree field of view): the test image is guard-padded (FastCfg::pad_*), so the
     // gather needs no index clamp
     static_assert(!kPad || (kCandidatesOnly && kElDirect && !kDeferred), "the padded test image exists for the scan-minus-map short path only");
     static_assert(!kAdaptive || (kCandidatesOnly && !kDeferred), "the true minimum does not depend on the threshold");
+    // kBall: the warps claim the tiles of ba.list (ball_tile_list_kernel); a point outside ball k is absent from keyframe k -- no
+    // certainty decision, queue entry, atomic or deferred-list entry.  The claim order cannot change a result (DESIGN.md 4.3).
     extern __shared__ uint64_t s_queues[];
     const int warp = threadIdx.x >> 5;
     uint64_t* s_qa = s_queues + warp * (2 * kQueueCap);
@@ -360,8 +422,8 @@ __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFast
     unsigned tile_u = 0;
     if (lane == 0) tile_u = atomicAdd(work_counter, 1u);
     tile_u = __shfl_sync(0xffffffffu, tile_u, 0);
-    if ((long long)tile_u >= total_tiles) break;
-    const long long tile = (kDeferred && da.order) ? (long long)(uint32_t)da.order[tile_u] : (long long)tile_u;
+    if (kBall ? tile_u >= *ba.count : (long long)tile_u >= total_tiles) break;
+    const long long tile = kBall ? (long long)ba.list[tile_u] : (kDeferred && da.order) ? (long long)(uint32_t)da.order[tile_u] : (long long)tile_u;
     const int64_t base = (int64_t)tile * (32 * kFastPts) + lane;
     // map index of the lane's point j, and the push of its pair with keyframe k onto the full exact queue.  Recomputed at each use: caching
     // the indices across the keyframe loop would cost the padded variant its 64-register bound.
@@ -376,19 +438,31 @@ __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFast
     }
     // Tile culling (project_cull.cuh): lane l tests this 128-point tile against keyframe l of the launch; the ballot is the
     // set of keyframes in which no point of the tile can be a candidate -- those iterations of the k loop are skipped.
-    unsigned cull_mask = 0u;
+    // kBall: the keyframes whose ball holds no point of the tile are skipped like culled ones (their pairs were counted by the list kernel)
+    unsigned cull_mask = kBall ? ba.out_mask[tile] : 0u;
+    const unsigned ball_in = kBall ? ba.in_mask[tile] : 0u;
     if (kCandidatesOnly && ca.enabled) {
         const float4 t = ca.tiles[tile];
-        const bool c = ((int)lane < nb) && tile_culled<kAdaptive>(kb.kf[lane], t, fc, g, ca, (int)lane, thres);
-        cull_mask = __ballot_sync(0xffffffffu, c);
-        if (lane == 0) s_stat[warp][2] += __popc(cull_mask);
+        const bool c = ((int)lane < nb) && (!kBall || !((cull_mask >> lane) & 1u)) && tile_culled<kAdaptive>(kb.kf[lane], t, fc, g, ca, (int)lane, thres);
+        const unsigned m = __ballot_sync(0xffffffffu, c);
+        cull_mask |= m;
+        if (lane == 0) s_stat[warp][2] += __popc(m);
     }
     for (int k = 0; k < nb; ++k) {                    // a plain counted loop: k stays provably warp-uniform, so kb.kf[k] is read with LDCU
         if ((cull_mask >> k) & 1u) continue;         // warp-uniform (ballot)
         const float* __restrict__ kf = kb.kf[k];
+        // kBall: the membership of the thread's points in ball k (all members when the tile's `in` bit is set; warp-uniform branch)
+        bool in_[kFastPts];
+#pragma unroll
+        for (int j = 0; j < kFastPts; ++j) in_[j] = true;
+        if (kBall && !((ball_in >> k) & 1u)) {
+            const float4 bc = ba.centre[k];
+#pragma unroll
+            for (int j = 0; j < kFastPts; ++j) in_[j] = ball_member(px_[j], py_[j], pz_[j], bc, ba.r2);
+        }
         if (kf[15] == 0.0f) {                         // warp-uniform: no fast constants (non-rigid pose or extrinsic) -> all pairs exact
 #pragma unroll
-            for (int j = 0; j < kFastPts; ++j) push_full(j, k);
+            for (int j = 0; j < kFastPts; ++j) if (in_[j]) push_full(j, k);
         } else {
         // this keyframe's images (kPad: the padded test image)
         const uint32_t* __restrict__ test_k = kDeferred ? nullptr : kPad ? opaque_ptr(test_img + (uint32_t)(k * fc.pad_npx)) : test_img + (size_t)k * npx;
@@ -448,7 +522,7 @@ __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFast
                 const float fr = fr_[j], tv = tv_[j];
                 // tv = approximate range of the pixel's best pair as read in phase 1 (all-ones bits = NaN while the pixel is empty;
                 // every comparison is written so that NaN means "consider the pair")
-                enter_[j] = certain_[j] && !(fr > __fadd_rn(tv, __fmaf_rn(fc.mr2_rel, fr, fc.mr2_abs)));
+                enter_[j] = in_[j] && certain_[j] && !(fr > __fadd_rn(tv, __fmaf_rn(fc.mr2_rel, fr, fc.mr2_abs)));
                 lead_[j] = enter_[j] && !(fr >= tv);             // looks like a new best
                 old_[j] = 0ull; rwin_[j] = tv;
                 if (lead_[j]) {
@@ -473,7 +547,7 @@ __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFast
                         const unsigned slot = atomicAdd(da.count, 1u);
                         if (slot < da.capacity) da.list[slot] = q_pack((uint32_t)loser, pxl_[j], (uint32_t)k);
                     }
-                } else if (!certain_[j]) {
+                } else if (in_[j] && !certain_[j]) {
                     push_full(j, k);
                 }
             }
@@ -484,6 +558,7 @@ __global__ void __launch_bounds__(kFastThreads, kPad ? kFastCtasPerSmPad : kFast
 #pragma unroll
         for (int j = 0; j < kFastPts; ++j) {
             const float fr = fr_[j], tv = tv_[j];
+            if (!in_[j]) continue;                   // kBall: not in this keyframe's ball
             if (certain_[j]) {
                 bool maybe;
                 if (kCandidatesOnly) maybe = !(__fmaf_rn(fr, fc.rel_m1, tv) < thr_lo);   // scan - r + m_rel r >= thres - m_abs for some range within the margin

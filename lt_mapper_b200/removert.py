@@ -30,7 +30,7 @@ class Params(ctypes.Structure):
 
 
 HOST_EXPORTS = ["ltrh_params_default", "ltrh_create", "ltrh_destroy", "ltrh_last_error", "ltrh_context", "ltrh_comm_init_nccl", "ltrh_owns_session", "ltrh_invert_poses",
-                "ltrh_load_session", "ltrh_load_session_raw", "ltrh_run_step0", "ltrh_run_step12", "ltrh_run_step3", "ltrh_reset_to_step0", "ltrh_cascade_promote_updated", "ltrh_scanside_removal", "ltrh_set_icp_refinement", "ltrh_set_adaptive_threshold", "ltrh_icp_stats", "ltrh_stage", "ltrh_cloud",
+                "ltrh_load_session", "ltrh_load_session_raw", "ltrh_run_step0", "ltrh_run_step12", "ltrh_run_step3", "ltrh_reset_to_step0", "ltrh_cascade_promote_updated", "ltrh_scanside_removal", "ltrh_set_icp_refinement", "ltrh_set_adaptive_threshold", "ltrh_set_map_ball", "ltrh_icp_stats", "ltrh_stage", "ltrh_cloud",
                 "ltrh_scanset", "ltrh_timing", "ltrh_log_count", "ltrh_log_get", "ltrh_io_last_error", "ltrh_io_read_pcd", "ltrh_io_write_pcd",
                 "ltrh_io_read_poses", "ltrh_io_parse_keyframes", "ltrh_io_parse_keyframes_in_roi", "ltrh_io_voxel_grid", "ltrh_io_voxel_grid_scans", "ltrh_io_yaml_get"]
 
@@ -65,6 +65,7 @@ def host_lib():
     L.ltrh_scanside_removal.argtypes = [vp, i32, i32, i32]
     L.ltrh_set_icp_refinement.argtypes = [vp, i32]
     L.ltrh_set_adaptive_threshold.argtypes = [vp, ctypes.c_float]
+    L.ltrh_set_map_ball.argtypes = [vp, ctypes.c_float]
     L.ltrh_icp_stats.argtypes = [vp, i32, i32, P(i32), vp, vp, vp, vp, vp]
     L.ltrh_stage.argtypes = [vp, ctypes.c_char_p]
     L.ltrh_cloud.argtypes = [vp, ctypes.c_char_p, i32, P(i32)]
@@ -220,6 +221,11 @@ class Removerter:
         """The range-adaptive threshold fl(c * scan range) for later remove / revert / ND / PD passes (ltrh_set_adaptive_threshold;
         0 < c < 1, c = 0 turns it off, which is the default)."""
         self._ck(host_lib().ltrh_set_adaptive_threshold(self._h, c))
+
+    def set_map_ball(self, radius=80.0):
+        """The reference's ball subset of the map for later removeOnce / revertOnce passes (ltrh_set_map_ball): each keyframe projects
+        only the map points within `radius` m of its pose; radius = 0 turns it off, which is the default."""
+        self._ck(host_lib().ltrh_set_map_ball(self._h, radius))
 
     def icp_stats(self, sess):
         """This rank's refinement of session `sess` in the last Step 2 (ltrh_icp_stats): dict of per-keyframe arrays T (K, 4, 4) float32,
