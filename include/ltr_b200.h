@@ -297,6 +297,16 @@ int ltr_debug_pixel_index(ltr_ctx* ctx, const float* xyz /* n*3 */, int64_t n, i
 /* scan2RangeImg (Removerter.cpp:109-156) of keyframe `kf` exactly as ltr_remove_pass builds it (fast pixel evaluation when the context's
  * fast_path is on): rows*cols floats, 10000.0f = no point.  Lets tests compare the image itself, not only what is derived from it. */
 int ltr_debug_scan_rimg(ltr_ctx* ctx, ltr_scanset scans, int32_t kf, float res_alpha, float* rimg /* rows*cols */);
+/* The exact k-NN average of ltr_scanside_split's "scan minus map" criterion, (float)(double sum of the k smallest squared distances,
+ * ascending) / (float)k, for every point of `query` (taken as global coordinates), in one launch of the same search: self == 0 -> against
+ * `target` (avg_map); self != 0 -> keyframe j of `query` against its own points, `target` ignored (avg_scan).  unsettled (may be NULL):
+ * the queries the bounded pass on the finest level left over (what ltr_scanside_stats [1] / [2] count).  k outside [1, 16], an empty
+ * target, a non-finite coordinate, or more than 8192 keyframes with self set fail with LTR_ERR_UNSUPPORTED. */
+int ltr_debug_exact_knn_avg(ltr_ctx* ctx, ltr_scanset query, ltr_cloud target, int32_t self, int32_t k, float* avg /* n */, int64_t* unsettled);
+/* The correspondence search of ltr_icp_refine for every point of `query`: d = the smallest f32 L2_Simple squared distance to `target`,
+ * idx = the lowest target index at that distance.  Where d is +inf, idx is not specified (ltr_icp_refine drops such pairs).  An empty
+ * target or a non-finite coordinate fails with LTR_ERR_UNSUPPORTED. */
+int ltr_debug_nearest(ltr_ctx* ctx, ltr_cloud query, ltr_cloud target, float* d /* n */, int32_t* idx /* n */);
 /* Fast-path validation: for n map points and one inverse pose, writes per point 8 floats:
  * fast pre-round column, fast pre-round row, fast range, r/rho | reference pre-round column, row, range, fast azimuth [rad];
  * margins4 (optional) = column margin a, column margin b (x r/rho), row margin, relative range margin. */

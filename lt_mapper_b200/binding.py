@@ -44,7 +44,7 @@ EXPORTS = [
     "ltr_scanset_free", "ltr_scanset_concat_per_keyframe", "ltr_scanset_flatten", "ltr_poses_upload", "ltr_poses_free",
     "ltr_preclean", "ltr_merge_scans_global", "ltr_voxel_centroid", "ltr_voxel_centroid_per_keyframe", "ltr_voxel_grid", "ltr_voxel_grid_per_keyframe", "ltr_remove_pass", "ltr_remove_pass_adaptive", "ltr_remove_pass_ball", "ltr_scan_images_release",
     "ltr_flags_device_ptr", "ltr_flags_download", "ltr_flags_upload", "ltr_apply_partition", "ltr_parse_projected",
-    "ltr_knn_diff", "ltr_knn_split_cloud", "ltr_scanside_split", "ltr_scanside_stats", "ltr_icp_params_default", "ltr_icp_refine", "ltr_knn_diff_refined", "ltr_debug_pixel_index", "ltr_debug_scan_rimg", "ltr_debug_fast_project", "ltr_debug_atan_sweep", "ltr_debug_margins", "ltr_reset_rimg_size", "ltr_last_pass_stats", "ltr_profile_get", "ltr_profile_reset", "ltr_timer_start", "ltr_timer_stop", "ltr_trace_dump",
+    "ltr_knn_diff", "ltr_knn_split_cloud", "ltr_scanside_split", "ltr_scanside_stats", "ltr_icp_params_default", "ltr_icp_refine", "ltr_knn_diff_refined", "ltr_debug_pixel_index", "ltr_debug_scan_rimg", "ltr_debug_exact_knn_avg", "ltr_debug_nearest", "ltr_debug_fast_project", "ltr_debug_atan_sweep", "ltr_debug_margins", "ltr_reset_rimg_size", "ltr_last_pass_stats", "ltr_profile_get", "ltr_profile_reset", "ltr_timer_start", "ltr_timer_stop", "ltr_trace_dump",
     "ltr_pinned_alloc", "ltr_pinned_free", "ltr_nccl_unique_id", "ltr_nccl_init", "ltr_nccl_split", "ltr_nccl_info", "ltr_nccl_destroy", "ltr_nccl_version", "ltr_nccl_allreduce_flags",
     "ltr_nccl_allgather_clouds", "ltr_nccl_exchange_clouds", "ltr_nccl_voxel_centroid_merged", "ltr_nccl_allgather_i64", "ltr_nccl_max_f64", "ltr_nccl_barrier", "ltr_stream_handle",
 ]
@@ -116,6 +116,8 @@ def lib():
     L.ltr_knn_diff_refined.argtypes = [vp, i32, i32, i32, i32, i32, f32, vp, vp, P(i32), P(i32)]
     L.ltr_debug_pixel_index.argtypes = [vp, vp, i64, i32, i32, vp, vp, vp, vp, vp]
     L.ltr_debug_scan_rimg.argtypes = [vp, i32, i32, ctypes.c_float, vp]
+    L.ltr_debug_exact_knn_avg.argtypes = [vp, i32, i32, i32, i32, vp, P(i64)]
+    L.ltr_debug_nearest.argtypes = [vp, i32, i32, vp, vp]
     L.ltr_debug_fast_project.argtypes = [vp, vp, i64, vp, f32, vp, vp]
     L.ltr_debug_atan_sweep.argtypes = [vp, i32, P(ctypes.c_double), P(f32)]
     L.ltr_debug_margins.argtypes = [vp, f32, vp]
@@ -441,6 +443,24 @@ class Context:
         out = np.empty((rows, cols), np.float32)
         self._ck(lib().ltr_debug_scan_rimg(self._h, scans, kf, res_alpha, out.ctypes.data))
         return out
+
+    def debug_exact_knn_avg(self, query, k, target=None):
+        """(avg (n,) float32, unsettled) of ltr_debug_exact_knn_avg: scan set `query` against cloud `target`, or each keyframe of `query`
+        against its own points when target is None."""
+        n = self.scanset_info(query)[1]
+        out = np.empty(n, np.float32)
+        un = ctypes.c_int64()
+        self._ck(lib().ltr_debug_exact_knn_avg(self._h, query, -1 if target is None else target, 1 if target is None else 0, k,
+                                               out.ctypes.data, ctypes.byref(un)))
+        return out, un.value
+
+    def debug_nearest(self, query, target):
+        """(d (n,) float32, idx (n,) int32) of ltr_debug_nearest: ICP's nearest target point for every point of cloud `query`."""
+        n = self.cloud_size(query)
+        d = np.empty(n, np.float32)
+        idx = np.empty(n, np.int32)
+        self._ck(lib().ltr_debug_nearest(self._h, query, target, d.ctypes.data, idx.ctypes.data))
+        return d, idx
 
     def debug_fast_project(self, xyz, inv_pose, res_alpha):
         x = _f32(xyz).reshape(-1, 3)

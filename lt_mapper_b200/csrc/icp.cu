@@ -303,6 +303,28 @@ __global__ void __launch_bounds__(kIcpThreads) icp_kernel(Levels T, PtrView tgt,
     }
 }
 
+// every level of pyr up to the final one: nn1 may search all of them
+int build_all_levels(Pyramid& pyr, Levels* lv) {
+    *lv = Levels{};
+    for (int l = 0;; ++l) {
+        const Level* L;
+        LTR_TRY(pyr.get(l, &L));
+        lv->L[l] = *L;
+        lv->n = l + 1;
+        if (L->final_level) return LTR_OK;
+    }
+}
+
+__global__ void __launch_bounds__(256) nearest_debug_kernel(Levels T, PtrView q, float* __restrict__ d, int32_t* __restrict__ idx) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= q.n) return;
+    float v;
+    uint32_t j;
+    nn1(T, q.x[i], q.y[i], q.z[i], &v, &j);
+    d[i] = v;
+    idx[i] = (int32_t)j;
+}
+
 int check_scans_poses(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_offset, DevScanSet** sp, DevPoses** pp) {
     LTR_TRY(scanset_get(ctx, scans_h, sp));
     LTR_TRY(poses_get(ctx, poses_h, pp));
@@ -381,14 +403,8 @@ int ltr_icp_refine(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t
         // 2. the target's grid levels, all of them: every iteration searches them
         Pyramid pyr(ctx);
         pyr.init(view(tgt), nullptr, 1, tmn, tmx);
-        Levels lv{};
-        for (int l = 0;; ++l) {
-            const Level* L;
-            LTR_TRY(pyr.get(l, &L));
-            lv.L[l] = *L;
-            lv.n = l + 1;
-            if (L->final_level) break;
-        }
+        Levels lv;
+        LTR_TRY(build_all_levels(pyr, &lv));
         // 3. keyframe chunks of at most LTR_ICP_CHUNK_POINTS source points, one CTA per keyframe
         int64_t max_chunk = 0;
         const std::vector<int> kf_cut = plan_keyframe_chunks(src.h_off, env_points("LTR_ICP_CHUNK_POINTS", kChunkPoints, (int64_t)1 << 30), K,
@@ -442,6 +458,42 @@ int ltr_knn_diff_refined(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, i
     DevPoses* pp;
     LTR_TRY(check_scans_poses(ctx, scans_h, poses_h, pose_offset, &sp, &pp));   // this entry checks the pose range before k and thr
     return knn_diff(ctx, scans_h, poses_h, pose_offset, target_h, k, thr, true, T16, accepted, out_coexist, out_diff);
+}
+
+// The correspondence search of ltr_icp_refine (nn1 over every level of the target's pyramid) for every point of query_h.
+int ltr_debug_nearest(ltr_ctx* ctx, ltr_cloud query_h, ltr_cloud target_h, float* d_out, int32_t* idx_out) {
+    ApiTrace tr__(ctx, "ltr_debug_nearest");
+    if (!ctx || !d_out || !idx_out) return fail(ctx, LTR_ERR_INVALID, "null argument");
+    DevCloud* qp;
+    DevCloud* tp;
+    LTR_TRY(cloud_get(ctx, query_h, &qp));
+    LTR_TRY(cloud_get(ctx, target_h, &tp));
+    if (tp->n < 1) return fail(ctx, LTR_ERR_UNSUPPORTED, "empty target");
+    const DevCloud q = *qp, tgt = *tp;
+    float mn[3], mx[3];
+    uint32_t nonfinite = 0;
+    if (q.n > 0) {
+        LTR_TRY(minmax_xyz(ctx, q, mn, mx, &nonfinite));
+        if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite query coordinates (%u points)", nonfinite);
+    }
+    LTR_TRY(minmax_xyz(ctx, tgt, mn, mx, &nonfinite));
+    if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite target coordinates (%u points)", nonfinite);
+    if (q.n == 0) return LTR_OK;
+    Pyramid pyr(ctx);
+    pyr.init(view(tgt), nullptr, 1, mn, mx);
+    Levels lv;
+    LTR_TRY(build_all_levels(pyr, &lv));
+    void* p = nullptr;
+    ScratchGuard g_p(ctx, &p);
+    LTR_TRY(dev_alloc(ctx, &p, (size_t)q.n * 8));
+    float* dd = (float*)p;
+    int32_t* di = (int32_t*)(dd + q.n);
+    nearest_debug_kernel<<<(unsigned)((q.n + 255) / 256), 256, 0, ctx->stream>>>(lv, view(q), dd, di);
+    LTR_LAUNCH_CHECK(ctx);
+    LTR_CUDA(ctx, cudaMemcpyAsync(d_out, dd, (size_t)q.n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    LTR_CUDA(ctx, cudaMemcpyAsync(idx_out, di, (size_t)q.n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return LTR_OK;
 }
 
 }  // extern "C"

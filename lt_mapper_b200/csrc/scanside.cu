@@ -369,4 +369,51 @@ int ltr_scanside_stats(ltr_ctx* ctx, int64_t* stats4) {
     return LTR_OK;
 }
 
+// The exact k-NN averages of ltr_scanside_split (Pyramid + exact_avg_all, as its "scan minus map" branch calls them) for every point of
+// `query_h`, in one launch: against target_h (self == 0, avg_map), or keyframe j against its own points (self != 0, avg_scan).
+int ltr_debug_exact_knn_avg(ltr_ctx* ctx, ltr_scanset query_h, ltr_cloud target_h, int32_t self, int32_t k, float* avg_out, int64_t* unsettled) {
+    ApiTrace tr__(ctx, "ltr_debug_exact_knn_avg");
+    if (!ctx || !avg_out) return fail(ctx, LTR_ERR_INVALID, "null argument");
+    DevScanSet* sp;
+    LTR_TRY(scanset_get(ctx, query_h, &sp));
+    DevCloud* tp = nullptr;
+    if (!self) LTR_TRY(cloud_get(ctx, target_h, &tp));
+    if (k < 1 || k > kMaxK) return fail(ctx, LTR_ERR_UNSUPPORTED, "k = %d outside [1, %d]", k, kMaxK);
+    if (self && sp->K > kMaxSegments) return fail(ctx, LTR_ERR_UNSUPPORTED, "%d keyframes in one launch (at most %d)", sp->K, kMaxSegments);
+    if (!self && tp->n < 1) return fail(ctx, LTR_ERR_UNSUPPORTED, "empty target");
+    const DevScanSet q = *sp;
+    const int64_t n = q.pts.n;
+    if (n >= ((int64_t)1 << 32)) return fail(ctx, LTR_ERR_UNSUPPORTED, "%lld query points", (long long)n);
+    float qmn[3], qmx[3];
+    uint32_t nonfinite = 0;
+    if (n > 0) {
+        LTR_TRY(minmax_xyz(ctx, q.pts, qmn, qmx, &nonfinite));
+        if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite query coordinates (%u points)", nonfinite);
+    }
+    Pyramid T(ctx);
+    if (!self) {
+        float mn[3], mx[3];
+        LTR_TRY(minmax_xyz(ctx, *tp, mn, mx, &nonfinite));
+        if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite target coordinates (%u points)", nonfinite);
+        T.init(view(*tp), nullptr, 1, mn, mx);
+    }
+    int64_t un = 0;
+    if (n > 0) {
+        if (self) T.init(view(q.pts), q.d_off, q.K, qmn, qmx);
+        const int64_t cap = round_cap(n);
+        void* work = nullptr;
+        ScratchGuard g_work(ctx, &work);
+        LTR_TRY(dev_alloc(ctx, &work, (size_t)cap * 12 + 256));   // avg | two lists | counter
+        float* avg = (float*)work;
+        uint32_t* list_a = (uint32_t*)(avg + cap);
+        uint32_t* list_b = list_a + cap;
+        unsigned int* d_cnt = (unsigned int*)(list_b + cap);
+        LTR_TRY(exact_avg_all(ctx, T, k, view(q.pts), self ? q.d_off : nullptr, self ? q.K : 1, avg, list_a, list_b, d_cnt, &un));
+        LTR_CUDA(ctx, cudaMemcpyAsync(avg_out, avg, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    }
+    if (unsettled) *unsettled = un;
+    return LTR_OK;
+}
+
 }  // extern "C"
