@@ -280,7 +280,8 @@ int ltr_nccl_allgather_clouds(ltr_ctx* ctx, int32_t comm, int32_t count, const l
 /* octreeDownsampling (utility.cpp:204-219) of the rank-ordered concatenation of every rank's `local` cloud (a cloud merged over all
  * keyframes, utility.cpp:177-189), WITHOUT gathering the raw points: all-reduced bounding box, key-prefix ranges of equal population,
  * one exchange of each point to the owner of its range, local voxelisation with the global box, all-gather of the centroid slices.
- * The result (replicated on every rank) is bit-identical to ltr_voxel_centroid of the gathered cloud. */
+ * The result (replicated on every rank) is bit-identical to ltr_voxel_centroid of the gathered cloud.  A non-finite coordinate on any
+ * rank fails on every rank with LTR_ERR_UNSUPPORTED (as ltr_voxel_centroid), before any rank computes a key. */
 int ltr_nccl_voxel_centroid_merged(ltr_ctx* ctx, int32_t comm, ltr_cloud local, float leaf, ltr_cloud* out);
 /* n_send clouds go to `peer`, n_recv clouds come from `peer` (the peer calls with the mirrored counts) */
 int ltr_nccl_exchange_clouds(ltr_ctx* ctx, int32_t comm, int32_t peer, int32_t n_send, const ltr_cloud* send, int32_t n_recv, ltr_cloud* recv);
@@ -320,6 +321,12 @@ int ltr_debug_atan_sweep(ltr_ctx* ctx, int32_t which, double* max_abs_err, float
  * el_direct flag, the derived (un-inflated) column / row error bounds in pixels at r/rho = 1, and the seam limit [rad]: a fast azimuth
  * with |az| >= it is never certain (half a pixel short of +-pi) */
 int ltr_debug_margins(ltr_ctx* ctx, float res_alpha, float* margins9);
+/* ltr_nccl_voxel_centroid_merged for `world` simulated ranks in this one context, rank r holding locals[r]: the same rank-local stages,
+ * with host reductions for the all-reduces and rank-order concatenations for the point exchange and the final all-gather.  cuts (world - 1
+ * entries, may be NULL) receives the first prefix bin of each range after the first, send_counts (world * world, may be NULL) at
+ * [r * world + d] the points rank r sends to rank d; both are 0 when every rank is empty.  Errors as ltr_nccl_voxel_centroid_merged. */
+int ltr_debug_voxel_distributed(ltr_ctx* ctx, int32_t world, const ltr_cloud* locals /* world */, float leaf, ltr_cloud* out,
+                                uint32_t* cuts /* world-1, may be null */, int64_t* send_counts /* world*world, may be null */);
 /* resetRimgSize (utility.cpp:222-236) */
 void ltr_reset_rimg_size(float vfov, float hfov, float alpha, int32_t* rows, int32_t* cols);
 /* Statistics of the last ltr_remove_pass / ltr_parse_projected: [0] (point, keyframe) pairs projected, [1] pairs settled by

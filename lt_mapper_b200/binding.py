@@ -44,7 +44,7 @@ EXPORTS = [
     "ltr_scanset_free", "ltr_scanset_concat_per_keyframe", "ltr_scanset_flatten", "ltr_poses_upload", "ltr_poses_free",
     "ltr_preclean", "ltr_merge_scans_global", "ltr_voxel_centroid", "ltr_voxel_centroid_per_keyframe", "ltr_voxel_grid", "ltr_voxel_grid_per_keyframe", "ltr_remove_pass", "ltr_remove_pass_adaptive", "ltr_remove_pass_ball", "ltr_scan_images_release",
     "ltr_flags_device_ptr", "ltr_flags_download", "ltr_flags_upload", "ltr_apply_partition", "ltr_parse_projected",
-    "ltr_knn_diff", "ltr_knn_split_cloud", "ltr_scanside_split", "ltr_scanside_stats", "ltr_icp_params_default", "ltr_icp_refine", "ltr_knn_diff_refined", "ltr_debug_pixel_index", "ltr_debug_scan_rimg", "ltr_debug_exact_knn_avg", "ltr_debug_nearest", "ltr_debug_fast_project", "ltr_debug_atan_sweep", "ltr_debug_margins", "ltr_reset_rimg_size", "ltr_last_pass_stats", "ltr_profile_get", "ltr_profile_reset", "ltr_timer_start", "ltr_timer_stop", "ltr_trace_dump",
+    "ltr_knn_diff", "ltr_knn_split_cloud", "ltr_scanside_split", "ltr_scanside_stats", "ltr_icp_params_default", "ltr_icp_refine", "ltr_knn_diff_refined", "ltr_debug_pixel_index", "ltr_debug_scan_rimg", "ltr_debug_exact_knn_avg", "ltr_debug_nearest", "ltr_debug_fast_project", "ltr_debug_atan_sweep", "ltr_debug_margins", "ltr_debug_voxel_distributed", "ltr_reset_rimg_size", "ltr_last_pass_stats", "ltr_profile_get", "ltr_profile_reset", "ltr_timer_start", "ltr_timer_stop", "ltr_trace_dump",
     "ltr_pinned_alloc", "ltr_pinned_free", "ltr_nccl_unique_id", "ltr_nccl_init", "ltr_nccl_split", "ltr_nccl_info", "ltr_nccl_destroy", "ltr_nccl_version", "ltr_nccl_allreduce_flags",
     "ltr_nccl_allgather_clouds", "ltr_nccl_exchange_clouds", "ltr_nccl_voxel_centroid_merged", "ltr_nccl_allgather_i64", "ltr_nccl_max_f64", "ltr_nccl_barrier", "ltr_stream_handle",
 ]
@@ -121,6 +121,7 @@ def lib():
     L.ltr_debug_fast_project.argtypes = [vp, vp, i64, vp, f32, vp, vp]
     L.ltr_debug_atan_sweep.argtypes = [vp, i32, P(ctypes.c_double), P(f32)]
     L.ltr_debug_margins.argtypes = [vp, f32, vp]
+    L.ltr_debug_voxel_distributed.argtypes = [vp, i32, vp, f32, P(i32), vp, vp]
     L.ltr_reset_rimg_size.argtypes = [f32, f32, f32, P(i32), P(i32)]
     L.ltr_reset_rimg_size.restype = None
     L.ltr_last_pass_stats.argtypes = [vp, vp]
@@ -242,6 +243,12 @@ class Context:
     def cloud_concat(self, a, b):
         h = ctypes.c_int32()
         self._ck(lib().ltr_cloud_concat(self._h, a, b, ctypes.byref(h)))
+        return h.value
+
+    def cloud_slice(self, c, begin, end):
+        """Non-owning view of the points [begin, end) of cloud `c` (ltr_cloud_slice): valid while `c` lives, freed like any cloud."""
+        h = ctypes.c_int32()
+        self._ck(lib().ltr_cloud_slice(self._h, c, begin, end, ctypes.byref(h)))
         return h.value
 
     def scanset_upload(self, xyzi, offsets):
@@ -480,6 +487,17 @@ class Context:
         m = np.zeros(9, np.float32)
         self._ck(lib().ltr_debug_margins(self._h, res_alpha, m.ctypes.data))
         return m
+
+    def debug_voxel_distributed(self, locals_, leaf):
+        """ltr_debug_voxel_distributed over len(locals_) simulated ranks, rank r holding cloud locals_[r]: (handle of the voxelised
+        concatenation, cuts (world - 1,) uint32, send counts (world, world) int64 with [r, d] = points rank r sends to rank d)."""
+        G = len(locals_)
+        hs = np.ascontiguousarray(locals_, np.int32)
+        cuts = np.zeros(max(G - 1, 1), np.uint32)
+        sc = np.zeros((max(G, 1), max(G, 1)), np.int64)
+        h = ctypes.c_int32()
+        self._ck(lib().ltr_debug_voxel_distributed(self._h, G, hs.ctypes.data, leaf, ctypes.byref(h), cuts.ctypes.data, sc.ctypes.data))
+        return h.value, cuts[: max(G - 1, 0)], sc[:G, :G]
 
     def last_pass_stats(self):
         s = np.zeros(7, np.float64)

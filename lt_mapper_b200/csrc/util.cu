@@ -6,6 +6,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <algorithm>
+#include <deque>
 
 namespace ltr {
 
@@ -354,7 +355,7 @@ static inline float ord2f(uint32_t o) {
 }
 
 // nonfinite (may be null): incremented by the number of points with a non-finite x, y or z.  fminf / fmaxf skip NaN, so the
-// extrema alone do not reveal them (an all-NaN cloud leaves the initial encodings, which decode to NaN).
+// extrema alone do not reveal them (an all-NaN cloud gives min FLT_MAX and max -FLT_MAX).
 __global__ void __launch_bounds__(256) minmax_kernel(PtrView c, uint32_t* __restrict__ out /* 6: min xyz, max xyz (ordered encoding) */,
                                                      uint32_t* __restrict__ nonfinite) {
     float mn[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, mx[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
@@ -618,12 +619,25 @@ static int voxel_view(ltr_ctx* ctx, const PtrView& v, float leaf, DevCloud* out,
 //      each group to its owner, which receives them in source-rank order == global insertion order
 //   4. the owner voxelises its range with the global box (stable sort + sequential f32 sums: bit-identical to the serial result)
 //   5. the centroid slices (8x fewer points than the input) are all-gathered in range order == octree order.
+// The rank-local work is split into the stages A-D below, which every rank runs between the collectives; voxel_distributed joins
+// them with NCCL, ltr_debug_voxel_distributed with host reductions and concatenations over simulated ranks of one context.  Every
+// decision that ends the call early is taken on a reduced value, so all ranks leave at the same point.
 // ------------------------------------------------------------------------------------------------
 constexpr int kDistHistBits = 12;
+constexpr int kDistHistWords = (1 << kDistHistBits) + 1;   // prefix bins, then the points outside the box
+// one rank's extrema block: [0, 3) min xyz, [3, 6) max xyz (ordered encodings), [6] points with a non-finite coordinate or
+// kDistTooLarge; then the local and the global histogram (kDistHistWords each).  [0, 3) is min-reduced, [3, 7) max-reduced.
+constexpr int kDistMmWords = 7;
+constexpr uint32_t kDistTooLarge = 0xffffffffu;
+constexpr size_t kDistMmBytes = (8 + 2 * (size_t)kDistHistWords) * sizeof(uint32_t);
 
-__global__ void __launch_bounds__(256) vox_prefix_hist_kernel(const uint64_t* __restrict__ keys, int64_t n, int shift, uint32_t* __restrict__ hist) {
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-        atomicAdd(&hist[(uint32_t)(keys[i] >> shift)], 1u);     // Morton-ordered or scan-ordered inputs: neighbouring threads mostly hit different bins
+// a point outside the box (counted by vox_key_kernel, and the call is rejected) has a code past the last bin: it is not binned
+__global__ void __launch_bounds__(256) vox_prefix_hist_kernel(const uint64_t* __restrict__ keys, int64_t n, int shift, uint32_t nbins,
+                                                              uint32_t* __restrict__ hist) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const uint64_t b = keys[i] >> shift;
+        if (b < nbins) atomicAdd(&hist[b], 1u);     // Morton-ordered or scan-ordered inputs: neighbouring threads mostly hit different bins
+    }
 }
 
 struct DestCuts { uint32_t ub[16]; int world; };   // destination of prefix bin b = number of cuts ub[j] (j < world - 1) with b >= ub[j]
@@ -645,112 +659,262 @@ __global__ void __launch_bounds__(256) gather_points_kernel(PtrView in, const ui
     out.x()[i] = in.x[s]; out.y()[i] = in.y[s]; out.z()[i] = in.z[s]; out.i()[i] = in.i[s];
 }
 
-static int voxel_distributed(ltr_ctx* ctx, int comm, const DevCloud& loc, float leaf, ltr_cloud* out_h) {
-    int me = 0, G = 1;
-    LTR_TRY(nccl_comm_info(ctx, comm, &me, &G));
+static int dist_check_args(ltr_ctx* ctx, int G, float leaf) {
     if (!(leaf > 0.0f)) return fail(ctx, LTR_ERR_INVALID, "voxel leaf must be positive");
     if (G > 16) return fail(ctx, LTR_ERR_UNSUPPORTED, "distributed voxeliser: more than 16 ranks");
-    const int64_t n = loc.n;
-    if (n >= (int64_t)1 << 31) return fail(ctx, LTR_ERR_UNSUPPORTED, "cloud too large for voxel centroid");
-    // 1. global extrema
-    void* p_mm = nullptr;
-    ScratchGuard g_mm(ctx, &p_mm);
-    LTR_TRY(dev_alloc(ctx, &p_mm, 8 * sizeof(uint32_t) + 2 * ((size_t)1 << kDistHistBits) * sizeof(uint32_t)));
-    uint32_t* d_mm = (uint32_t*)p_mm;
-    uint32_t* d_hist_loc = d_mm + 8;                       // 4096 local, then 4096 global
-    uint32_t* d_hist_glb = d_hist_loc + ((size_t)1 << kDistHistBits);
-    const uint32_t init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
+    return LTR_OK;
+}
+
+// Stage A: allocates the rank's extrema block (kDistMmBytes) and enqueues its local extrema and non-finite count
+static int dist_stage_extrema(ltr_ctx* ctx, const PtrView& loc, void** mm_block) {
+    LTR_TRY(dev_alloc(ctx, mm_block, kDistMmBytes));
+    uint32_t* d_mm = (uint32_t*)*mm_block;
+    const bool too_large = loc.n >= (int64_t)1 << 31;
+    const uint32_t init[kDistMmWords] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u, too_large ? kDistTooLarge : 0u};
     LTR_CUDA(ctx, cudaMemcpyAsync(d_mm, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
-    if (n > 0) {
-        const int blocks = (int)std::min<int64_t>((n + 255) / 256, (int64_t)ctx->sm_count * 8);
-        minmax_kernel<<<std::max(blocks, 1), 256, 0, ctx->stream>>>(view(loc), d_mm, nullptr);
+    if (loc.n > 0 && !too_large) {
+        const int blocks = (int)std::min<int64_t>((loc.n + 255) / 256, (int64_t)ctx->sm_count * 8);
+        minmax_kernel<<<std::max(blocks, 1), 256, 0, ctx->stream>>>(loc, d_mm, d_mm + 6);
         LTR_LAUNCH_CHECK(ctx);
     }
-    LTR_TRY(nccl_allreduce_u32(ctx, comm, d_mm, 3, 1));
-    LTR_TRY(nccl_allreduce_u32(ctx, comm, d_mm + 3, 3, 2));
-    uint32_t h_mm[6];
-    LTR_CUDA(ctx, cudaMemcpyAsync(h_mm, d_mm, sizeof(h_mm), cudaMemcpyDeviceToHost, ctx->stream));
-    LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (h_mm[0] == 0xffffffffu && h_mm[3] == 0u) return cloud_new(ctx, 0, out_h);    // every rank's cloud is empty
+    return LTR_OK;
+}
+
+// From the reduced extrema block: rejects non-finite input before define_box (whose cast of ceil(inf or NaN) to unsigned is undefined)
+// and before the empty test (an all-NaN cloud has no extrema), then either reports that every rank is empty or gives the global box and
+// the prefix histogram's bits and shift
+static int dist_decide_box(ltr_ctx* ctx, const uint32_t mm[kDistMmWords], float leaf, bool* empty, VoxBox* b, int* hb, int* shift) {
+    if (mm[6] == kDistTooLarge) return fail(ctx, LTR_ERR_UNSUPPORTED, "cloud too large for voxel centroid");
+    if (mm[6]) return fail(ctx, LTR_ERR_UNSUPPORTED, "points with non-finite coordinates (up to %u on one rank)", mm[6]);
+    *empty = mm[0] == 0xffffffffu && mm[3] == 0u;
+    if (*empty) return LTR_OK;
     float mn[3], mx[3];
-    for (int d = 0; d < 3; ++d) { mn[d] = ord2f(h_mm[d]); mx[d] = ord2f(h_mm[3 + d]); }
-    const VoxBox b = define_box(mn, mx, leaf);
-    if (b.depth > 21) return fail(ctx, LTR_ERR_UNSUPPORTED, "octree depth %d > 21 (extent/leaf too large)", b.depth);
-    // 2. local keys + prefix histogram
-    void* p = nullptr;
-    ScratchGuard g_p(ctx, &p);
+    for (int d = 0; d < 3; ++d) { mn[d] = ord2f(mm[d]); mx[d] = ord2f(mm[3 + d]); }
+    *b = define_box(mn, mx, leaf);
+    if (b->depth > 21) return fail(ctx, LTR_ERR_UNSUPPORTED, "octree depth %d > 21 (extent/leaf too large)", b->depth);
+    *hb = std::min(kDistHistBits, 3 * b->depth);
+    *shift = 3 * b->depth - *hb;
+    return LTR_OK;
+}
+
+// the key block of a rank with n local points: keys0 | keys1 | idx0 | idx1
+struct DistKeys { uint64_t *keys0, *keys1; uint32_t *idx0, *idx1; };
+static DistKeys dist_keys(void* block, int64_t n) {
     const int64_t nn = std::max<int64_t>(n, 1);
-    LTR_TRY(dev_alloc(ctx, &p, 2 * (size_t)nn * sizeof(uint64_t) + 2 * (size_t)nn * sizeof(uint32_t) + 256));
-    uint64_t* keys0 = (uint64_t*)p;
-    uint64_t* keys1 = keys0 + nn;
-    uint32_t* idx0 = (uint32_t*)(keys1 + nn);
-    uint32_t* idx1 = idx0 + nn;
-    unsigned int* bad = (unsigned int*)(idx1 + nn);
-    LTR_CUDA(ctx, cudaMemsetAsync(bad, 0, sizeof(unsigned int), ctx->stream));
-    LTR_CUDA(ctx, cudaMemsetAsync(d_hist_loc, 0, 2 * ((size_t)1 << kDistHistBits) * sizeof(uint32_t), ctx->stream));
-    const int hb = std::min(kDistHistBits, 3 * b.depth);
-    const int shift = 3 * b.depth - hb;
+    DistKeys k;
+    k.keys0 = (uint64_t*)block; k.keys1 = k.keys0 + nn;
+    k.idx0 = (uint32_t*)(k.keys1 + nn); k.idx1 = k.idx0 + nn;
+    return k;
+}
+
+// Stage B: allocates the key block and enqueues the local Morton keys under the global box and the local prefix histogram into
+// hist[0, 2^hb), the points outside the box into hist[2^hb]; clears the global histogram after it
+static int dist_stage_keys(ltr_ctx* ctx, const PtrView& loc, const VoxBox& b, int hb, int shift, uint32_t* hist, void** key_block) {
+    const int64_t n = loc.n, nn = std::max<int64_t>(n, 1);
+    LTR_TRY(dev_alloc(ctx, key_block, 2 * (size_t)nn * sizeof(uint64_t) + 2 * (size_t)nn * sizeof(uint32_t)));
+    const DistKeys k = dist_keys(*key_block, n);
+    LTR_CUDA(ctx, cudaMemsetAsync(hist, 0, 2 * (size_t)kDistHistWords * sizeof(uint32_t), ctx->stream));
     if (n > 0) {
-        vox_key_kernel<<<(unsigned)((n + kVoxKeyStride - 1) / kVoxKeyStride), 256, 0, ctx->stream>>>(view(loc), b, keys0, idx0, 0, bad, nullptr);
+        vox_key_kernel<<<(unsigned)((n + kVoxKeyStride - 1) / kVoxKeyStride), 256, 0, ctx->stream>>>(loc, b, k.keys0, k.idx0, 0, hist + (1 << hb), nullptr);
         LTR_LAUNCH_CHECK(ctx);
         const int blocks = (int)std::min<int64_t>((n + 255) / 256, (int64_t)ctx->sm_count * 8);
-        vox_prefix_hist_kernel<<<std::max(blocks, 1), 256, 0, ctx->stream>>>(keys0, n, shift, d_hist_loc);
+        vox_prefix_hist_kernel<<<std::max(blocks, 1), 256, 0, ctx->stream>>>(k.keys0, n, shift, 1u << hb, hist);
         LTR_LAUNCH_CHECK(ctx);
     }
-    LTR_CUDA(ctx, cudaMemcpyAsync(d_hist_glb, d_hist_loc, ((size_t)1 << kDistHistBits) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->stream));
-    LTR_TRY(nccl_allreduce_u32(ctx, comm, d_hist_glb, (size_t)1 << hb, 0));
-    std::vector<uint32_t> h_hist(2 * ((size_t)1 << kDistHistBits));
-    unsigned int hbad = 0;
-    LTR_CUDA(ctx, cudaMemcpyAsync(h_hist.data(), d_hist_loc, h_hist.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    LTR_CUDA(ctx, cudaMemcpyAsync(&hbad, bad, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
-    LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (hbad) return fail(ctx, LTR_ERR_UNSUPPORTED, "%u points fall outside the octree bounding box (non-finite coordinates?)", hbad);
-    const uint32_t* hl = h_hist.data();
-    const uint32_t* hg = h_hist.data() + ((size_t)1 << kDistHistBits);
-    const int nbins = 1 << hb;
+    return LTR_OK;
+}
+
+// Stage C, host part, from the global histogram hg (identical on every rank; hg[nbins] = points outside the box) and this rank's hl:
+// the cuts, and how many of this rank's points go to each rank
+static int dist_plan(ltr_ctx* ctx, const uint32_t* hl, const uint32_t* hg, int nbins, int G, DestCuts* cuts, std::vector<int64_t>* scount) {
+    if (hg[nbins]) return fail(ctx, LTR_ERR_UNSUPPORTED, "%u points fall outside the octree bounding box (non-finite coordinates?)", hg[nbins]);
     uint64_t total = 0;
     for (int i = 0; i < nbins; ++i) total += hg[i];
-    DestCuts cuts;
-    cuts.world = G;
-    {   // cut j = first bin at which the cumulative population reaches (j + 1) / G of the total (identical on every rank: global histogram)
+    cuts->world = G;
+    {   // cut j = first bin at which the cumulative population reaches (j + 1) / G of the total
         uint64_t cum = 0;
         int j = 0;
         for (int i = 0; i < nbins && j < G - 1; ++i) {
             cum += hg[i];
-            while (j < G - 1 && cum * (uint64_t)G >= total * (uint64_t)(j + 1)) cuts.ub[j++] = (uint32_t)(i + 1);
+            while (j < G - 1 && cum * (uint64_t)G >= total * (uint64_t)(j + 1)) cuts->ub[j++] = (uint32_t)(i + 1);
         }
-        while (j < G - 1) cuts.ub[j++] = (uint32_t)nbins;
+        while (j < G - 1) cuts->ub[j++] = (uint32_t)nbins;
     }
-    std::vector<int64_t> scount((size_t)G, 0);
+    scount->assign((size_t)G, 0);
+    std::vector<uint64_t> range((size_t)G, 0);
     for (int i = 0; i < nbins; ++i) {
         int d = 0;
-        for (int j = 0; j < G - 1; ++j) d += ((uint32_t)i >= cuts.ub[j]) ? 1 : 0;
-        scount[(size_t)d] += hl[i];
+        for (int j = 0; j < G - 1; ++j) d += ((uint32_t)i >= cuts->ub[j]) ? 1 : 0;
+        (*scount)[(size_t)d] += hl[i];
+        range[(size_t)d] += hg[i];
     }
-    // 3. group the local points by destination (stable), move them to their owners
+    for (int d = 0; d < G; ++d)
+        if (range[(size_t)d] >= (uint64_t)1 << 31) return fail(ctx, LTR_ERR_UNSUPPORTED, "cloud too large for voxel centroid (range %d)", d);
+    return LTR_OK;
+}
+
+// Stage C, device part: groups the local points by destination (stable) into `send`, segment d holding the points of range d
+static int dist_stage_group(ltr_ctx* ctx, const PtrView& loc, void* key_block, int shift, const DestCuts& cuts, const DevCloud& send) {
+    const int64_t n = loc.n;
+    if (n == 0) return LTR_OK;
+    const DistKeys k = dist_keys(key_block, n);
+    vox_dest_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(k.keys0, n, shift, cuts, k.keys1, k.idx1);
+    LTR_LAUNCH_CHECK(ctx);
+    uint64_t* ks; uint32_t* is;
+    LTR_TRY(radix_sort_pairs(ctx, k.keys1, k.keys0, k.idx1, k.idx0, n, 0, 8, &ks, &is));
+    gather_points_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(loc, is, send);
+    LTR_LAUNCH_CHECK(ctx);
+    return LTR_OK;
+}
+
+// Stage D is voxel_view(recv, leaf, &slice, &global_box): the owner's range with the GLOBAL box.
+
+static int voxel_distributed(ltr_ctx* ctx, int comm, const DevCloud& loc, float leaf, ltr_cloud* out_h) {
+    int me = 0, G = 1;
+    LTR_TRY(nccl_comm_info(ctx, comm, &me, &G));
+    LTR_TRY(dist_check_args(ctx, G, leaf));
+    const PtrView lv = view(loc);
+    // A. global extrema and non-finite flag
+    void* p_mm = nullptr;
+    ScratchGuard g_mm(ctx, &p_mm);
+    LTR_TRY(dist_stage_extrema(ctx, lv, &p_mm));
+    uint32_t* d_mm = (uint32_t*)p_mm;
+    LTR_TRY(nccl_allreduce_u32(ctx, comm, d_mm, 3, 1));
+    LTR_TRY(nccl_allreduce_u32(ctx, comm, d_mm + 3, 4, 2));
+    uint32_t h_mm[kDistMmWords];
+    LTR_CUDA(ctx, cudaMemcpyAsync(h_mm, d_mm, sizeof(h_mm), cudaMemcpyDeviceToHost, ctx->stream));
+    LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    bool empty = false;
+    VoxBox b;
+    int hb = 0, shift = 0;
+    LTR_TRY(dist_decide_box(ctx, h_mm, leaf, &empty, &b, &hb, &shift));
+    if (empty) return cloud_new(ctx, 0, out_h);    // every rank's cloud is empty
+    // B. local keys + prefix histogram, summed over the ranks
+    uint32_t* d_hist_loc = d_mm + 8;
+    uint32_t* d_hist_glb = d_hist_loc + kDistHistWords;
+    const int nbins = 1 << hb;
+    void* p = nullptr;
+    ScratchGuard g_p(ctx, &p);
+    LTR_TRY(dist_stage_keys(ctx, lv, b, hb, shift, d_hist_loc, &p));
+    LTR_CUDA(ctx, cudaMemcpyAsync(d_hist_glb, d_hist_loc, (size_t)(nbins + 1) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->stream));
+    LTR_TRY(nccl_allreduce_u32(ctx, comm, d_hist_glb, (size_t)nbins + 1, 0));
+    std::vector<uint32_t> h_hist(2 * (size_t)kDistHistWords);
+    LTR_CUDA(ctx, cudaMemcpyAsync(h_hist.data(), d_hist_loc, h_hist.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    // C. group the local points by destination (stable), move them to their owners
+    DestCuts cuts;
+    std::vector<int64_t> scount;
+    LTR_TRY(dist_plan(ctx, h_hist.data(), h_hist.data() + kDistHistWords, nbins, G, &cuts, &scount));
     CloudOwner g_send(ctx), g_recv(ctx), g_slice(ctx);
-    LTR_TRY(cloud_new(ctx, n, &g_send.h));
-    const ltr_cloud send_h = g_send.h;
-    if (n > 0) {
-        vox_dest_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(keys0, n, shift, cuts, keys1, idx1);
-        LTR_LAUNCH_CHECK(ctx);
-        uint64_t* ks; uint32_t* is;
-        LTR_TRY(radix_sort_pairs(ctx, keys1, keys0, idx1, idx0, n, 0, 8, &ks, &is));
-        gather_points_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(view(loc), is, ctx->clouds[send_h]);
-        LTR_LAUNCH_CHECK(ctx);
-    }
+    LTR_TRY(cloud_new(ctx, lv.n, &g_send.h));
+    LTR_TRY(dist_stage_group(ctx, lv, p, shift, cuts, ctx->clouds[g_send.h]));
     g_p.release();
-    LTR_TRY(nccl_alltoallv_cloud(ctx, comm, ctx->clouds[send_h], scount, &g_recv.h));
+    LTR_TRY(nccl_alltoallv_cloud(ctx, comm, ctx->clouds[g_send.h], scount, &g_recv.h));
     g_send.reset();
-    // 4. my range, with the GLOBAL box
+    // D. my range, with the GLOBAL box
     const DevCloud recv = ctx->clouds[g_recv.h];
     LTR_TRY(cloud_new(ctx, recv.n, &g_slice.h));
     DevCloud slice = ctx->clouds[g_slice.h];
     LTR_TRY(voxel_view(ctx, view(recv), leaf, &slice, &b));
     ctx->clouds[g_slice.h].n = slice.n;
-    // 5. slices in range order == octree order
+    // slices in range order == octree order
     const ltr_cloud local[1] = {g_slice.h};
     return ltr_nccl_allgather_clouds(ctx, comm, 1, local, out_h);
+}
+
+// The stages of voxel_distributed for `world` simulated ranks of one context: the min / max and sum all-reduces become host reductions,
+// the alltoallv a concatenation of every rank's destination segment in source-rank order, the all-gather a concatenation in rank order.
+static int voxel_distributed_simulated(ltr_ctx* ctx, int G, const ltr_cloud* locals, float leaf, ltr_cloud* out_h, uint32_t* cuts_out,
+                                       int64_t* send_counts) {
+    LTR_TRY(dist_check_args(ctx, G, leaf));
+    std::vector<PtrView> lv((size_t)G);
+    for (int r = 0; r < G; ++r) { DevCloud* c; LTR_TRY(cloud_get(ctx, locals[r], &c)); lv[(size_t)r] = view(*c); }
+    std::vector<void*> p_mm((size_t)G, nullptr), p_keys((size_t)G, nullptr);
+    std::deque<ScratchGuard> guards;
+    for (int r = 0; r < G; ++r) { guards.emplace_back(ctx, &p_mm[(size_t)r]); guards.emplace_back(ctx, &p_keys[(size_t)r]); }
+    // A
+    uint32_t mm[kDistMmWords] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u, 0u};
+    for (int r = 0; r < G; ++r) {
+        LTR_TRY(dist_stage_extrema(ctx, lv[(size_t)r], &p_mm[(size_t)r]));
+        uint32_t h[kDistMmWords];
+        LTR_CUDA(ctx, cudaMemcpyAsync(h, p_mm[(size_t)r], sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+        LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        for (int w = 0; w < kDistMmWords; ++w) mm[w] = w < 3 ? std::min(mm[w], h[w]) : std::max(mm[w], h[w]);
+    }
+    bool empty = false;
+    VoxBox b;
+    int hb = 0, shift = 0;
+    LTR_TRY(dist_decide_box(ctx, mm, leaf, &empty, &b, &hb, &shift));
+    if (cuts_out) for (int j = 0; j < G - 1; ++j) cuts_out[j] = 0;
+    if (send_counts) for (int j = 0; j < G * G; ++j) send_counts[j] = 0;
+    if (empty) return cloud_new(ctx, 0, out_h);
+    // B
+    const int nbins = 1 << hb;
+    std::vector<uint32_t> hl((size_t)G * kDistHistWords), hg((size_t)kDistHistWords, 0u);
+    for (int r = 0; r < G; ++r) {
+        uint32_t* hist = (uint32_t*)p_mm[(size_t)r] + 8;
+        LTR_TRY(dist_stage_keys(ctx, lv[(size_t)r], b, hb, shift, hist, &p_keys[(size_t)r]));
+        LTR_CUDA(ctx, cudaMemcpyAsync(&hl[(size_t)r * kDistHistWords], hist, kDistHistWords * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    for (int r = 0; r < G; ++r)
+        for (int i = 0; i <= nbins; ++i) hg[(size_t)i] += hl[(size_t)r * kDistHistWords + i];
+    // C
+    DestCuts cuts;
+    std::vector<std::vector<int64_t>> scount((size_t)G);
+    for (int r = 0; r < G; ++r) LTR_TRY(dist_plan(ctx, &hl[(size_t)r * kDistHistWords], hg.data(), nbins, G, &cuts, &scount[(size_t)r]));
+    std::deque<CloudOwner> send, recv, slice;
+    for (int r = 0; r < G; ++r) {
+        send.emplace_back(ctx);
+        LTR_TRY(cloud_new(ctx, lv[(size_t)r].n, &send.back().h));
+        LTR_TRY(dist_stage_group(ctx, lv[(size_t)r], p_keys[(size_t)r], shift, cuts, ctx->clouds[send.back().h]));
+    }
+    guards.clear();
+    for (int d = 0; d < G; ++d) {
+        int64_t m = 0;
+        for (int r = 0; r < G; ++r) m += scount[(size_t)r][(size_t)d];
+        recv.emplace_back(ctx);
+        LTR_TRY(cloud_new(ctx, m, &recv.back().h));
+        const DevCloud dst = ctx->clouds[recv.back().h];
+        int64_t at = 0;
+        for (int r = 0; r < G; ++r) {
+            const DevCloud src = ctx->clouds[send[(size_t)r].h];
+            int64_t from = 0;
+            for (int e = 0; e < d; ++e) from += scount[(size_t)r][(size_t)e];
+            const int64_t k = scount[(size_t)r][(size_t)d];
+            if (k > 0) LTR_CUDA(ctx, cudaMemcpy2DAsync(dst.base + at, (size_t)dst.cap * 4, src.base + from, (size_t)src.cap * 4, (size_t)k * 4, 4,
+                                                       cudaMemcpyDeviceToDevice, ctx->stream));
+            at += k;
+        }
+    }
+    send.clear();
+    // D
+    int64_t total = 0;
+    for (int d = 0; d < G; ++d) {
+        const DevCloud rc = ctx->clouds[recv[(size_t)d].h];
+        slice.emplace_back(ctx);
+        LTR_TRY(cloud_new(ctx, rc.n, &slice.back().h));
+        DevCloud s = ctx->clouds[slice.back().h];
+        LTR_TRY(voxel_view(ctx, view(rc), leaf, &s, &b));
+        ctx->clouds[slice.back().h].n = s.n;
+        total += s.n;
+    }
+    CloudOwner g_out(ctx);
+    LTR_TRY(cloud_new(ctx, total, &g_out.h));
+    const DevCloud o = ctx->clouds[g_out.h];
+    int64_t at = 0;
+    for (int d = 0; d < G; ++d) {
+        const DevCloud s = ctx->clouds[slice[(size_t)d].h];
+        if (s.n > 0) LTR_CUDA(ctx, cudaMemcpy2DAsync(o.base + at, (size_t)o.cap * 4, s.base, (size_t)s.cap * 4, (size_t)s.n * 4, 4,
+                                                     cudaMemcpyDeviceToDevice, ctx->stream));
+        at += s.n;
+    }
+    LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (cuts_out) for (int j = 0; j < G - 1; ++j) cuts_out[j] = cuts.ub[j];
+    if (send_counts) for (int r = 0; r < G; ++r) for (int d = 0; d < G; ++d) send_counts[r * G + d] = scount[(size_t)r][(size_t)d];
+    *out_h = g_out.h;
+    g_out.h = -1;
+    return LTR_OK;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -928,6 +1092,13 @@ int ltr_nccl_voxel_centroid_merged(ltr_ctx* ctx, int32_t comm, ltr_cloud local, 
     LTR_TRY(cloud_get(ctx, local, &c));
     const DevCloud loc = *c;
     return voxel_distributed(ctx, comm, loc, leaf, out);
+}
+
+int ltr_debug_voxel_distributed(ltr_ctx* ctx, int32_t world, const ltr_cloud* locals, float leaf, ltr_cloud* out, uint32_t* cuts,
+                                int64_t* send_counts) {
+    ApiTrace tr__(ctx, "ltr_debug_voxel_distributed");
+    if (!ctx || !out || !locals || world < 1) return fail(ctx, LTR_ERR_INVALID, "bad argument");
+    return voxel_distributed_simulated(ctx, world, locals, leaf, out, cuts, send_counts);
 }
 
 int ltr_voxel_centroid_per_keyframe(ltr_ctx* ctx, ltr_scanset in, float leaf, ltr_scanset* out) {
