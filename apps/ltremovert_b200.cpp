@@ -24,6 +24,15 @@
 //                      0.1 m (the range-proportional threshold calcDescrepancyAndParseDynamicPointIdx leaves commented out,
 //                      Removerter.cpp:393-402); c defaults to the reference's 0.05 and must lie in (0, 1).  Prints one summary line; the
 //                      output tree keeps its layout.  There is no yaml key: the reference has none.
+//     --compose=<gen_dir>[,<gen_dir>...]  LT-map change composition and map rollback (DESIGN.md §5.3) instead of Steps 0-3: the yaml's central
+//                      session (e.g. the last run's scans_updated/ with the central pose file, same keyframe selection and load-time
+//                      VoxelGrid) is the live map; the listed output trees of earlier runs, oldest first, give one delta each
+//                      (scans_pd/<name>, scans_nd_strong/<name> of every keyframe).  Writes composed/scans_pd/, composed/scans_nd_strong/
+//                      (the changes since the first listed run) and composed/scans_restored/ (the central scans as the first listed run
+//                      found them) under save_pcd_directory, and with saveMapPCD composed/restored_map.pcd.  The yaml's query session
+//                      must still list (its scan directory and pose file are read for the keyframe selection), but none of its scans
+//                      is loaded.  The Step 0-3 options (--selfremovert, --clean-scans, --icp-refinement, --adaptive-threshold,
+//                      --map-ball) are rejected with it.  Every listed file is checked on every rank before any collective.
 //     --map-ball       every removeOnce / revertOnce projects, per keyframe, only the map points within R m of the keyframe's pose (the
 //                      reference's kUseSubsetMapCloud / kBallSize, Removerter.h:46-48, off there; takeGlobalMapSubsetWithinBall,
 //                      Removerter.cpp:415-427); R defaults to the reference's 80 and must be finite and > 0.  The ND / PD filter passes and
@@ -136,7 +145,8 @@ int main(int argc, char** argv) {
     float adaptive_c = 0.0f;   // 0: the constant threshold
     float ball_r = 0.0f;       // 0: the full map
     const char* usage = "usage: %s --config params.yaml [--selfremovert] [--pcl110] [--no-split] [--clean-scans[=map|scan-minus-map]] [--icp-refinement]"
-                        " [--adaptive-threshold[=c], 0 < c < 1] [--map-ball[=R], R > 0]\n";
+                        " [--adaptive-threshold[=c], 0 < c < 1] [--map-ball[=R], R > 0] [--compose=<gen_dir>[,<gen_dir>...]]\n";
+    std::vector<std::string> compose_dirs;   // --compose: output trees of earlier runs, oldest first
     for (int i = 1; i < argc; ++i) {
         if (!std::strcmp(argv[i], "--config") && i + 1 < argc) cfg_path = argv[++i];
         else if (!std::strcmp(argv[i], "--selfremovert")) selfremovert = true;
@@ -152,6 +162,17 @@ int main(int argc, char** argv) {
             ball_r = std::strtof(argv[i] + 11, &end);
             if (end == argv[i] + 11 || *end || !(ball_r > 0.0f && ball_r <= 3.4028235e38f)) { std::fprintf(stderr, usage, argv[0]); return 2; }
         }
+        else if (!std::strncmp(argv[i], "--compose=", 10)) {
+            std::string list = argv[i] + 10;
+            for (size_t a = 0; a <= list.size();) {
+                const size_t b = std::min(list.find(',', a), list.size());
+                if (b == a) { std::fprintf(stderr, usage, argv[0]); return 2; }
+                std::string d = list.substr(a, b - a);
+                if (d.back() != '/') d += "/";
+                compose_dirs.push_back(d);
+                a = b + 1;
+            }
+        }
         else if (!std::strncmp(argv[i], "--adaptive-threshold=", 21)) {
             char* end = nullptr;
             adaptive_c = std::strtof(argv[i] + 21, &end);
@@ -160,6 +181,11 @@ int main(int argc, char** argv) {
         else { std::fprintf(stderr, usage, argv[0]); return 2; }
     }
     if (cfg_path.empty()) { std::fprintf(stderr, usage, argv[0]); return 2; }
+    if (!compose_dirs.empty() && (selfremovert || clean_scans >= 0 || icp_refinement || adaptive_c != 0.0f || ball_r != 0.0f)) {
+        std::fprintf(stderr, "--compose runs no Step 0-3: --selfremovert, --clean-scans, --icp-refinement, --adaptive-threshold and --map-ball "
+                             "cannot be combined with it\n");
+        return 2;
+    }
     const int rank = env_int("RANK", 0), world = std::max(1, env_int("WORLD_SIZE", 1));
     const bool split = world >= 2 && world % 2 == 0 && !no_split;
     YamlParams y;
@@ -195,10 +221,12 @@ int main(int argc, char** argv) {
     const int keyframe_gap = (int)y.num("removert/keyframe_gap", 10);
 
     // output tree (Removerter.cpp:28-50)
+    const bool compose = !compose_dirs.empty();
     fsmkdir(save_dir);
     const std::string d_updated = save_dir + "scans_updated", d_updated_strong = save_dir + "scans_updated_strong", d_pd = save_dir + "scans_pd",
                       d_pd_strong = save_dir + "scans_pd_strong", d_nd_strong = save_dir + "scans_nd_strong";
-    for (const std::string& d : {d_updated, d_updated_strong, d_pd, d_pd_strong, d_nd_strong, save_dir + "map_static", save_dir + "map_dynamic"}) fsmkdir(d);
+    if (!compose)
+        for (const std::string& d : {d_updated, d_updated_strong, d_pd, d_pd_strong, d_nd_strong, save_dir + "map_static", save_dir + "map_dynamic"}) fsmkdir(d);
 
     // Step 0 host side: loadSessionInfo, parseKeyframes, loadKeyframes (run() :1656-1659)
     LoadedSession C, Q;
@@ -224,8 +252,30 @@ int main(int argc, char** argv) {
     const bool owns_c = !split || rank < world / 2, owns_q = !split || rank >= world / 2;
     size_t c0, c1, q0, q1;
     block(C.files.keyframe_idx.size(), owns_c, &c0, &c1);
-    block(Q.files.keyframe_idx.size(), owns_q, &q0, &q1);
+    block(Q.files.keyframe_idx.size(), owns_q && !compose, &q0, &q1);   // composition needs no query session
     if (!load_keyframes(C, c0, c1, &err) || !load_keyframes(Q, q0, q1, &err)) { std::fprintf(stderr, "%s\n", err.c_str()); return 1; }
+    // --compose: one generation per listed tree, what its Step 3 added (scans_pd/) and removed (scans_nd_strong/) in each of this rank's
+    // keyframes; read before any collective, so that a missing file stops every rank (agreed below) instead of leaving the others waiting
+    std::vector<std::vector<float>> delta_pts;
+    std::vector<std::vector<int64_t>> delta_off;
+    std::string delta_bad;
+    for (const std::string& g : compose_dirs) {
+        for (const char* sub : {"scans_pd/", "scans_nd_strong/"}) {
+            delta_pts.emplace_back();
+            delta_off.emplace_back(1, 0);
+            for (const std::string& name : C.keyframe_names) {
+                const std::string path = g + sub + name;
+                HostCloud pts;
+                if (delta_bad.empty() && (!fs::exists(path) || !read_pcd(path, &pts, &err))) delta_bad = path;
+                if (!delta_bad.empty()) break;
+                const float* f = reinterpret_cast<const float*>(pts.data());
+                delta_pts.back().insert(delta_pts.back().end(), f, f + 4 * pts.size());
+                delta_off.back().push_back(delta_off.back().back() + (int64_t)pts.size());
+            }
+        }
+    }
+    if (!delta_bad.empty()) std::fprintf(stderr, "[rank %d] cannot read delta scan %s\n", rank, delta_bad.c_str());
+    if (!delta_bad.empty() && world == 1) return 1;
 
     Removerter R(P);
     if (R.init() != LTR_OK) { std::fprintf(stderr, "GPU context: %s\n", R.err.c_str()); return 1; }
@@ -244,6 +294,37 @@ int main(int argc, char** argv) {
         if (overflow_warnings)
             std::fprintf(stderr, "[pcl::VoxelGrid::applyFilter] Leaf size is too small for the input dataset (%d scans returned unchanged)\n", overflow_warnings);
         std::vector<float>().swap(S.xyzi);   // the raw scans now live on the device
+    }
+    if (compose) {
+        int64_t bad = delta_bad.empty() ? 0 : 1;
+        if (world > 1) {   // every rank leaves when any rank lacks a delta file
+            std::vector<int64_t> all((size_t)world);
+            ck(ltr_nccl_allgather_i64(R.ctx, R.nccl_world, &bad, 1, all.data()), "delta file check");
+            for (int64_t b : all) bad |= b;
+        }
+        if (bad) {
+            if (delta_bad.empty()) std::fprintf(stderr, "[rank %d] another rank cannot read its delta scans\n", rank);
+            return 1;
+        }
+        ck(R.set_delta_maps(true), "delta maps");
+        for (size_t g = 0; g < compose_dirs.size(); ++g)
+            ck(R.delta_load(delta_pts[2 * g].data(), delta_off[2 * g].data(), delta_pts[2 * g + 1].data(), delta_off[2 * g + 1].data()), "delta_load");
+        std::vector<std::vector<float>>().swap(delta_pts);
+        const int T = (int)R.deltas_.size();
+        ck(R.compose_changes(0, T), "compose_changes");
+        ck(R.rollback(0), "rollback");
+        const std::string dc = save_dir + "composed/";
+        bool ok = true;
+        if (owns_c) {
+            for (const char* d : {"scans_pd", "scans_nd_strong", "scans_restored"}) fsmkdir(dc + d);
+            ok &= save_scans(R, R.central_sess_.composed_pd_, C.keyframe_names, dc + "scans_pd", false);
+            ok &= save_scans(R, R.central_sess_.composed_nd_, C.keyframe_names, dc + "scans_nd_strong", false);
+            ok &= save_scans(R, R.central_sess_.keyframe_scans_restored_, C.keyframe_names, dc + "scans_restored", true);
+            if (save_map_pcd && rank == 0) ok &= save_cloud(R, R.saved.at("restored_map"), dc + "restored_map.pcd", true);
+        }
+        if (world > 1 && R.nccl_world >= 0) ltr_nccl_barrier(R.ctx, R.nccl_world);
+        if (rank == 0) std::printf(" %d generations composed, outputs written to %s (%s)\n", T, dc.c_str(), ok ? "ok" : "WITH ERRORS");
+        return ok ? 0 : 1;
     }
     R.adaptiveThresholdCoeff_ = adaptive_c;   // checked above
     if (adaptive_c != 0.0f && rank == 0)

@@ -202,6 +202,15 @@ int ltr_knn_diff(ltr_ctx* ctx, ltr_scanset scans, ltr_poses poses, int32_t pose_
  * Session::removeWeakNDMapPointsHavingStrongNDInNear (Session.cpp:452-484). near = |avg| < thr, far = the rest.
  * With any query point, a target of k or more points with a non-finite coordinate fails with LTR_ERR_UNSUPPORTED. */
 int ltr_knn_split_cloud(ltr_ctx* ctx, ltr_cloud query, ltr_cloud target, int32_t k, float thr, ltr_cloud* out_near, ltr_cloud* out_far);
+/* The same decision rule keyframe by keyframe, the set difference of LT-map change composition (DESIGN.md §5.3): every point of keyframe j
+ * of `query` against the points of keyframe j of `target` only (no transforms).  near = |avg| < thr, far = the rest, both in input order
+ * within each keyframe; either output may be NULL.  A target keyframe of 0 < n < k points contributes all n (sum still divided by k); an
+ * EMPTY target keyframe is not an error here: all its query points are far.  query and target must have the same number of keyframes
+ * (LTR_ERR_INVALID), 1 <= k <= 16 (LTR_ERR_UNSUPPORTED), thr finite and > 0 (LTR_ERR_INVALID).  A non-finite coordinate in either input fails
+ * with LTR_ERR_UNSUPPORTED before any output exists.  Keyframes go in launches of at most 8192 keyframes and LTR_DELTA_CHUNK_POINTS query +
+ * target points (environment; default 2^24, one keyframe at least). */
+int ltr_knn_split_per_keyframe(ltr_ctx* ctx, ltr_scanset query, ltr_scanset target, int32_t k, float thr, ltr_scanset* out_near,
+                               ltr_scanset* out_far);
 
 /* criteria of ltr_scanside_split */
 typedef enum ltr_scanside_criterion {

@@ -85,6 +85,26 @@ int ltrh_reset_to_step0(ltrh_removerter* r);
  * entry does exactly that in device memory (the scans never leave the GPU) after ltrh_run_step3: central keyframe_scans_ <- VoxelGrid(keyframe_scans_updated_), central poses
  * kept, query session and every derived cloud released, log cleared.  Then ltrh_load_session(r, 1, next query) and run the steps again. */
 int ltrh_cascade_promote_updated(ltrh_removerter* r);
+/* LT-map delta maps, change composition and map rollback (the LT-mapper paper's Fig. 10, §IV-C; DESIGN.md §5.3).  Off by default.  With
+ * on != 0 every later ltrh_cascade_promote_updated records the finished generation's delta (PD_g, ND_g) = (keyframe_scans_pd_,
+ * keyframe_scans_strong_nd_) of the central session, per keyframe in that keyframe's LiDAR frame, instead of releasing it.  on == 0 frees
+ * the recorded generations (as ltrh_destroy does). */
+int ltrh_set_delta_maps(ltrh_removerter* r, int32_t on);
+/* Appends one generation from host arrays (what an earlier run wrote to scans_pd/ and scans_nd_strong/): K + 1 offsets each, K = this
+ * rank's central keyframes.  Delta maps must be on (LTR_ERR_INVALID otherwise). */
+int ltrh_delta_load(ltrh_removerter* r, const float* pd_xyzi, const int64_t* pd_off, const float* nd_xyzi, const int64_t* nd_off);
+/* number of recorded generations */
+int32_t ltrh_delta_count(ltrh_removerter* r);
+/* The changes from generation i to generation j, composed from the deltas [i, j) (0 <= i < j <= count): the central scan sets "composed_pd_"
+ * (points added since i) and "composed_nd_" (points removed since i) (ltrh_scanset).  One generation gives its recorded delta unchanged.
+ * Delta maps off or a bad range: LTR_ERR_INVALID. */
+int ltrh_compose_changes(ltrh_removerter* r, int32_t i, int32_t j);
+/* Map rollback: the central scans as of generation i (0 <= i <= count; i == count gives the live scans), restored from the live central
+ * keyframe_scans_ and the deltas [i, count) without snapshots: the scan set "keyframe_scans_restored_" and the cloud "saved:restored_map"
+ * (merged and voxelised at 0.05 m).  An approximation of the earlier session, as in the paper.  Delta maps off or i outside [0, count]:
+ * LTR_ERR_INVALID.  Multi-GPU (this and ltrh_compose_changes): every rank calls; each works on its own central keyframes, the restored
+ * map is merged over them, ranks without central keyframes return LTR_OK. */
+int ltrh_rollback(ltrh_removerter* r, int32_t i);
 /* Removerter::scansideRemovalForEachScan(map_sess, scan_sess) (Removerter.cpp:1253-1310, commented out in the reference; what
  * saveCleanScansPCD asks for): every keyframe of scan_sess held by this rank is split by ltr_scanside_split against map_sess's
  * map_global_curr_static_ with num_nn_points_within / dist_nn_points_within; criterion = ltr_scanside_criterion.  Results: the scan sets

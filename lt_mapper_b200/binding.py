@@ -44,7 +44,7 @@ EXPORTS = [
     "ltr_scanset_free", "ltr_scanset_concat_per_keyframe", "ltr_scanset_flatten", "ltr_poses_upload", "ltr_poses_free",
     "ltr_preclean", "ltr_merge_scans_global", "ltr_voxel_centroid", "ltr_voxel_centroid_per_keyframe", "ltr_voxel_grid", "ltr_voxel_grid_per_keyframe", "ltr_remove_pass", "ltr_remove_pass_adaptive", "ltr_remove_pass_ball", "ltr_scan_images_release",
     "ltr_flags_device_ptr", "ltr_flags_download", "ltr_flags_upload", "ltr_apply_partition", "ltr_parse_projected",
-    "ltr_knn_diff", "ltr_knn_split_cloud", "ltr_scanside_split", "ltr_scanside_stats", "ltr_icp_params_default", "ltr_icp_refine", "ltr_knn_diff_refined", "ltr_debug_pixel_index", "ltr_debug_scan_rimg", "ltr_debug_exact_knn_avg", "ltr_debug_nearest", "ltr_debug_fast_project", "ltr_debug_atan_sweep", "ltr_debug_margins", "ltr_debug_voxel_distributed", "ltr_reset_rimg_size", "ltr_last_pass_stats", "ltr_profile_get", "ltr_profile_reset", "ltr_timer_start", "ltr_timer_stop", "ltr_trace_dump",
+    "ltr_knn_diff", "ltr_knn_split_cloud", "ltr_knn_split_per_keyframe", "ltr_scanside_split", "ltr_scanside_stats", "ltr_icp_params_default", "ltr_icp_refine", "ltr_knn_diff_refined", "ltr_debug_pixel_index", "ltr_debug_scan_rimg", "ltr_debug_exact_knn_avg", "ltr_debug_nearest", "ltr_debug_fast_project", "ltr_debug_atan_sweep", "ltr_debug_margins", "ltr_debug_voxel_distributed", "ltr_reset_rimg_size", "ltr_last_pass_stats", "ltr_profile_get", "ltr_profile_reset", "ltr_timer_start", "ltr_timer_stop", "ltr_trace_dump",
     "ltr_pinned_alloc", "ltr_pinned_free", "ltr_nccl_unique_id", "ltr_nccl_init", "ltr_nccl_split", "ltr_nccl_info", "ltr_nccl_destroy", "ltr_nccl_version", "ltr_nccl_allreduce_flags",
     "ltr_nccl_allgather_clouds", "ltr_nccl_exchange_clouds", "ltr_nccl_voxel_centroid_merged", "ltr_nccl_allgather_i64", "ltr_nccl_max_f64", "ltr_nccl_barrier", "ltr_stream_handle",
 ]
@@ -108,6 +108,7 @@ def lib():
     L.ltr_parse_projected.argtypes = [vp, i32, i32, i32, i32, f32, P(i32)]
     L.ltr_knn_diff.argtypes = [vp, i32, i32, i32, i32, i32, f32, P(i32), P(i32)]
     L.ltr_knn_split_cloud.argtypes = [vp, i32, i32, i32, f32, P(i32), P(i32)]
+    L.ltr_knn_split_per_keyframe.argtypes = [vp, i32, i32, i32, f32, P(i32), P(i32)]
     L.ltr_scanside_split.argtypes = [vp, i32, i32, i32, i32, i32, i32, f32, P(i32), P(i32)]
     L.ltr_scanside_stats.argtypes = [vp, vp]
     L.ltr_icp_params_default.argtypes = [P(IcpParams)]
@@ -394,6 +395,13 @@ class Context:
     def knn_split_cloud(self, query, target, k, thr):
         a, b = ctypes.c_int32(), ctypes.c_int32()
         self._ck(lib().ltr_knn_split_cloud(self._h, query, target, k, thr, ctypes.byref(a), ctypes.byref(b)))
+        return a.value, b.value
+
+    def knn_split_per_keyframe(self, query, target, k, thr):
+        """(near, far) scan sets of ltr_knn_split_per_keyframe: keyframe j of `query` against keyframe j of `target`; an empty target
+        keyframe makes all its query points far."""
+        a, b = ctypes.c_int32(), ctypes.c_int32()
+        self._ck(lib().ltr_knn_split_per_keyframe(self._h, query, target, k, thr, ctypes.byref(a), ctypes.byref(b)))
         return a.value, b.value
 
     def scanside_split(self, scans, poses, map_, criterion, k, thr, pose_offset=0):

@@ -43,7 +43,8 @@ std::map<std::string, ltr_scanset*> Session::scanset_names() {
             {"scans_knn_diff_", &scans_knn_diff_}, {"keyframe_scans_updated_", &keyframe_scans_updated_},
             {"keyframe_scans_updated_strong_", &keyframe_scans_updated_strong_}, {"keyframe_scans_pd_", &keyframe_scans_pd_},
             {"keyframe_scans_strong_pd_", &keyframe_scans_strong_pd_}, {"keyframe_scans_strong_nd_", &keyframe_scans_strong_nd_},
-            {"keyframe_scans_weak_nd_", &keyframe_scans_weak_nd_}, {"scans_static_", &scans_static_}, {"scans_dynamic_", &scans_dynamic_}};
+            {"keyframe_scans_weak_nd_", &keyframe_scans_weak_nd_}, {"scans_static_", &scans_static_}, {"scans_dynamic_", &scans_dynamic_},
+            {"composed_pd_", &composed_pd_}, {"composed_nd_", &composed_nd_}, {"keyframe_scans_restored_", &keyframe_scans_restored_}};
 }
 
 Removerter::Removerter(const ltrh_params& p) : P(p) {
@@ -52,7 +53,7 @@ Removerter::Removerter(const ltrh_params& p) : P(p) {
 }
 
 Removerter::~Removerter() {
-    if (ctx) ltr_destroy(ctx);
+    if (ctx) { free_deltas(); ltr_destroy(ctx); }
 }
 
 int Removerter::fail(int code, const std::string& msg) { err = msg; return code; }
@@ -665,6 +666,16 @@ int Removerter::cascade_promote_updated() {
     if (owns(C) && C.keyframe_scans_updated_ < 0) return fail(LTR_ERR_INVALID, "cascade: Step 3 has not run (no keyframe_scans_updated_)");
     ltr_scanset promoted = -1;
     if (owns(C)) CK(ltr_voxel_grid_per_keyframe(ctx, C.keyframe_scans_updated_, P.downsample_voxel_size, &promoted, nullptr));
+    // with delta maps on, this generation's delta (what Step 3 added and removed, in each keyframe's frame) moves out of the session into
+    // deltas_ before the release below, so that it stays owned even if a free fails
+    if (deltaMaps_) {
+        std::pair<ltr_scanset, ltr_scanset> delta{-1, -1};
+        if (owns(C)) {
+            delta = {C.keyframe_scans_pd_, C.keyframe_scans_strong_nd_};
+            C.keyframe_scans_pd_ = C.keyframe_scans_strong_nd_ = -1;
+        }
+        deltas_.push_back(delta);
+    }
     for (Session* s : {&central_sess_, &query_sess_}) {
         for (auto& kv : s->cloud_names()) if (*kv.second >= 0) { CK(ltr_cloud_free(ctx, *kv.second)); *kv.second = -1; }
         for (auto& kv : s->scanset_names()) if (*kv.second >= 0) { CK(ltr_scanset_free(ctx, *kv.second)); *kv.second = -1; }
@@ -678,6 +689,142 @@ int Removerter::cascade_promote_updated() {
     log.clear();
     timing.clear();
     return LTR_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// LT-map delta maps: change composition and map rollback (DESIGN.md §5.3; the LT-mapper paper's Fig. 10, §IV-C).  Generation g's delta
+// is (PD_g, ND_g) = (keyframe_scans_pd_, keyframe_scans_strong_nd_) of the central session after Step 3 of the g-th pair: Step 3 adds
+// exactly PD (Session.cpp:362-380) and drops exactly strong ND (Removerter.cpp:1489-1512).  With per-keyframe clouds in each keyframe's
+// LiDAR frame, A (-) B = ltr_knn_split_per_keyframe's far part of A against B (num_nn_points_within, dist_nn_points_within),
+// V = ltr_voxel_centroid_per_keyframe at 0.05 m, ++ = ltr_scanset_concat_per_keyframe.  Composition over [i, j) starts from
+// (PD_i, ND_i) unchanged and folds every further generation g in:
+//   ND' = V((ND (-) PD_g) ++ (ND_g (-) PD)),   PD' = V((PD (-) ND_g) ++ (PD_g (-) ND))
+// so that removed-then-re-added and added-then-removed points cancel.  Rollback to generation i composes [i, T) over the T recorded
+// generations and restores V((L (-) PD) ++ ND) from the live central scans L.  Multi-GPU: each rank works on its own central keyframe
+// block; only the restored map's mergeAndDownsample crosses ranks.  Ranks without central keyframes record placeholders and return.
+// ---------------------------------------------------------------------------------------------------------------
+int Removerter::free_deltas() {
+    for (auto& g : deltas_) {
+        if (g.first >= 0) CK(ltr_scanset_free(ctx, g.first));
+        if (g.second >= 0) CK(ltr_scanset_free(ctx, g.second));
+    }
+    deltas_.clear();
+    return LTR_OK;
+}
+
+int Removerter::set_delta_maps(bool on) {
+    if (!on) CK(free_deltas());
+    deltaMaps_ = on;
+    return LTR_OK;
+}
+
+int Removerter::delta_load(const float* pd_xyzi, const int64_t* pd_off, const float* nd_xyzi, const int64_t* nd_off) {
+    if (!deltaMaps_) return fail(LTR_ERR_INVALID, "delta_load: delta maps are off (ltrh_set_delta_maps)");
+    std::pair<ltr_scanset, ltr_scanset> g{-1, -1};
+    if (owns(central_sess_)) {
+        if (!pd_off || !nd_off) return fail(LTR_ERR_INVALID, "delta_load: null offsets");
+        CK(ltr_scanset_upload(ctx, pd_xyzi, pd_off, central_sess_.num_keyframes_, &g.first));
+        const int rc = ltr_scanset_upload(ctx, nd_xyzi, nd_off, central_sess_.num_keyframes_, &g.second);
+        if (rc != LTR_OK) { err = ltr_last_error(ctx); ltr_scanset_free(ctx, g.first); return rc; }
+    }
+    deltas_.push_back(g);
+    return LTR_OK;
+}
+
+int Removerter::copy_scanset(ltr_scanset s, ltr_scanset* out) {
+    int32_t K = 0;
+    CK(ltr_scanset_info(ctx, s, &K, nullptr));
+    const std::vector<int64_t> zero((size_t)K + 1, 0);
+    ltr_scanset empty;
+    CK(ltr_scanset_upload(ctx, nullptr, zero.data(), K, &empty));
+    const int rc = ltr_scanset_concat_per_keyframe(ctx, s, empty, out);
+    ltr_scanset_free(ctx, empty);
+    CK(rc);
+    return LTR_OK;
+}
+
+int Removerter::set_difference(ltr_scanset a, ltr_scanset b, ltr_scanset* out) {
+    CK(ltr_knn_split_per_keyframe(ctx, a, b, P.num_nn_points_within, P.dist_nn_points_within, nullptr, out));
+    return LTR_OK;
+}
+
+int Removerter::concat_voxelise(ltr_scanset a, ltr_scanset b, ltr_scanset* out) {
+    ltr_scanset c = -1;
+    int rc = ltr_scanset_concat_per_keyframe(ctx, a, b, &c);
+    ltr_scanset_free(ctx, a);
+    ltr_scanset_free(ctx, b);
+    if (rc == LTR_OK) {
+        rc = ltr_voxel_centroid_per_keyframe(ctx, c, 0.05f, out);   // Session.cpp:374
+        ltr_scanset_free(ctx, c);
+    }
+    CK(rc);
+    return LTR_OK;
+}
+
+// (PD, ND) composed over the generations [i, j), i < j; new handles
+int Removerter::compose(int i, int j, ltr_scanset* pd_out, ltr_scanset* nd_out) {
+    ltr_scanset pd = -1, nd = -1;
+    CK(copy_scanset(deltas_[(size_t)i].first, &pd));
+    int rc = copy_scanset(deltas_[(size_t)i].second, &nd);
+    for (int g = i + 1; g < j && rc == LTR_OK; ++g) {
+        const ltr_scanset pdg = deltas_[(size_t)g].first, ndg = deltas_[(size_t)g].second;
+        ltr_scanset a = -1, b = -1, c = -1, d = -1, nd2 = -1, pd2 = -1;
+        if ((rc = set_difference(nd, pdg, &a)) != LTR_OK) break;
+        if ((rc = set_difference(ndg, pd, &b)) != LTR_OK) { ltr_scanset_free(ctx, a); break; }
+        if ((rc = set_difference(pd, ndg, &c)) != LTR_OK) { ltr_scanset_free(ctx, a); ltr_scanset_free(ctx, b); break; }
+        if ((rc = set_difference(pdg, nd, &d)) != LTR_OK) { ltr_scanset_free(ctx, a); ltr_scanset_free(ctx, b); ltr_scanset_free(ctx, c); break; }
+        if ((rc = concat_voxelise(a, b, &nd2)) != LTR_OK) { ltr_scanset_free(ctx, c); ltr_scanset_free(ctx, d); break; }
+        if ((rc = concat_voxelise(c, d, &pd2)) != LTR_OK) { ltr_scanset_free(ctx, nd2); break; }
+        ltr_scanset_free(ctx, pd); ltr_scanset_free(ctx, nd);
+        pd = pd2; nd = nd2;
+    }
+    if (rc != LTR_OK) {
+        if (pd >= 0) ltr_scanset_free(ctx, pd);
+        if (nd >= 0) ltr_scanset_free(ctx, nd);
+        return rc;
+    }
+    *pd_out = pd;
+    *nd_out = nd;
+    return LTR_OK;
+}
+
+int Removerter::compose_changes(int i, int j) {
+    if (!deltaMaps_) return fail(LTR_ERR_INVALID, "compose_changes: delta maps are off (ltrh_set_delta_maps)");
+    const int T = (int)deltas_.size();
+    if (i < 0 || i >= j || j > T) return fail(LTR_ERR_INVALID, "compose_changes: [" + std::to_string(i) + ", " + std::to_string(j) +
+                                                               ") is not a non-empty range of the " + std::to_string(T) + " recorded generations");
+    Session& C = central_sess_;
+    if (!owns(C)) return LTR_OK;
+    ltr_scanset pd, nd;
+    CK(compose(i, j, &pd, &nd));
+    CK(set(&C.composed_pd_, pd, true));
+    return set(&C.composed_nd_, nd, true);
+}
+
+int Removerter::rollback(int i) {
+    if (!deltaMaps_) return fail(LTR_ERR_INVALID, "rollback: delta maps are off (ltrh_set_delta_maps)");
+    const int T = (int)deltas_.size();
+    if (i < 0 || i > T) return fail(LTR_ERR_INVALID, "rollback: generation " + std::to_string(i) + " outside [0, " + std::to_string(T) + "]");
+    Session& C = central_sess_;
+    if (!owns(C)) return LTR_OK;
+    if (C.keyframe_scans_ < 0) return fail(LTR_ERR_INVALID, "rollback: no central keyframe scans");
+    ltr_scanset restored = -1;
+    if (i == T) {
+        CK(copy_scanset(C.keyframe_scans_, &restored));
+    } else {
+        ltr_scanset pd, nd, kept = -1;
+        CK(compose(i, T, &pd, &nd));
+        const int rc = set_difference(C.keyframe_scans_, pd, &kept);
+        ltr_scanset_free(ctx, pd);
+        if (rc != LTR_OK) { ltr_scanset_free(ctx, nd); return rc; }
+        CK(concat_voxelise(kept, nd, &restored));
+    }
+    CK(set(&C.keyframe_scans_restored_, restored, true));
+    ltr_cloud m;
+    CK(mergeAndDownsample(C, C.keyframe_scans_restored_, 0.05f, &m));
+    const int rc = save("restored_map", m);
+    ltr_cloud_free(ctx, m);
+    return rc;
 }
 
 }  // namespace ltremovert_b200
@@ -749,6 +896,28 @@ int ltrh_run_step12(ltrh_removerter* r) { r->R->err.clear(); return r->R->run_st
 int ltrh_run_step3(ltrh_removerter* r) { r->R->err.clear(); return r->R->run_step3(); }
 int ltrh_reset_to_step0(ltrh_removerter* r) { r->R->err.clear(); return r->R->reset_to_step0(); }
 int ltrh_cascade_promote_updated(ltrh_removerter* r) { if (!r) return LTR_ERR_INVALID; r->R->err.clear(); return r->R->cascade_promote_updated(); }
+
+int ltrh_set_delta_maps(ltrh_removerter* r, int32_t on) {
+    if (!r) return LTR_ERR_INVALID;
+    r->R->err.clear();
+    return r->R->set_delta_maps(on != 0);
+}
+int ltrh_delta_load(ltrh_removerter* r, const float* pd_xyzi, const int64_t* pd_off, const float* nd_xyzi, const int64_t* nd_off) {
+    if (!r) return LTR_ERR_INVALID;
+    r->R->err.clear();
+    return r->R->delta_load(pd_xyzi, pd_off, nd_xyzi, nd_off);
+}
+int32_t ltrh_delta_count(ltrh_removerter* r) { return r ? (int32_t)r->R->deltas_.size() : 0; }
+int ltrh_compose_changes(ltrh_removerter* r, int32_t i, int32_t j) {
+    if (!r) return LTR_ERR_INVALID;
+    r->R->err.clear();
+    return r->R->compose_changes(i, j);
+}
+int ltrh_rollback(ltrh_removerter* r, int32_t i) {
+    if (!r) return LTR_ERR_INVALID;
+    r->R->err.clear();
+    return r->R->rollback(i);
+}
 
 int ltrh_scanside_removal(ltrh_removerter* r, int32_t map_sess, int32_t scan_sess, int32_t criterion) {
     if (!r || (map_sess != 0 && map_sess != 1) || (scan_sess != 0 && scan_sess != 1)) return LTR_ERR_INVALID;

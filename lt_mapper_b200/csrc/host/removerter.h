@@ -7,6 +7,7 @@
 #include <cstdint>
 #include <map>
 #include <string>
+#include <utility>
 #include <vector>
 #include "../../../include/ltr_removert.h"
 
@@ -32,6 +33,9 @@ public:
                 keyframe_scans_strong_pd_ = -1, keyframe_scans_strong_nd_ = -1, keyframe_scans_weak_nd_ = -1;
     // scan-side removal of this session's scans (the commented central_/query_scans_{static,dynamic}_ of Removerter.h)
     ltr_scanset scans_static_ = -1, scans_dynamic_ = -1;
+    // LT-map change composition (DESIGN.md §5.3) on the central session: the composed delta of ltrh_compose_changes and the scans of
+    // ltrh_rollback, per keyframe of this rank
+    ltr_scanset composed_pd_ = -1, composed_nd_ = -1, keyframe_scans_restored_ = -1;
     // ICP refinement of the last extractLowDynPointsViaKnnDiff with useICPrefinement_ on (ltr_icp_refine), per keyframe of this rank
     std::vector<float> icp_T16_;
     std::vector<double> icp_fitness_;
@@ -81,6 +85,11 @@ public:
     int run_step3();
     int reset_to_step0();  // benchmark plumbing, see include/ltr_removert.h
     int cascade_promote_updated();  // LT-map cascade: keyframe_scans_updated_ -> the next run's central keyframe_scans_ (see .cpp)
+    // ---- LT-map delta maps (DESIGN.md §5.3; see .cpp) ----
+    int set_delta_maps(bool on);
+    int delta_load(const float* pd_xyzi, const int64_t* pd_off, const float* nd_xyzi, const int64_t* nd_off);
+    int compose_changes(int i, int j);
+    int rollback(int i);
 
     // ---- Session methods (Session.cpp) ----
     int parseScansViaProjection(Session& s, ltr_cloud map, ltr_scanset* vec_to_store);     // Session.cpp:348-360
@@ -125,6 +134,10 @@ public:
     ltrh_params P;
     bool useICPrefinement_ = false;   // Session.cpp:551 (`bool useICPrefinement { false }`), set by ltrh_set_icp_refinement
     float adaptiveThresholdCoeff_ = 0.0f;   // Removerter.cpp:395-396 (`adaptive_coeff`, commented out); 0: the constant 0.1 (:398), set by ltrh_set_adaptive_threshold
+    bool deltaMaps_ = false;   // ltrh_set_delta_maps: cascade_promote_updated records each generation's delta in deltas_
+    // per generation (PD_g, ND_g) = (keyframe_scans_pd_, keyframe_scans_strong_nd_) of this rank's central keyframes; -1 on ranks without
+    // central keyframes, so that every rank counts the same generations
+    std::vector<std::pair<ltr_scanset, ltr_scanset>> deltas_;
     float mapBallRadius_ = 0.0f;   // Removerter.h:46-48 (`kUseSubsetMapCloud` off, `kBallSize` 80 m); 0: the full map, set by ltrh_set_map_ball
     ltr_ctx* ctx = nullptr;
     int rank = 0, world = 1;
@@ -144,6 +157,11 @@ public:
 
 private:
     int load_session_scans(int sess, ltr_scanset ss, const double* poses, const double* inv_poses, int K);
+    int free_deltas();
+    int copy_scanset(ltr_scanset s, ltr_scanset* out);
+    int set_difference(ltr_scanset a, ltr_scanset b, ltr_scanset* out);          // a (-) b: the far part of a against b, per keyframe
+    int concat_voxelise(ltr_scanset a, ltr_scanset b, ltr_scanset* out);         // V(a ++ b), consumes a and b
+    int compose(int i, int j, ltr_scanset* pd, ltr_scanset* nd);
     int partitionCurrentMapGeneric(ltr_cloud* map, Session& source, ltr_scanset scans, int mode, float res, const char* what,
                                    bool keep_dynamic, ltr_cloud* stat, ltr_cloud* dyn);
 };

@@ -30,7 +30,7 @@ class Params(ctypes.Structure):
 
 
 HOST_EXPORTS = ["ltrh_params_default", "ltrh_create", "ltrh_destroy", "ltrh_last_error", "ltrh_context", "ltrh_comm_init_nccl", "ltrh_owns_session", "ltrh_invert_poses",
-                "ltrh_load_session", "ltrh_load_session_raw", "ltrh_run_step0", "ltrh_run_step12", "ltrh_run_step3", "ltrh_reset_to_step0", "ltrh_cascade_promote_updated", "ltrh_scanside_removal", "ltrh_set_icp_refinement", "ltrh_set_adaptive_threshold", "ltrh_set_map_ball", "ltrh_icp_stats", "ltrh_stage", "ltrh_cloud",
+                "ltrh_load_session", "ltrh_load_session_raw", "ltrh_run_step0", "ltrh_run_step12", "ltrh_run_step3", "ltrh_reset_to_step0", "ltrh_cascade_promote_updated", "ltrh_set_delta_maps", "ltrh_delta_load", "ltrh_delta_count", "ltrh_compose_changes", "ltrh_rollback", "ltrh_scanside_removal", "ltrh_set_icp_refinement", "ltrh_set_adaptive_threshold", "ltrh_set_map_ball", "ltrh_icp_stats", "ltrh_stage", "ltrh_cloud",
                 "ltrh_scanset", "ltrh_timing", "ltrh_log_count", "ltrh_log_get", "ltrh_io_last_error", "ltrh_io_read_pcd", "ltrh_io_write_pcd",
                 "ltrh_io_read_poses", "ltrh_io_parse_keyframes", "ltrh_io_parse_keyframes_in_roi", "ltrh_io_voxel_grid", "ltrh_io_voxel_grid_scans", "ltrh_io_yaml_get"]
 
@@ -62,6 +62,11 @@ def host_lib():
     L.ltrh_load_session_raw.argtypes = [vp, i32, vp, vp, vp, vp, i32]
     for f in ("ltrh_run_step0", "ltrh_run_step12", "ltrh_run_step3", "ltrh_reset_to_step0", "ltrh_cascade_promote_updated"):
         getattr(L, f).argtypes = [vp]
+    L.ltrh_set_delta_maps.argtypes = [vp, i32]
+    L.ltrh_delta_load.argtypes = [vp, vp, vp, vp, vp]
+    L.ltrh_delta_count.argtypes = [vp]
+    L.ltrh_compose_changes.argtypes = [vp, i32, i32]
+    L.ltrh_rollback.argtypes = [vp, i32]
     L.ltrh_scanside_removal.argtypes = [vp, i32, i32, i32]
     L.ltrh_set_icp_refinement.argtypes = [vp, i32]
     L.ltrh_set_adaptive_threshold.argtypes = [vp, ctypes.c_float]
@@ -208,6 +213,29 @@ class Removerter:
     def cascade_promote_updated(self):
         """LT-map cascade: the updated scans become the central session of the next run (ltrh_cascade_promote_updated)."""
         self._ck(host_lib().ltrh_cascade_promote_updated(self._h))
+
+    def set_delta_maps(self, on=True):
+        """LT-map delta maps (ltrh_set_delta_maps): later cascade promotions record each generation's (PD, strong ND) per keyframe; off
+        (the default) frees what was recorded."""
+        self._ck(host_lib().ltrh_set_delta_maps(self._h, 1 if on else 0))
+
+    def delta_load(self, pd_xyzi, pd_offsets, nd_xyzi, nd_offsets):
+        """Appends one generation's delta from arrays (ltrh_delta_load), offsets over this rank's central keyframes."""
+        pd = np.ascontiguousarray(pd_xyzi, np.float32).reshape(-1, 4); po = np.ascontiguousarray(pd_offsets, np.int64)
+        nd = np.ascontiguousarray(nd_xyzi, np.float32).reshape(-1, 4); no = np.ascontiguousarray(nd_offsets, np.int64)
+        self._ck(host_lib().ltrh_delta_load(self._h, pd.ctypes.data, po.ctypes.data, nd.ctypes.data, no.ctypes.data))
+
+    def delta_count(self):
+        return host_lib().ltrh_delta_count(self._h)
+
+    def compose_changes(self, i, j):
+        """Changes from generation i to j (ltrh_compose_changes): fills the central scan sets "composed_pd_" / "composed_nd_"."""
+        self._ck(host_lib().ltrh_compose_changes(self._h, i, j))
+
+    def rollback(self, i):
+        """The central scans as of generation i (ltrh_rollback): fills the scan set "keyframe_scans_restored_" and the cloud
+        "saved:restored_map"."""
+        self._ck(host_lib().ltrh_rollback(self._h, i))
 
     def scanside_removal(self, map_sess, scan_sess, criterion=0):
         """scansideRemovalForEachScan (ltrh_scanside_removal): fills the scan sets "scans_static_" / "scans_dynamic_" of scan_sess."""
