@@ -1,15 +1,15 @@
 // libltr_b200.so -- per-keyframe kNN set difference, the primitive of LT-map change composition and map rollback (DESIGN.md §5.3).
 //
 // ltr_knn_split_per_keyframe: every point of keyframe k of `query` is tested against the points of keyframe k of `target` only, with
-// the rule of ltr_knn_split_cloud (knn.cu): near iff |(float)(sum_double of its k smallest L2_Simple squared distances) / float(k)| < thr,
-// the distances ((dx*dx) + dy*dy) + dz*dz in f32 without FMA and summed in ascending order in double; a target keyframe of 0 < n < k
-// points contributes all n and the sum is still divided by k.  Unlike the other kNN entry points an empty target keyframe is not an
-// error: its query points are all "far" (an empty per-keyframe delta is the common case of composition).
+// the rule of every kNN decision (ref_math.cuh, TopK): near iff |(float)(sum_double of its k smallest L2_Simple squared distances) /
+// float(k)| < thr; a target keyframe of 0 < n < k points contributes all n and the sum is still divided by k (knn_label_all).  Unlike
+// the other kNN entry points an empty target keyframe is not an error: its query points are all "far" (an empty per-keyframe delta is the
+// common case of composition).
 //
 // Search.  One sparse grid level (sparse_grid.cuh, built by scanside.cu's build_level) keyed by (keyframe of the launch, cell) holds the
-// targets of the launch's keyframes.  One thread per query point walks the 27 cells around its own cell in its own keyframe, keeping
-// the k smallest distances in registers, and leaves as soon as the current k smallest give a mean below thr (knn.cu's early exit: the
-// final k smallest are element-wise <= the current ones and the double sum, its f32 rounding and the division are monotone).
+// targets of the launch's keyframes.  One thread per query point walks the 27 cells around its own cell in its own keyframe with the
+// dense grid's walk (ref_math.cuh, knn_label_27: k smallest distances in registers, early exit on "near"), one sparse row lookup
+// (sparse_grid.cuh, row_points) per row of three cells.
 // Why 27 cells are exact.  Let c = 1 / inv_cell be the cell side the indices are computed with and B(1) = ((1 - 2^-6) c)^2 (1 - 2^-20)
 // (shell_bound).  sparse_grid.cuh's header proves that every target point outside the 27-cell block has a computed distance STRICTLY
 // greater than B(1).  The host picks c so that B(1) >= k thr (1 + 2^-21), evaluated in double (relative error < 2^-50, far inside the
@@ -38,87 +38,26 @@ namespace ltr {
 
 namespace {
 
-constexpr int kMaxK = 16;
 constexpr int64_t kChunkPoints = (int64_t)1 << 24;
-
-// the KT smallest distances pushed so far, ascending; seen = pushes
-template <int KT>
-struct Smallest {
-    float d[KT];
-    int seen;
-    __device__ __forceinline__ void init() {
-#pragma unroll
-        for (int j = 0; j < KT; ++j) d[j] = __int_as_float(0x7f800000);
-        seen = 0;
-    }
-    __device__ __forceinline__ void push(float v) {
-        ++seen;
-        if (v < d[KT - 1]) {
-            d[KT - 1] = v;
-#pragma unroll
-            for (int j = KT - 1; j > 0; --j)
-                if (d[j] < d[j - 1]) { const float t = d[j]; d[j] = d[j - 1]; d[j - 1] = t; }
-        }
-    }
-    // accumulate(..., 0.0) in double over the min(seen, k) smallest, ascending; float(sum) / float(k) (Session.cpp:470-471, 592-594)
-    __device__ __forceinline__ bool near(int k, float thr) const {
-        const int cnt = seen < k ? seen : k;
-        double sum = 0.0;
-#pragma unroll
-        for (int j = 0; j < KT; ++j) if (j < cnt) sum = da(sum, (double)d[j]);
-        return fabsf(fd(__double2float_rn(sum), (float)k)) < thr;
-    }
-};
 
 // 1 = far, 0 = near for the query (qx, qy, qz) against segment seg of the level (a target keyframe of >= k points)
 template <int KT>
 __device__ __forceinline__ uint8_t grid_label(const Level& L, int seg, float qx, float qy, float qz, int k, float thr) {
-    Smallest<KT> b;
-    b.init();
-    long long c[3];
+    int c[3];
     const float q[3] = {qx, qy, qz};
+    // clamped to [-2, dim + 1]: a query's cell farther outside the box has no cell of the block either way
 #pragma unroll
-    for (int d = 0; d < 3; ++d) c[d] = cell_index((double)q[d], L.origin[d], L.inv_cell);
-    const long long xa = max(c[0] - 1, 0ll), xb = min(c[0] + 1, (long long)L.dim[0] - 1);
-    if (xa > xb) return 1;
+    for (int d = 0; d < 3; ++d) c[d] = (int)min(max(cell_index((double)q[d], L.origin[d], L.inv_cell), -2ll), (long long)L.dim[d] + 1);
     const uint32_t c0 = L.seg_first[seg], c1 = L.seg_first[seg + 1];
-    // rows of three x-adjacent cells, the query's own row first (knn.cu's order: most points settle there)
-    const unsigned pack_dy = 0x22161U, pack_dz = 0x28215U;
-#pragma unroll 1
-    for (int o = 0; o < 9; ++o) {
-        const long long z = c[2] + (long long)((pack_dz >> (2 * o)) & 3u) - 1, y = c[1] + (long long)((pack_dy >> (2 * o)) & 3u) - 1;
-        if (z < 0 || z >= L.dim[2] || y < 0 || y >= L.dim[1]) continue;
-        const unsigned long long ka = cell_key(seg, xa, y, z), kb = cell_key(seg, xb, y, z);
-        uint32_t lo = c0, hi = c1;
-        while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (L.keys[mid] < ka) lo = mid + 1; else hi = mid; }
-        for (uint32_t ci = lo; ci < c1 && L.keys[ci] <= kb; ++ci) {
-            const uint32_t e = L.start[ci + 1];
-            for (uint32_t p = L.start[ci]; p < e; ++p) {
-                const float4 t = L.pts[p];
-                b.push(l2_simple(qx, qy, qz, t.x, t.y, t.z));
-                if (KT <= 4 && b.seen >= k && b.near(k, thr)) return 0;
-            }
-        }
-        if (KT > 4 && b.seen >= k && b.near(k, thr)) return 0;
-    }
-    // fewer than k points in the block: a true k-th neighbour lies outside it, beyond B(1) -> far (file header)
-    if (b.seen < k) return 1;
-    return b.near(k, thr) ? 0 : 1;
-}
-
-// the n < k points of a small target keyframe by brute force
-template <int KT>
-__device__ __forceinline__ uint8_t small_label(PtrView t, int64_t t0, int64_t n, float qx, float qy, float qz, int k, float thr) {
-    Smallest<KT> b;
-    b.init();
-    for (int64_t p = t0; p < t0 + n; ++p) b.push(l2_simple(qx, qy, qz, t.x[p], t.y[p], t.z[p]));
-    return b.near(k, thr) ? 0 : 1;
+    auto rows = [&](int y, int z, int xa, int xb, uint32_t* s, uint32_t* e) { row_points(L, c0, c1, seg, xa, xb, y, z, s, e); };
+    return knn_label_27<KT>(rows, L.pts, c[0], c[1], c[2], L.dim, qx, qy, qz, k, thr);
 }
 
 // The queries [qbase, qbase + m) of keyframes [kf0, kf0 + nkf): flag[i] = 1 (far) or 0 (near) against keyframe kf of the target.
-// Segment j of L is keyframe kf0 + j.
+// Segment j of L is keyframe kf0 + j.  sm_90a: 34-37 registers for k <= 4, 48 for k > 4, no spill; the minimum of 8 CTAs per SM does not
+// bind at 48 registers, but with the bare bound ptxas gives k > 4 40 registers and a 12 B spill.
 template <int KT>
-__global__ void __launch_bounds__(128) knn_split_kf_kernel(Level L, PtrView q, const int64_t* __restrict__ q_off, PtrView t,
+__global__ void __launch_bounds__(128, 8) knn_split_kf_kernel(Level L, PtrView q, const int64_t* __restrict__ q_off, PtrView t,
                                                            const int64_t* __restrict__ t_off, int kf0, int nkf, int64_t qbase, int64_t m,
                                                            int k, float thr, uint8_t* __restrict__ flag) {
     const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -130,14 +69,9 @@ __global__ void __launch_bounds__(128) knn_split_kf_kernel(Level L, PtrView q, c
     const float x = q.x[i], y = q.y[i], z = q.z[i];
     uint8_t f;
     if (nt == 0) f = 1;
-    else if (nt < k) f = small_label<KT>(t, t0, nt, x, y, z, k, thr);
+    else if (nt < k) f = knn_label_all<KT>((int)nt, [&](int p) { return make_float4(t.x[t0 + p], t.y[t0 + p], t.z[t0 + p], 0.0f); }, x, y, z, k, thr);
     else f = grid_label<KT>(L, seg, x, y, z, k, thr);
     flag[i] = f;
-}
-
-__global__ void __launch_bounds__(256) rel_offsets_kernel(const int64_t* __restrict__ off, int kf0, int nkf, int64_t* __restrict__ out) {
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j <= nkf) out[j] = off[kf0 + j] - off[kf0];
 }
 
 int launch_split(ltr_ctx* ctx, int k, const Level& L, PtrView q, const int64_t* q_off, PtrView t, const int64_t* t_off, int kf0, int nkf,
@@ -148,7 +82,7 @@ int launch_split(ltr_ctx* ctx, int k, const Level& L, PtrView q, const int64_t* 
 #define LTR_DELTA_CASE(KK, KT) \
         case KK: knn_split_kf_kernel<KT><<<nb, 128, 0, ctx->stream>>>(L, q, q_off, t, t_off, kf0, nkf, qbase, m, k, thr, flag); break;
         LTR_DELTA_CASE(1, 1) LTR_DELTA_CASE(2, 2) LTR_DELTA_CASE(3, 3) LTR_DELTA_CASE(4, 4)
-        default: knn_split_kf_kernel<kMaxK><<<nb, 128, 0, ctx->stream>>>(L, q, q_off, t, t_off, kf0, nkf, qbase, m, k, thr, flag); break;
+        default: knn_split_kf_kernel<kKnnMaxK><<<nb, 128, 0, ctx->stream>>>(L, q, q_off, t, t_off, kf0, nkf, qbase, m, k, thr, flag); break;
 #undef LTR_DELTA_CASE
     }
     LTR_LAUNCH_CHECK(ctx);
@@ -185,20 +119,13 @@ int ltr_knn_split_per_keyframe(ltr_ctx* ctx, ltr_scanset query_h, ltr_scanset ta
     LTR_TRY(scanset_get(ctx, query_h, &qp));
     LTR_TRY(scanset_get(ctx, target_h, &tp));
     if (qp->K != tp->K) return fail(ctx, LTR_ERR_INVALID, "query has %d keyframes, target %d", qp->K, tp->K);
-    if (k < 1 || k > kMaxK) return fail(ctx, LTR_ERR_UNSUPPORTED, "k = %d outside [1, %d]", k, kMaxK);
+    if (k < 1 || k > kKnnMaxK) return fail(ctx, LTR_ERR_UNSUPPORTED, "k = %d outside [1, %d]", k, kKnnMaxK);
     if (!(thr > 0.0f) || !std::isfinite(thr)) return fail(ctx, LTR_ERR_INVALID, "threshold must be positive and finite");
     const DevScanSet Q = *qp, T = *tp;
     const int K = Q.K;
     float mn[3], mx[3];
-    uint32_t nonfinite = 0;
-    if (Q.pts.n > 0) {
-        LTR_TRY(minmax_xyz(ctx, Q.pts, mn, mx, &nonfinite));
-        if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite query coordinates (%u points)", nonfinite);
-    }
-    if (T.pts.n > 0) {
-        LTR_TRY(minmax_xyz(ctx, T.pts, mn, mx, &nonfinite));
-        if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite target coordinates (%u points)", nonfinite);
-    }
+    if (Q.pts.n > 0) LTR_TRY(finite_extent(ctx, Q.pts, "query", mn, mx));
+    if (T.pts.n > 0) LTR_TRY(finite_extent(ctx, T.pts, "target", mn, mx));
     if (Q.pts.n == 0) {
         const std::vector<int64_t> off((size_t)K + 1, 0);
         if (out_near) LTR_TRY(scanset_new(ctx, off, out_near));
@@ -238,8 +165,7 @@ int ltr_knn_split_per_keyframe(ltr_ctx* ctx, ltr_scanset query_h, ltr_scanset ta
                 tc.n = nt;
                 float tmn[3], tmx[3];
                 LTR_TRY(minmax_xyz(ctx, tc, tmn, tmx));
-                rel_offsets_kernel<<<(nkf + 1 + 255) / 256, 256, 0, ctx->stream>>>(T.d_off, kf0, nkf, t_rel);
-                LTR_LAUNCH_CHECK(ctx);
+                LTR_TRY(relative_offsets(ctx, T.d_off, kf0, nkf, t_rel));
                 LTR_TRY(build_level(ctx, view(tc), t_rel, nkf, tmn, tmx, launch_cell(k, thr, tmn, tmx), true, &lb));
             }
             LTR_TRY(launch_split(ctx, k, lb.L, view(Q.pts), Q.d_off, view(T.pts), T.d_off, kf0, nkf, qbase, m, thr, (uint8_t*)flags));

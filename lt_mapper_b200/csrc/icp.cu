@@ -325,14 +325,6 @@ __global__ void __launch_bounds__(256) nearest_debug_kernel(Levels T, PtrView q,
     idx[i] = (int32_t)j;
 }
 
-int check_scans_poses(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_offset, DevScanSet** sp, DevPoses** pp) {
-    LTR_TRY(scanset_get(ctx, scans_h, sp));
-    LTR_TRY(poses_get(ctx, poses_h, pp));
-    if (pose_offset < 0 || pose_offset + (*sp)->K > (*pp)->K)
-        return fail(ctx, LTR_ERR_INVALID, "pose range [%d,%d) outside [0,%d)", pose_offset, pose_offset + (*sp)->K, (*pp)->K);
-    return LTR_OK;
-}
-
 }  // namespace
 }  // namespace ltr
 
@@ -365,7 +357,9 @@ int ltr_icp_refine(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t
     DevScanSet* sp;
     DevPoses* pp;
     DevCloud* tp;
-    LTR_TRY(check_scans_poses(ctx, scans_h, poses_h, pose_offset, &sp, &pp));
+    LTR_TRY(scanset_get(ctx, scans_h, &sp));
+    LTR_TRY(poses_get(ctx, poses_h, &pp));
+    LTR_TRY(check_pose_range(ctx, *sp, *pp, pose_offset));
     LTR_TRY(cloud_get(ctx, target_h, &tp));
     if (tp->n < 1) return fail(ctx, LTR_ERR_UNSUPPORTED, "empty ICP target");
     const DevScanSet scans = *sp;
@@ -373,11 +367,7 @@ int ltr_icp_refine(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t
     const DevCloud tgt = *tp;
     const int K = scans.K;
     float tmn[3], tmx[3];
-    {
-        uint32_t nonfinite = 0;
-        LTR_TRY(minmax_xyz(ctx, tgt, tmn, tmx, &nonfinite));
-        if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite ICP target coordinates (%u points)", nonfinite);
-    }
+    LTR_TRY(finite_extent(ctx, tgt, "ICP target", tmn, tmx));
     std::vector<float> hT((size_t)K * 16);
     std::vector<double> hfit((size_t)K, DBL_MAX);
     std::vector<int32_t> hit((size_t)K, 0), hex((size_t)K, kExitNoCorrespondences);
@@ -393,9 +383,7 @@ int ltr_icp_refine(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t
                                 g.y(), g.z(), g.i()));
         {
             float mn[3], mx[3];
-            uint32_t nonfinite = 0;
-            LTR_TRY(minmax_xyz(ctx, g, mn, mx, &nonfinite));
-            if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite scan coordinates (%u points)", nonfinite);
+            LTR_TRY(finite_extent(ctx, g, "scan", mn, mx));
         }
         LTR_TRY(ltr_voxel_centroid_per_keyframe(ctx, g_glob.h, P.source_leaf, &g_src.h));
         g_glob.reset();
@@ -456,7 +444,9 @@ int ltr_knn_diff_refined(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, i
     if (!ctx) return LTR_ERR_INVALID;
     DevScanSet* sp;
     DevPoses* pp;
-    LTR_TRY(check_scans_poses(ctx, scans_h, poses_h, pose_offset, &sp, &pp));   // this entry checks the pose range before k and thr
+    LTR_TRY(scanset_get(ctx, scans_h, &sp));
+    LTR_TRY(poses_get(ctx, poses_h, &pp));
+    LTR_TRY(check_pose_range(ctx, *sp, *pp, pose_offset));   // this entry checks the pose range before k and thr
     return knn_diff(ctx, scans_h, poses_h, pose_offset, target_h, k, thr, true, T16, accepted, out_coexist, out_diff);
 }
 
@@ -471,13 +461,8 @@ int ltr_debug_nearest(ltr_ctx* ctx, ltr_cloud query_h, ltr_cloud target_h, float
     if (tp->n < 1) return fail(ctx, LTR_ERR_UNSUPPORTED, "empty target");
     const DevCloud q = *qp, tgt = *tp;
     float mn[3], mx[3];
-    uint32_t nonfinite = 0;
-    if (q.n > 0) {
-        LTR_TRY(minmax_xyz(ctx, q, mn, mx, &nonfinite));
-        if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite query coordinates (%u points)", nonfinite);
-    }
-    LTR_TRY(minmax_xyz(ctx, tgt, mn, mx, &nonfinite));
-    if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite target coordinates (%u points)", nonfinite);
+    if (q.n > 0) LTR_TRY(finite_extent(ctx, q, "query", mn, mx));
+    LTR_TRY(finite_extent(ctx, tgt, "target", mn, mx));
     if (q.n == 0) return LTR_OK;
     Pyramid pyr(ctx);
     pyr.init(view(tgt), nullptr, 1, mn, mx);

@@ -19,21 +19,13 @@
 
 namespace ltr {
 
-constexpr int kMaxK = 16;
-
-struct Grid {
-    double origin[3];
-    double inv_cell;
-    int dim[3];
-};
-
-__device__ __forceinline__ void cell_of(const Grid& g, float x, float y, float z, int* cx, int* cy, int* cz) {
+__device__ __forceinline__ void cell_of(const KnnTarget& g, float x, float y, float z, int* cx, int* cy, int* cz) {
     *cx = (int)floor(((double)x - g.origin[0]) * g.inv_cell);
     *cy = (int)floor(((double)y - g.origin[1]) * g.inv_cell);
     *cz = (int)floor(((double)z - g.origin[2]) * g.inv_cell);
 }
 
-__global__ void __launch_bounds__(256) grid_count_kernel(PtrView t, Grid g, uint32_t* __restrict__ cell_cnt) {
+__global__ void __launch_bounds__(256) grid_count_kernel(PtrView t, KnnTarget g, uint32_t* __restrict__ cell_cnt) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= t.n) return;
     int cx, cy, cz;
@@ -42,8 +34,7 @@ __global__ void __launch_bounds__(256) grid_count_kernel(PtrView t, Grid g, uint
     atomicAdd(&cell_cnt[((size_t)cz * g.dim[1] + cy) * g.dim[0] + cx], 1u);
 }
 
-__global__ void __launch_bounds__(256) grid_fill_kernel(PtrView t, Grid g, const uint32_t* __restrict__ cell_start, uint32_t* __restrict__ cursor,
-                                                        float4* __restrict__ sorted) {
+__global__ void __launch_bounds__(256) grid_fill_kernel(PtrView t, KnnTarget g, uint32_t* __restrict__ cursor, float4* __restrict__ sorted) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= t.n) return;
     const float x = t.x[i], y = t.y[i], z = t.z[i];
@@ -51,92 +42,39 @@ __global__ void __launch_bounds__(256) grid_fill_kernel(PtrView t, Grid g, const
     cell_of(g, x, y, z, &cx, &cy, &cz);
     cx = min(max(cx, 0), g.dim[0] - 1); cy = min(max(cy, 0), g.dim[1] - 1); cz = min(max(cz, 0), g.dim[2] - 1);
     const size_t c = ((size_t)cz * g.dim[1] + cy) * g.dim[0] + cx;
-    const uint32_t slot = cell_start[c] + atomicAdd(&cursor[c], 1u);
+    const uint32_t slot = g.cell_start[c] + atomicAdd(&cursor[c], 1u);
     sorted[slot] = make_float4(x, y, z, 0.0f);
 }
 
-// k smallest squared distances of (qx,qy,qz) among the 27 neighbouring cells -> decision "far" (1) or "near" (0).
-// KT >= k is the compile-time capacity of the register-resident ascending top list.
+// decision "far" (1) or "near" (0) of (qx,qy,qz) from the 27 cells around its cell of the dense grid
 template <int KT>
-__device__ __forceinline__ uint8_t knn_label(const Grid& g, const uint32_t* __restrict__ cell_start, const float4* __restrict__ sorted,
-                                             float qx, float qy, float qz, int k, float thr) {
-    const float kInf = __int_as_float(0x7f800000);
-    float best[KT];
-#pragma unroll
-    for (int j = 0; j < KT; ++j) best[j] = kInf;
+__device__ __forceinline__ uint8_t knn_label(const KnnTarget& t, float qx, float qy, float qz, int k, float thr) {
     int cx, cy, cz;
-    cell_of(g, qx, qy, qz, &cx, &cy, &cz);
-    const int x0 = max(cx - 1, 0), x1 = min(cx + 1, g.dim[0] - 1);
-    if (x0 <= x1) {
-        // rows of 3 x-adjacent cells, the query's own row first: most points have their k neighbours right there and
-        // leave through the early exit below
-        // (dy, dz) + 1 packed 2 bits per step: dy = {0,-1,1,0,0,-1,1,-1,1}, dz = {0,0,0,-1,1,-1,-1,1,1}
-        const unsigned pack_dy = 0x22161U, pack_dz = 0x28215U;
-#pragma unroll 1
-        for (int o = 0; o < 9; ++o) {
-            const int z = cz + (int)((pack_dz >> (2 * o)) & 3u) - 1, y = cy + (int)((pack_dy >> (2 * o)) & 3u) - 1;
-            if (z < 0 || z >= g.dim[2] || y < 0 || y >= g.dim[1]) continue;
-            const size_t row = ((size_t)z * g.dim[1] + y) * g.dim[0];
-            const uint32_t s = cell_start[row + x0], e = cell_start[row + x1 + 1];
-            for (uint32_t p = s; p < e; ++p) {
-                const float4 t = sorted[p];
-                const float d = l2_simple(qx, qy, qz, t.x, t.y, t.z);
-                if (d < best[KT - 1]) {
-                    best[KT - 1] = d;
-#pragma unroll
-                    for (int j = KT - 1; j > 0; --j)
-                        if (best[j] < best[j - 1]) { const float t2 = best[j]; best[j] = best[j - 1]; best[j - 1] = t2; }
-                    // Early exit: the final k smallest distances are element-wise <= the current ones, and double sum, float
-                    // rounding and division are monotone, so "current mean < thr" already decides "near".
-                    if (KT <= 4 && best[k - 1 < KT ? k - 1 : KT - 1] != kInf) {
-                        double sum = 0.0;
-#pragma unroll
-                        for (int j = 0; j < KT; ++j) if (j < k) sum = da(sum, (double)best[j]);
-                        if (fabsf(fd(__double2float_rn(sum), (float)k)) < thr) return 0;
-                    }
-                }
-            }
-        }
-    }
-    // Fewer than k neighbours inside the 27 cells: a true k-th neighbour lies farther than the cell size, i.e. beyond
-    // sqrt(k*thr) -> "far" (see file header).  The API rejects targets with fewer than k points up front.
-    // accumulate(..., 0.0) in double (Session.cpp:593), float(sum) / float(k) (Session.cpp:594).
-    double sum = 0.0;
-    bool full = true;
-#pragma unroll
-    for (int j = 0; j < KT; ++j)
-        if (j < k) { if (best[j] == kInf) full = false; else sum = da(sum, (double)best[j]); }
-    if (!full) return 1;
-    const float avg = fd(__double2float_rn(sum), (float)k);
-    return (fabsf(avg) < thr) ? 0 : 1;
+    cell_of(t, qx, qy, qz, &cx, &cy, &cz);
+    auto rows = [&](int y, int z, int x0, int x1, uint32_t* s, uint32_t* e) {
+        const size_t row = ((size_t)z * t.dim[1] + y) * t.dim[0];
+        *s = t.cell_start[row + x0];
+        *e = t.cell_start[row + x1 + 1];
+    };
+    return knn_label_27<KT>(rows, t.sorted, cx, cy, cz, t.dim, qx, qy, qz, k, thr);
 }
 
-// Target with fewer than k points (1 <= n < k <= kMaxK): PCL's nearestKSearch returns all n of them (ascending), the reference still
-// divides their sum by k (Session.cpp:470-471, 592-594).  Brute force over the n points held in shared memory.
-__device__ __forceinline__ uint8_t knn_label_small(const float4* __restrict__ s_t, int n, float qx, float qy, float qz, int k, float thr) {
-    float d[kMaxK];
-#pragma unroll
-    for (int j = 0; j < kMaxK; ++j) d[j] = __int_as_float(0x7f800000);
-    for (int p = 0; p < n; ++p) {
-        float v = l2_simple(qx, qy, qz, s_t[p].x, s_t[p].y, s_t[p].z);
-#pragma unroll
-        for (int j = 0; j < kMaxK; ++j) if (v < d[j]) { const float t = d[j]; d[j] = v; v = t; }   // ascending insertion
-    }
-    double sum = 0.0;
-#pragma unroll
-    for (int j = 0; j < kMaxK; ++j) if (j < n) sum = da(sum, (double)d[j]);
-    return (fabsf(fd(__double2float_rn(sum), (float)k)) < thr) ? 0 : 1;
-}
-
-__device__ __forceinline__ uint8_t knn_label_dispatch(const Grid& g, const uint32_t* __restrict__ cell_start, const float4* __restrict__ sorted,
-                                                      float qx, float qy, float qz, int k, float thr) {
+// the same against any target: a target of fewer than k points (s_t, in shared memory) by brute force
+__device__ __forceinline__ uint8_t knn_label_dispatch(const KnnTarget& t, const float4* s_t, float qx, float qy, float qz, int k, float thr) {
+    if (t.small.n > 0) return knn_label_all<kKnnMaxK>((int)t.small.n, [&](int p) { return s_t[p]; }, qx, qy, qz, k, thr);
     switch (k) {
-        case 1: return knn_label<1>(g, cell_start, sorted, qx, qy, qz, k, thr);
-        case 2: return knn_label<2>(g, cell_start, sorted, qx, qy, qz, k, thr);
-        case 3: return knn_label<3>(g, cell_start, sorted, qx, qy, qz, k, thr);
-        case 4: return knn_label<4>(g, cell_start, sorted, qx, qy, qz, k, thr);
-        default: return knn_label<kMaxK>(g, cell_start, sorted, qx, qy, qz, k, thr);
+        case 1: return knn_label<1>(t, qx, qy, qz, k, thr);
+        case 2: return knn_label<2>(t, qx, qy, qz, k, thr);
+        case 3: return knn_label<3>(t, qx, qy, qz, k, thr);
+        case 4: return knn_label<4>(t, qx, qy, qz, k, thr);
+        default: return knn_label<kKnnMaxK>(t, qx, qy, qz, k, thr);
     }
+}
+
+// a target of fewer than k points (at most kKnnMaxK - 1) into shared memory, for knn_label_dispatch
+__device__ __forceinline__ void load_small_target(const KnnTarget& t, float4* s_t) {
+    if (t.small.n > 0 && threadIdx.x < t.small.n) s_t[threadIdx.x] = make_float4(t.small.x[threadIdx.x], t.small.y[threadIdx.x], t.small.z[threadIdx.x], 0.0f);
+    if (t.small.n > 0) __syncthreads();
 }
 
 // scans: local -> (base2lidar as written at Session.cpp:545) -> pose => global query, then, with T16 != null, the points of an accepted
@@ -144,12 +82,11 @@ __device__ __forceinline__ uint8_t knn_label_dispatch(const Grid& g, const uint3
 // CTAs keeps that allocation: with the bare bound ptxas picks 32 registers and a 44 B spill since the kernel carries the refinement.
 __global__ void __launch_bounds__(128, 12) knn_scan_label_kernel(PtrView scans, const int64_t* __restrict__ off, int K, const double* __restrict__ poses,
                                                              const double* __restrict__ ext, int order, const float* __restrict__ T16,
-                                                             const uint8_t* __restrict__ accept, Grid g, const uint32_t* __restrict__ cell_start,
-                                                             const float4* __restrict__ sorted, int k, float thr, uint8_t* __restrict__ label,
-                                                             float* __restrict__ gx, float* __restrict__ gy, float* __restrict__ gz, PtrView small_target) {
-    __shared__ float4 s_t[kMaxK];
-    if (small_target.n > 0 && threadIdx.x < small_target.n) s_t[threadIdx.x] = make_float4(small_target.x[threadIdx.x], small_target.y[threadIdx.x], small_target.z[threadIdx.x], 0.0f);
-    if (small_target.n > 0) __syncthreads();
+                                                             const uint8_t* __restrict__ accept, KnnTarget t, int k, float thr,
+                                                             uint8_t* __restrict__ label, float* __restrict__ gx, float* __restrict__ gy,
+                                                             float* __restrict__ gz) {
+    __shared__ float4 s_t[kKnnMaxK];
+    load_small_target(t, s_t);
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= scans.n) return;
     const int kf = find_kf(off, K, i);
@@ -161,37 +98,27 @@ __global__ void __launch_bounds__(128, 12) knn_scan_label_kernel(PtrView scans, 
         x = nx; y = ny; z = nz;
     }
     gx[i] = x; gy[i] = y; gz[i] = z;
-    label[i] = small_target.n > 0 ? knn_label_small(s_t, (int)small_target.n, x, y, z, k, thr) : knn_label_dispatch(g, cell_start, sorted, x, y, z, k, thr);
+    label[i] = knn_label_dispatch(t, s_t, x, y, z, k, thr);
 }
 
-// sm_90a: 32 registers and a 44 B spill (L1-resident) at full occupancy.  __launch_bounds__(128, 12) removes the spill (40 registers)
-// but was measured 11 % slower on an H100 (4 M queries against 1 M targets, k = 2: 0.67 vs 0.61 ms), so the bare bound stays.
-__global__ void __launch_bounds__(128) knn_cloud_label_kernel(PtrView q, Grid g, const uint32_t* __restrict__ cell_start,
-                                                              const float4* __restrict__ sorted, int k, float thr, uint8_t* __restrict__ label,
-                                                              PtrView small_target) {
-    __shared__ float4 s_t[kMaxK];
-    if (small_target.n > 0 && threadIdx.x < small_target.n) s_t[threadIdx.x] = make_float4(small_target.x[threadIdx.x], small_target.y[threadIdx.x], small_target.z[threadIdx.x], 0.0f);
-    if (small_target.n > 0) __syncthreads();
+// sm_90a: 32 registers and a 44 B spill (L1-resident) at full occupancy, which the minimum of 16 CTAs per SM keeps (the bare bound gives
+// 40 registers).  __launch_bounds__(128, 12) removes the spill (40 registers) but was measured 11 % slower on an H100 (4 M queries
+// against 1 M targets, k = 2: 0.67 vs 0.61 ms).
+__global__ void __launch_bounds__(128, 16) knn_cloud_label_kernel(PtrView q, KnnTarget t, int k, float thr, uint8_t* __restrict__ label) {
+    __shared__ float4 s_t[kKnnMaxK];
+    load_small_target(t, s_t);
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= q.n) return;
-    label[i] = small_target.n > 0 ? knn_label_small(s_t, (int)small_target.n, q.x[i], q.y[i], q.z[i], k, thr)
-                                  : knn_label_dispatch(g, cell_start, sorted, q.x[i], q.y[i], q.z[i], k, thr);
+    label[i] = knn_label_dispatch(t, s_t, q.x[i], q.y[i], q.z[i], k, thr);
 }
 
-struct GridBuf {
-    Grid g;
-    uint32_t* cell_start = nullptr;  // ncell + 1
-    float4* sorted = nullptr;
-    void* block = nullptr;
-};
-
-static int build_grid(ltr_ctx* ctx, const DevCloud& target, int k, float thr, GridBuf* gb) {
+int knn_target_build(ltr_ctx* ctx, const DevCloud& target, int k, float thr, KnnTarget* t, void** block) {
+    *t = KnnTarget();
+    if (target.n < k) { t->small = view(target); return LTR_OK; }
     float mn[3], mx[3];
-    uint32_t nonfinite = 0;
-    LTR_TRY(minmax_xyz(ctx, target, mn, mx, &nonfinite));
     // an infinite or NaN extent would keep the cell loop below from ever terminating.  Targets of the path are voxelised maps,
     // which the voxeliser has already checked, so nothing reproduces PCL's skipping of invalid points here.
-    if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite target coordinates (%u points)", nonfinite);
+    LTR_TRY(finite_extent(ctx, target, "target", mn, mx));
     const double reach = std::sqrt((double)k * (double)thr) * 1.001 + 1e-6;
     double cell = reach;
     // bound the dense grid to 2^29 cells by growing the cell (exactness only needs cell >= reach)
@@ -201,7 +128,7 @@ static int build_grid(ltr_ctx* ctx, const DevCloud& target, int k, float thr, Gr
         if (cells <= 536870912.0) break;
         cell *= 1.25;
     }
-    Grid g;
+    KnnTarget g;
     g.inv_cell = 1.0 / cell;
     size_t ncell = 1;
     for (int d = 0; d < 3; ++d) {
@@ -210,45 +137,32 @@ static int build_grid(ltr_ctx* ctx, const DevCloud& target, int k, float thr, Gr
         ncell *= (size_t)g.dim[d];
     }
     void* p = nullptr;
-    ScratchGuard g_p(ctx, &p);   // handed to the caller (gb->block) only when the grid is complete
+    ScratchGuard g_p(ctx, &p);   // handed to the caller (*block) only when the grid is complete
     const size_t cs_bytes = (ncell + 1) * sizeof(uint32_t);
     const size_t cs_pad = (cs_bytes + 255) / 256 * 256;
     LTR_TRY(dev_alloc(ctx, &p, 2 * cs_pad + (size_t)target.n * sizeof(float4)));
     uint32_t* cnt = (uint32_t*)p;
     uint32_t* start = (uint32_t*)((char*)p + cs_pad);
     float4* sorted = (float4*)((char*)p + 2 * cs_pad);
+    g.cell_start = start;
+    g.sorted = sorted;
     LTR_CUDA(ctx, cudaMemsetAsync(cnt, 0, cs_pad, ctx->stream));
     const unsigned nb = (unsigned)((target.n + 255) / 256);
     grid_count_kernel<<<nb, 256, 0, ctx->stream>>>(view(target), g, cnt);
     LTR_LAUNCH_CHECK(ctx);
     LTR_TRY(exclusive_scan_u32(ctx, cnt, start, (int64_t)ncell + 1));
     LTR_CUDA(ctx, cudaMemsetAsync(cnt, 0, cs_pad, ctx->stream));
-    grid_fill_kernel<<<nb, 256, 0, ctx->stream>>>(view(target), g, start, cnt, sorted);
+    grid_fill_kernel<<<nb, 256, 0, ctx->stream>>>(view(target), g, cnt, sorted);
     LTR_LAUNCH_CHECK(ctx);
-    gb->g = g; gb->cell_start = start; gb->sorted = sorted; gb->block = p;
-    p = nullptr;   // ownership moves to gb
-    return LTR_OK;
-}
-
-int knn_target_build(ltr_ctx* ctx, const DevCloud& target, int k, float thr, KnnTarget* t, void** block) {
-    *t = KnnTarget();
-    if (target.n < k) { t->small = view(target); return LTR_OK; }
-    GridBuf gb;
-    LTR_TRY(build_grid(ctx, target, k, thr, &gb));
-    for (int d = 0; d < 3; ++d) { t->origin[d] = gb.g.origin[d]; t->dim[d] = gb.g.dim[d]; }
-    t->inv_cell = gb.g.inv_cell;
-    t->cell_start = gb.cell_start;
-    t->sorted = gb.sorted;
-    *block = gb.block;
+    *t = g;
+    *block = p;
+    p = nullptr;   // ownership moves to the caller
     return LTR_OK;
 }
 
 int knn_target_label(ltr_ctx* ctx, const KnnTarget& t, PtrView q, int k, float thr, uint8_t* label) {
     if (q.n == 0) return LTR_OK;
-    Grid g;
-    for (int d = 0; d < 3; ++d) { g.origin[d] = t.origin[d]; g.dim[d] = t.dim[d]; }
-    g.inv_cell = t.inv_cell;
-    knn_cloud_label_kernel<<<(unsigned)((q.n + 127) / 128), 128, 0, ctx->stream>>>(q, g, t.cell_start, t.sorted, k, thr, label, t.small);
+    knn_cloud_label_kernel<<<(unsigned)((q.n + 127) / 128), 128, 0, ctx->stream>>>(q, t, k, thr, label);
     LTR_LAUNCH_CHECK(ctx);
     return LTR_OK;
 }
@@ -261,13 +175,12 @@ int knn_diff(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_
     LTR_TRY(scanset_get(ctx, scans_h, &sp));
     LTR_TRY(poses_get(ctx, poses_h, &pp));
     LTR_TRY(cloud_get(ctx, target_h, &tp));
-    if (k < 1 || k > kMaxK) return fail(ctx, LTR_ERR_UNSUPPORTED, "k = %d outside [1, %d]", k, kMaxK);
+    if (k < 1 || k > kKnnMaxK) return fail(ctx, LTR_ERR_UNSUPPORTED, "k = %d outside [1, %d]", k, kKnnMaxK);
     if (!(thr > 0.0f)) return fail(ctx, LTR_ERR_INVALID, "threshold must be positive");
-    if (pose_offset < 0 || pose_offset + sp->K > pp->K) return fail(ctx, LTR_ERR_INVALID, "pose range [%d,%d) outside [0,%d)", pose_offset, pose_offset + sp->K, pp->K);
+    LTR_TRY(check_pose_range(ctx, *sp, *pp, pose_offset));
     if (tp->n < 1) return fail(ctx, LTR_ERR_UNSUPPORTED, "empty target map (PCL's nearestKSearch asserts on an empty tree)");
     const DevScanSet scans = *sp;
     if (refined && scans.K > 0 && (!T16 || !accepted)) return fail(ctx, LTR_ERR_INVALID, "null transforms or accept mask");
-    const bool small = tp->n < k;   // fewer than k target points: all of them are returned and the sum is still divided by k (Session.cpp:592-594)
     const DevPoses poses = *pp;
     const DevCloud target = *tp;
     const int64_t n = scans.pts.n;
@@ -275,11 +188,10 @@ int knn_diff(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_
     ScanSplit split(ctx, scans, poses.d + (size_t)pose_offset * 24);
     LTR_TRY(split.init());
     if (n > 0) {
-        GridBuf gb;
-        ScratchGuard g_grid(ctx, &gb.block);
-        PtrView small_view{nullptr, nullptr, nullptr, nullptr, 0};
-        if (small) small_view = view(target);
-        else LTR_TRY(build_grid(ctx, target, k, thr, &gb));
+        KnnTarget t;
+        void* t_block = nullptr;
+        ScratchGuard g_grid(ctx, &t_block);
+        LTR_TRY(knn_target_build(ctx, target, k, thr, &t, &t_block));
         void* p = nullptr;
         ScratchGuard g_p(ctx, &p);
         const size_t b_g = ((size_t)n * 12 + 255) / 256 * 256, b_T = T16 ? ((size_t)K * 64 + 255) / 256 * 256 : 0;
@@ -298,8 +210,7 @@ int knn_diff(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_
             LTR_CUDA(ctx, cudaMemcpyAsync(dacc, acc.data(), (size_t)K, cudaMemcpyHostToDevice, ctx->stream));
         }
         knn_scan_label_kernel<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(view(scans.pts), scans.d_off, K, poses.d + (size_t)pose_offset * 24,
-            ctx->ext_identity ? nullptr : ctx->d_ext, ctx->cfg.transform_order, dT, dacc, gb.g, gb.cell_start, gb.sorted, k, thr, split.flags,
-            gx, gy, gz, small_view);
+            ctx->ext_identity ? nullptr : ctx->d_ext, ctx->cfg.transform_order, dT, dacc, t, k, thr, split.flags, gx, gy, gz);
         LTR_LAUNCH_CHECK(ctx);
         g_grid.release();
         // every point goes back; partitioning afterwards keeps the arithmetic identical to the reference, which transforms the two
@@ -328,24 +239,21 @@ int ltr_knn_split_cloud(ltr_ctx* ctx, ltr_cloud query_h, ltr_cloud target_h, int
     DevCloud *qp, *tp;
     LTR_TRY(cloud_get(ctx, query_h, &qp));
     LTR_TRY(cloud_get(ctx, target_h, &tp));
-    if (k < 1 || k > kMaxK) return fail(ctx, LTR_ERR_UNSUPPORTED, "k = %d outside [1, %d]", k, kMaxK);
+    if (k < 1 || k > kKnnMaxK) return fail(ctx, LTR_ERR_UNSUPPORTED, "k = %d outside [1, %d]", k, kKnnMaxK);
     if (!(thr > 0.0f)) return fail(ctx, LTR_ERR_INVALID, "threshold must be positive");
     if (tp->n < 1) return fail(ctx, LTR_ERR_UNSUPPORTED, "empty target (PCL's nearestKSearch asserts on an empty tree)");
-    const bool small = tp->n < k;
     const DevCloud q = *qp, target = *tp;
-    GridBuf gb;
-    ScratchGuard g_grid(ctx, &gb.block);
-    PtrView small_view{nullptr, nullptr, nullptr, nullptr, 0};
-    if (small) small_view = view(target);
-    else if (q.n > 0) LTR_TRY(build_grid(ctx, target, k, thr, &gb));   // before the outputs exist, so that a rejected target leaks nothing
+    KnnTarget t;
+    void* t_block = nullptr;
+    ScratchGuard g_grid(ctx, &t_block);
+    if (q.n > 0) LTR_TRY(knn_target_build(ctx, target, k, thr, &t, &t_block));   // before the outputs exist, so that a rejected target leaks nothing
     LTR_TRY(cloud_new(ctx, q.n, out_near));
     LTR_TRY(cloud_new(ctx, q.n, out_far));
     if (q.n == 0) return LTR_OK;
     void* p = nullptr;
     ScratchGuard g_p(ctx, &p);
     LTR_TRY(dev_alloc(ctx, &p, (size_t)q.n));
-    knn_cloud_label_kernel<<<(unsigned)((q.n + 127) / 128), 128, 0, ctx->stream>>>(view(q), gb.g, gb.cell_start, gb.sorted, k, thr, (uint8_t*)p, small_view);
-    LTR_LAUNCH_CHECK(ctx);
+    LTR_TRY(knn_target_label(ctx, t, view(q), k, thr, (uint8_t*)p));
     g_grid.release();
     DevCloud o0 = ctx->clouds[*out_near], o1 = ctx->clouds[*out_far];
     int64_t nf = 0;

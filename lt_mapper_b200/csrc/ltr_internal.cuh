@@ -221,6 +221,13 @@ int count_flags(ltr_ctx* ctx, const uint8_t* flags, int64_t n, int64_t* count);
 int exclusive_scan_u32(ltr_ctx* ctx, const uint32_t* in, uint32_t* out, int64_t n);  // out[n] elements; returns via out
 // *nonfinite (if non-null): number of points with a non-finite x, y or z (NaN coordinates do not show in mn / mx)
 int minmax_xyz(ltr_ctx* ctx, const DevCloud& c, float mn[3], float mx[3], uint32_t* nonfinite = nullptr);
+// minmax_xyz of a cloud a grid is built over: a point with a non-finite coordinate fails with LTR_ERR_UNSUPPORTED,
+// "non-finite <what> coordinates (<count> points<where>)"
+int finite_extent(ltr_ctx* ctx, const DevCloud& c, const char* what, float mn[3], float mx[3], const char* where = "");
+// pose_offset + [0, scans.K) must be keyframes of poses: LTR_ERR_INVALID otherwise
+int check_pose_range(ltr_ctx* ctx, const DevScanSet& scans, const DevPoses& poses, int32_t pose_offset);
+// out[j] = off[kf0 + j] - off[kf0] for j <= nkf (device offsets of the keyframes [kf0, kf0 + nkf) relative to the first)
+int relative_offsets(ltr_ctx* ctx, const int64_t* off, int kf0, int nkf, int64_t* out);
 // stable LSD radix sort of (keys0, vals0) on the key bits [bit_lo, bit_hi), 8 bits per pass, ping-ponging with (keys1, vals1);
 // *keys_sorted / *vals_sorted point at whichever buffer holds the result.  vals0 == vals1 == nullptr: keys only.
 int radix_sort_pairs(ltr_ctx* ctx, uint64_t* keys0, uint64_t* keys1, uint32_t* vals0, uint32_t* vals1, int64_t n, int bit_lo, int bit_hi,
@@ -273,9 +280,13 @@ int64_t env_points(const char* name, int64_t def, int64_t hi);
 // except that a keyframe is never split (a larger one goes alone); *max_points = the largest launch's points.
 std::vector<int> plan_keyframe_chunks(const std::vector<int64_t>& off, int64_t cap, int max_kf, int64_t* max_points);
 
-// The thresholded kNN decision of ltr_knn_split_cloud (knn.cu) against one target, built once and applied to any number of query views
-// already in the target's frame (scan-side removal, scanside.cu).  knn_target_build: 1 <= k <= 16, thr > 0, target of >= 1 finite points;
-// the caller returns *block to the allocator.  knn_target_label: label[i] = 1 if |avg| >= thr ("far"), else 0.
+constexpr int kKnnMaxK = 16;   // the largest k of every kNN search
+
+// The thresholded kNN decision of the kNN diff and ltr_knn_split_cloud (knn.cu) against one target, built once and applied to any number
+// of query views already in the target's frame (also scan-side removal, scanside.cu): a dense grid (origin, inv_cell, dim; cell_start has
+// one entry per cell plus one, sorted holds the points cell by cell).  knn_target_build: 1 <= k <= kKnnMaxK, thr > 0, target of >= 1
+// points, finite unless it has fewer than k; the caller returns *block to the allocator.  knn_target_label: label[i] = 1 if |avg| >= thr
+// ("far"), else 0.
 struct KnnTarget {
     double origin[3] = {0, 0, 0};
     double inv_cell = 0;

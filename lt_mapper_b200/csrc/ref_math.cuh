@@ -177,4 +177,86 @@ LTR_DEV float l2_simple(float qx, float qy, float qz, float px, float py, float 
     return fa(fa(fm(dx, dx), fm(dy, dy)), fm(dz, dz));
 }
 
+// The KT smallest values pushed so far in ascending order (+inf where fewer were pushed); seen counts the pushes.  Every search pushes the
+// points of one grid, whose point indices are 32-bit, so seen cannot wrap.
+template <int KT>
+struct TopK {
+    float d[KT];
+    uint32_t seen;
+    LTR_DEV void init() {
+#pragma unroll
+        for (int j = 0; j < KT; ++j) d[j] = __int_as_float(0x7f800000);
+        seen = 0;
+    }
+    // true when v entered the list
+    LTR_DEV bool push(float v) {
+        ++seen;
+        if (!(v < d[KT - 1])) return false;
+        d[KT - 1] = v;
+#pragma unroll
+        for (int j = KT - 1; j > 0; --j)
+            if (d[j] < d[j - 1]) { const float t = d[j]; d[j] = d[j - 1]; d[j - 1] = t; }
+        return true;
+    }
+    LTR_DEV bool has(int k) const { return seen >= (uint32_t)k; }
+    // The reference's mean of the k nearest squared distances: accumulate(..., 0.0) in double over the min(seen, k) smallest, ascending,
+    // then float(sum) / float(k) (Session.cpp:470-471, 592-594; Removerter.cpp:1052-1053, 1097-1098).
+    LTR_DEV float mean(int k) const {
+        const int cnt = has(k) ? k : (int)seen;
+        double sum = 0.0;
+#pragma unroll
+        for (int j = 0; j < KT; ++j) if (j < cnt) sum = da(sum, (double)d[j]);
+        return fd(__double2float_rn(sum), (float)k);
+    }
+    // the kNN diff's test |mean| < thr: "near"
+    LTR_DEV bool near(int k, float thr) const { return fabsf(mean(k)) < thr; }
+};
+
+// The thresholded kNN decision, 1 = far and 0 = near, of the query q over the 27 cells around its cell (cx, cy, cz) in a grid of dim
+// cells, KT >= k.  rows(y, z, xa, xb, &s, &e) gives the points pts[s, e) of the cells [xa, xb] of row (y, z).  The caller's cells are wide
+// enough that a true k-th neighbour outside the block already makes the mean >= thr (knn.cu and delta.cu prove it for their grids), so
+// fewer than k points in the block mean "far".
+template <int KT, class Rows>
+LTR_DEV uint8_t knn_label_27(Rows rows, const float4* __restrict__ pts, int cx, int cy, int cz, const int (&dim)[3], float qx, float qy,
+                             float qz, int k, float thr) {
+    TopK<KT> b;
+    b.init();
+    const int x0 = max(cx - 1, 0), x1 = min(cx + 1, dim[0] - 1);
+    if (x0 <= x1) {
+        // rows of 3 x-adjacent cells, the query's own row first: most points have their k neighbours right there and leave through the
+        // early exit below
+        // (dy, dz) + 1 packed 2 bits per step: dy = {0,-1,1,0,0,-1,1,-1,1}, dz = {0,0,0,-1,1,-1,-1,1,1}
+        const unsigned pack_dy = 0x22161U, pack_dz = 0x28215U;
+#pragma unroll 1
+        for (int o = 0; o < 9; ++o) {
+            const int z = cz + (int)((pack_dz >> (2 * o)) & 3u) - 1, y = cy + (int)((pack_dy >> (2 * o)) & 3u) - 1;
+            if (z < 0 || z >= dim[2] || y < 0 || y >= dim[1]) continue;
+            uint32_t s, e;
+            rows(y, z, x0, x1, &s, &e);
+            for (uint32_t p = s; p < e; ++p) {
+                const float4 t = pts[p];
+                // Early exit: the final k smallest distances are element-wise <= the current ones, and the double sum, its float
+                // rounding and the division are monotone, so "current mean < thr" already decides "near".  Short lists check after
+                // each insertion, long ones after each row.
+                if (b.push(l2_simple(qx, qy, qz, t.x, t.y, t.z)) && KT <= 4 && b.has(k) && b.near(k, thr)) return 0;
+            }
+            if (KT > 4 && b.has(k) && b.near(k, thr)) return 0;
+        }
+    }
+    return (b.has(k) && b.near(k, thr)) ? 0 : 1;
+}
+
+// A target of n < k points, pt(p) for p < n: PCL's nearestKSearch returns all n of them (ascending) and the reference still divides
+// their sum by k (Session.cpp:470-471, 592-594).  Brute force.
+template <int KT, class Pt>
+LTR_DEV uint8_t knn_label_all(int n, Pt pt, float qx, float qy, float qz, int k, float thr) {
+    TopK<KT> b;
+    b.init();
+    for (int p = 0; p < n; ++p) {
+        const float4 t = pt(p);
+        b.push(l2_simple(qx, qy, qz, t.x, t.y, t.z));
+    }
+    return b.near(k, thr) ? 0 : 1;
+}
+
 }  // namespace ltr

@@ -35,7 +35,6 @@ namespace ltr {
 
 namespace {
 
-constexpr int kMaxK = 16;
 constexpr int kSegShift = kGridSegShift;
 constexpr int kMaxSegments = kGridMaxSegments;   // 8192 keyframes per launch
 constexpr int kBoundedShells = 2;
@@ -147,28 +146,13 @@ int build_level(ltr_ctx* ctx, PtrView p, const int64_t* d_off, int nseg, const f
 namespace {
 
 // ---- exact k-NN ----------------------------------------------------------------------------------------------------------------------
-// the K smallest computed distances; the shell search's stop rule for them is in sparse_grid.cuh's header
+// the K smallest computed distances with the shell search's stop rule for them (sparse_grid.cuh's header)
 template <int K>
-struct Best {
-    float d[K];
-    long long seen;
-    __device__ __forceinline__ void init() {
-#pragma unroll
-        for (int j = 0; j < K; ++j) d[j] = __int_as_float(0x7f800000);
-        seen = 0;
-    }
-    __device__ __forceinline__ void push(float v, const float4&) {
-        ++seen;
-        if (v < d[K - 1]) {
-            d[K - 1] = v;
-#pragma unroll
-            for (int j = K - 1; j > 0; --j)
-                if (d[j] < d[j - 1]) { const float t = d[j]; d[j] = d[j - 1]; d[j - 1] = t; }
-        }
-    }
+struct Best : TopK<K> {
+    __device__ __forceinline__ void push(float v, const float4&) { TopK<K>::push(v); }
     __device__ __forceinline__ bool settled(long long s, double cell) const {
-        if (seen < K) return false;
-        const double dk = (double)d[K - 1], b = shell_bound(s, cell);
+        if (!this->has(K)) return false;
+        const double dk = (double)this->d[K - 1], b = shell_bound(s, cell);
         return dk == 0.0 || (s > 0 && dk <= b);
     }
 };
@@ -180,12 +164,7 @@ __device__ bool knn_exact_avg(const Level& L, int seg, float qx, float qy, float
     Best<K> b;
     b.init();
     if (!shell_search(L, seg, qx, qy, qz, max_shell, b)) return false;
-    // accumulate(..., 0.0) in double, ascending (Removerter.cpp:1052, 1097); float(sum) / float(k) (:1053, 1098)
-    const int cnt = b.seen < K ? (int)b.seen : K;
-    double sum = 0.0;
-#pragma unroll
-    for (int j = 0; j < K; ++j) if (j < cnt) sum = da(sum, (double)b.d[j]);
-    *avg = fd(__double2float_rn(sum), (float)K);
+    *avg = b.mean(K);
     return true;
 }
 
@@ -214,7 +193,7 @@ int launch_exact_knn(ltr_ctx* ctx, int k, const Level& L, PtrView q, const int64
         LTR_SCANSIDE_CASE(7) LTR_SCANSIDE_CASE(8) LTR_SCANSIDE_CASE(9) LTR_SCANSIDE_CASE(10) LTR_SCANSIDE_CASE(11) LTR_SCANSIDE_CASE(12)
         LTR_SCANSIDE_CASE(13) LTR_SCANSIDE_CASE(14) LTR_SCANSIDE_CASE(15) LTR_SCANSIDE_CASE(16)
 #undef LTR_SCANSIDE_CASE
-        default: return fail(ctx, LTR_ERR_UNSUPPORTED, "k = %d outside [1, %d]", k, kMaxK);
+        default: return fail(ctx, LTR_ERR_UNSUPPORTED, "k = %d outside [1, %d]", k, kKnnMaxK);
     }
     LTR_LAUNCH_CHECK(ctx);
     return LTR_OK;
@@ -252,11 +231,6 @@ __global__ void __launch_bounds__(256) scanside_diff_kernel(const float* __restr
     flag[t] = (fabsf(fs(avg_scan[t], avg_map[t])) < thr) ? 0 : 1;
 }
 
-__global__ void __launch_bounds__(256) chunk_offsets_kernel(const int64_t* __restrict__ off, int kf0, int nkf, int64_t* __restrict__ out) {
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j <= nkf) out[j] = off[kf0 + j] - off[kf0];
-}
-
 }  // namespace
 }  // namespace ltr
 
@@ -275,21 +249,17 @@ int ltr_scanside_split(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int
     LTR_TRY(poses_get(ctx, poses_h, &pp));
     LTR_TRY(cloud_get(ctx, map_h, &mp));
     if (criterion != LTR_SCANSIDE_MAP && criterion != LTR_SCANSIDE_SCAN_MINUS_MAP) return fail(ctx, LTR_ERR_INVALID, "unknown criterion %d", criterion);
-    if (k < 1 || k > kMaxK) return fail(ctx, LTR_ERR_UNSUPPORTED, "k = %d outside [1, %d]", k, kMaxK);
+    if (k < 1 || k > kKnnMaxK) return fail(ctx, LTR_ERR_UNSUPPORTED, "k = %d outside [1, %d]", k, kKnnMaxK);
     if (!(thr > 0.0f)) return fail(ctx, LTR_ERR_INVALID, "threshold must be positive");
-    if (pose_offset < 0 || pose_offset + sp->K > pp->K) return fail(ctx, LTR_ERR_INVALID, "pose range [%d,%d) outside [0,%d)", pose_offset, pose_offset + sp->K, pp->K);
+    LTR_TRY(check_pose_range(ctx, *sp, *pp, pose_offset));
     if (mp->n < 1) return fail(ctx, LTR_ERR_UNSUPPORTED, "empty map (PCL's nearestKSearch asserts on an empty tree)");
     const DevScanSet scans = *sp;
     const DevPoses poses = *pp;
     const DevCloud map = *mp;
     for (int j = 0; j < 4; ++j) ctx->scanside_stats[j] = 0;
     ctx->scanside_stats[0] = scans.pts.n;
-    {
-        float mn[3], mx[3];
-        uint32_t nonfinite = 0;
-        LTR_TRY(minmax_xyz(ctx, map, mn, mx, &nonfinite));
-        if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite map coordinates (%u points)", nonfinite);
-    }
+    float map_mn[3], map_mx[3];
+    LTR_TRY(finite_extent(ctx, map, "map", map_mn, map_mx));
     const int64_t n = scans.pts.n;
     const double* pose0 = poses.d + (size_t)pose_offset * 24;
     ScanSplit split(ctx, scans, pose0);
@@ -318,11 +288,7 @@ int ltr_scanside_split(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int
         ScratchGuard g_kt(ctx, &kt_block);
         Pyramid mapT(ctx);
         if (criterion == LTR_SCANSIDE_MAP) LTR_TRY(knn_target_build(ctx, map, k, thr, &kt, &kt_block));
-        else {
-            float mn[3], mx[3];
-            LTR_TRY(minmax_xyz(ctx, map, mn, mx));
-            mapT.init(view(map), nullptr, 1, mn, mx);
-        }
+        else mapT.init(view(map), nullptr, 1, map_mn, map_mx);
         for (size_t c = 0; c + 1 < kf_cut.size(); ++c) {
             const int kf0 = kf_cut[c], kf1 = kf_cut[c + 1], nkf = kf1 - kf0;
             const int64_t base = scans.h_off[kf0], m = scans.h_off[kf1] - base;
@@ -332,17 +298,16 @@ int ltr_scanside_split(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int
             LTR_TRY(scans_to_global(ctx, scans, base, m, pose0, ctx->ext_identity ? nullptr : ctx->d_ext + 12, g.x(), g.y(), g.z(), nullptr));
             g.n = m;
             float mn[3], mx[3];
-            uint32_t nonfinite = 0;
-            LTR_TRY(minmax_xyz(ctx, g, mn, mx, &nonfinite));
-            if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite scan coordinates (%u points in keyframes [%d,%d))", nonfinite, kf0, kf1);
+            char where[48];
+            snprintf(where, sizeof(where), " in keyframes [%d,%d)", kf0, kf1);
+            LTR_TRY(finite_extent(ctx, g, "scan", mn, mx, where));
             const PtrView q = view(g);
             uint8_t* fl = split.flags + base;
             if (criterion == LTR_SCANSIDE_MAP) {
                 // |avg_map| < thr -> static (Removerter.cpp:1056)
                 LTR_TRY(knn_target_label(ctx, kt, q, k, thr, fl));
             } else {
-                chunk_offsets_kernel<<<(nkf + 1 + 255) / 256, 256, 0, ctx->stream>>>(scans.d_off, kf0, nkf, c_off);
-                LTR_LAUNCH_CHECK(ctx);
+                LTR_TRY(relative_offsets(ctx, scans.d_off, kf0, nkf, c_off));
                 int64_t un = 0;
                 LTR_TRY(exact_avg_all(ctx, mapT, k, q, nullptr, 1, avg_map, list_a, list_b, d_cnt, &un));
                 ctx->scanside_stats[1] += un;
@@ -378,23 +343,18 @@ int ltr_debug_exact_knn_avg(ltr_ctx* ctx, ltr_scanset query_h, ltr_cloud target_
     LTR_TRY(scanset_get(ctx, query_h, &sp));
     DevCloud* tp = nullptr;
     if (!self) LTR_TRY(cloud_get(ctx, target_h, &tp));
-    if (k < 1 || k > kMaxK) return fail(ctx, LTR_ERR_UNSUPPORTED, "k = %d outside [1, %d]", k, kMaxK);
+    if (k < 1 || k > kKnnMaxK) return fail(ctx, LTR_ERR_UNSUPPORTED, "k = %d outside [1, %d]", k, kKnnMaxK);
     if (self && sp->K > kMaxSegments) return fail(ctx, LTR_ERR_UNSUPPORTED, "%d keyframes in one launch (at most %d)", sp->K, kMaxSegments);
     if (!self && tp->n < 1) return fail(ctx, LTR_ERR_UNSUPPORTED, "empty target");
     const DevScanSet q = *sp;
     const int64_t n = q.pts.n;
     if (n >= ((int64_t)1 << 32)) return fail(ctx, LTR_ERR_UNSUPPORTED, "%lld query points", (long long)n);
     float qmn[3], qmx[3];
-    uint32_t nonfinite = 0;
-    if (n > 0) {
-        LTR_TRY(minmax_xyz(ctx, q.pts, qmn, qmx, &nonfinite));
-        if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite query coordinates (%u points)", nonfinite);
-    }
+    if (n > 0) LTR_TRY(finite_extent(ctx, q.pts, "query", qmn, qmx));
     Pyramid T(ctx);
     if (!self) {
         float mn[3], mx[3];
-        LTR_TRY(minmax_xyz(ctx, *tp, mn, mx, &nonfinite));
-        if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite target coordinates (%u points)", nonfinite);
+        LTR_TRY(finite_extent(ctx, *tp, "target", mn, mx));
         T.init(view(*tp), nullptr, 1, mn, mx);
     }
     int64_t un = 0;

@@ -14,7 +14,7 @@
 // rounding is monotone, so |dx| = |fl(q_a - p_a)| >= fl((s - 2^-6) c) >= (s - 2^-6) c (1 - u), u = 2^-24, fl(dx*dx) >= dx^2 (1 - u), and the
 // two additions of non-negative terms round to no less than fl(dx*dx).  The computed distance of every point outside the block is
 // therefore >= ((s - 2^-6) c)^2 (1 - u)^3 > B(s): STRICTLY greater than B(s).
-//  * k smallest values (scanside.cu, Best<K>): once the k-th smallest computed distance D_k <= B(s), no point outside the block can
+//  * k smallest values (scanside.cu, Best<K> over ref_math.cuh's TopK): once the k-th smallest computed distance D_k <= B(s), no point outside the block can
 //    displace a value of the k smallest (a tie at D_k leaves the multiset unchanged), so the double sum in ascending order, its float
 //    rounding and the division by float(k) are final.  D_k = 0 cannot be undercut by any distance, so it settles in any shell, shell 0
 //    included.  How many values enter the sum is min(k, points evaluated), never "finite ones": an overflowed +inf distance is summed as
@@ -72,6 +72,18 @@ __device__ __forceinline__ long long cell_index(double v, double origin, double 
 __device__ __forceinline__ double shell_bound(long long s, double cell) {
     const double r = ((double)s - 0x1p-6) * cell;
     return r * r * (1.0 - 0x1p-20);
+}
+
+// the points L.pts[*s, *e) of the cells [xa, xb] of row (y, z) of segment seg (cells [c0, c1) of the level), in key order
+__device__ __forceinline__ void row_points(const Level& L, uint32_t c0, uint32_t c1, int seg, long long xa, long long xb, long long y, long long z,
+                                           uint32_t* s, uint32_t* e) {
+    const unsigned long long ka = cell_key(seg, xa, y, z), kb = cell_key(seg, xb, y, z);
+    uint32_t lo = c0, hi = c1;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (L.keys[mid] < ka) lo = mid + 1; else hi = mid; }
+    uint32_t ci = lo;
+    while (ci < c1 && L.keys[ci] <= kb) ++ci;
+    *s = L.start[lo];
+    *e = L.start[ci];
 }
 
 // the cells [xa, xb] of row (y, z) of segment seg (cells [c0, c1) of the level): acc.push(distance, point) in key order

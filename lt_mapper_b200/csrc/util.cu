@@ -398,6 +398,30 @@ static int minmax_view(ltr_ctx* ctx, const PtrView& v, float mn[3], float mx[3],
 
 int minmax_xyz(ltr_ctx* ctx, const DevCloud& c, float mn[3], float mx[3], uint32_t* nonfinite) { return minmax_view(ctx, view(c), mn, mx, nonfinite); }
 
+int finite_extent(ltr_ctx* ctx, const DevCloud& c, const char* what, float mn[3], float mx[3], const char* where) {
+    uint32_t nonfinite = 0;
+    LTR_TRY(minmax_xyz(ctx, c, mn, mx, &nonfinite));
+    if (nonfinite) return fail(ctx, LTR_ERR_UNSUPPORTED, "non-finite %s coordinates (%u points%s)", what, nonfinite, where);
+    return LTR_OK;
+}
+
+int check_pose_range(ltr_ctx* ctx, const DevScanSet& scans, const DevPoses& poses, int32_t pose_offset) {
+    if (pose_offset < 0 || pose_offset + scans.K > poses.K)
+        return fail(ctx, LTR_ERR_INVALID, "pose range [%d,%d) outside [0,%d)", pose_offset, pose_offset + scans.K, poses.K);
+    return LTR_OK;
+}
+
+__global__ void __launch_bounds__(256) relative_offsets_kernel(const int64_t* __restrict__ off, int kf0, int nkf, int64_t* __restrict__ out) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j <= nkf) out[j] = off[kf0 + j] - off[kf0];
+}
+
+int relative_offsets(ltr_ctx* ctx, const int64_t* off, int kf0, int nkf, int64_t* out) {
+    relative_offsets_kernel<<<(nkf + 1 + 255) / 256, 256, 0, ctx->stream>>>(off, kf0, nkf, out);
+    LTR_LAUNCH_CHECK(ctx);
+    return LTR_OK;
+}
+
 // ------------------------------------------------------------------------------------------------
 // Voxel centroid == pcl::octree::OctreePointCloudVoxelCentroid as used by octreeDownsampling
 // (ltremovert/src/utility.cpp:204-219).  PCL semantics (published PCL 1.10 sources, see DESIGN.md):
