@@ -330,33 +330,27 @@ class Context:
         self._ck(lib().ltr_voxel_grid_per_keyframe(self._h, scans, leaf, ctypes.byref(h), ctypes.byref(ov)))
         return h.value, ov.value
 
-    def remove_pass(self, map_, scans, poses, mode, res_alpha, diff_thres=0.1, kf_begin=0, kf_end=None, accumulate=False):
+    def _remove_pass(self, fn, map_, scans, poses, kf_begin, kf_end, mode, res_alpha, thresholds, accumulate):
+        """One ltr_remove_pass* call over [kf_begin, kf_end) (kf_end None: every keyframe of `scans`); returns the flagged count."""
         if kf_end is None:
             kf_end = self.scanset_info(scans)[0]
         n = ctypes.c_int64()
-        self._ck(lib().ltr_remove_pass(self._h, map_, scans, poses, kf_begin, kf_end, mode, res_alpha, diff_thres,
-                                       1 if accumulate else 0, ctypes.byref(n)))
+        self._ck(fn(self._h, map_, scans, poses, kf_begin, kf_end, mode, res_alpha, *thresholds, 1 if accumulate else 0, ctypes.byref(n)))
         return n.value
+
+    def remove_pass(self, map_, scans, poses, mode, res_alpha, diff_thres=0.1, kf_begin=0, kf_end=None, accumulate=False):
+        return self._remove_pass(lib().ltr_remove_pass, map_, scans, poses, kf_begin, kf_end, mode, res_alpha, (diff_thres,), accumulate)
 
     def remove_pass_adaptive(self, map_, scans, poses, mode, res_alpha, coeff=0.05, kf_begin=0, kf_end=None, accumulate=False):
         """remove_pass with the range-adaptive threshold fl(coeff * scan range) per pixel (ltr_remove_pass_adaptive; 0 < coeff < 1)."""
-        if kf_end is None:
-            kf_end = self.scanset_info(scans)[0]
-        n = ctypes.c_int64()
-        self._ck(lib().ltr_remove_pass_adaptive(self._h, map_, scans, poses, kf_begin, kf_end, mode, res_alpha, coeff,
-                                                1 if accumulate else 0, ctypes.byref(n)))
-        return n.value
+        return self._remove_pass(lib().ltr_remove_pass_adaptive, map_, scans, poses, kf_begin, kf_end, mode, res_alpha, (coeff,), accumulate)
 
     def remove_pass_ball(self, map_, scans, poses, mode, res_alpha, radius, diff_thres=0.1, adaptive_coeff=0.0, kf_begin=0, kf_end=None,
                          accumulate=False):
         """remove_pass in which each keyframe sees only the map points within `radius` of its pose's translation (ltr_remove_pass_ball);
         adaptive_coeff != 0 takes the range-adaptive threshold instead of diff_thres."""
-        if kf_end is None:
-            kf_end = self.scanset_info(scans)[0]
-        n = ctypes.c_int64()
-        self._ck(lib().ltr_remove_pass_ball(self._h, map_, scans, poses, kf_begin, kf_end, mode, res_alpha, diff_thres, adaptive_coeff, radius,
-                                            1 if accumulate else 0, ctypes.byref(n)))
-        return n.value
+        return self._remove_pass(lib().ltr_remove_pass_ball, map_, scans, poses, kf_begin, kf_end, mode, res_alpha,
+                                 (diff_thres, adaptive_coeff, radius), accumulate)
 
     def scan_images_release(self, free_storage=True):
         """Drops the scan-side images remove_pass keeps between passes; free_storage also frees their storage (ltr_scan_images_release)."""

@@ -296,11 +296,23 @@ __global__ void __launch_bounds__(256) atan_sweep_kernel(int which, uint32_t las
     if (wb > old) *arg_bits = worst_arg;   // racy between equal-ish maxima; the argument is informational only
 }
 
+// the 128-point tiles of a map of n points: the work units of map_project_fast_kernel's warps, and what culling, the ball and the
+// near-to-far claim order bound with a sphere
+static inline long long tile_count(int64_t n) { return (n + kTilePts - 1) / kTilePts; }
+
+// the bounding spheres of the map's tiles (float4 per tile) into a new scratch block *spheres; a pass computes them once for all readers
+static int tile_spheres(ltr_ctx* ctx, const DevCloud& map, void** spheres) {
+    const long long ntiles = tile_count(map.n);
+    LTR_TRY(dev_alloc(ctx, spheres, (size_t)ntiles * sizeof(float4)));
+    tile_sphere_kernel<<<(unsigned)((ntiles * 32 + 255) / 256), 256, 0, ctx->stream>>>(view(map), (float4*)*spheres, ntiles);
+    LTR_LAUNCH_CHECK(ctx);
+    return LTR_OK;
+}
+
 // persistent grid: up to 4 resident CTAs per SM (20 KB shared memory each; the 3-CTA variants leave the rest queued: the warps claim tiles
 // from a counter, so a late CTA only finds less work), never more CTAs than tiles need
 static inline unsigned fast_grid(const ltr_ctx* ctx, int64_t n) {
-    const int64_t tiles = (n + 32 * kFastPts - 1) / (32 * kFastPts);
-    const int64_t ctas = (tiles + kFastThreads / 32 - 1) / (kFastThreads / 32);
+    const int64_t ctas = (tile_count(n) + kFastThreads / 32 - 1) / (kFastThreads / 32);
     return (unsigned)std::max<int64_t>(1, std::min<int64_t>(ctas, (int64_t)ctx->sm_count * kFastCtasPerSmPad));
 }
 
@@ -367,9 +379,15 @@ static void pass_end(ltr_ctx* ctx, const PassPlan& p, int slot, double bytes_per
     ctx->stats[4] = (double)ms * 1000.0;
 }
 
-// FastCfg::el_direct as the kElDirect template argument: f(std::true_type{}) or f(std::false_type{})
+// Runtime bools as template arguments: with_bools(f, a, b) returns f(std::bool_constant<a>{}, std::bool_constant<b>{}).  f is
+// instantiated for every combination, so it must name only the kernels it may be asked for.
 template <class F>
-static auto with_el_direct(const FastCfg& fc, F f) { return fc.el_direct ? f(std::true_type{}) : f(std::false_type{}); }
+static auto with_bools(F f) { return f(); }
+template <class F, class... Rest>
+static auto with_bools(F f, bool b, Rest... rest) {
+    const auto bind = [&](auto c) { return with_bools([&](auto... cs) { return f(c, cs...); }, rest...); };
+    return b ? bind(std::true_type{}) : bind(std::false_type{});
+}
 
 // what one launch of the map projection computes in the winner image
 enum class Proj {
@@ -378,29 +396,28 @@ enum class Proj {
     kTrueMinDeferred,   // the same through the deferred mode of project_fast.cuh (fast path only): the fast kernel, then deferred_resolve_kernel
 };
 
-using FastKernel = decltype(&map_project_fast_kernel<true, true, false, true>);
-
 // One launch of the map projection over the keyframes [k0, k0 + nb) of `poses` into `win`, timed by an event pair.  rimg: the launch's scan
 // range images (scan-minus-map; unused by the true minimum), test_img: the test image of the scan-minus-map fast path.  amin (fast path,
 // may be null in the deferred mode): the approximate running minimum, reset here.  da: the deferred mode's scratch.  adaptive (scan-minus-map
-// only): `thres` is the coefficient c of the pixel threshold fl(c s), and test_img was built for it.  ball (nullptr or args.centre nullptr:
-// the full map): keyframe k sees only the points of its ball (args.centre[k], args.r2); on the fast path through the tile list of the
+// only): `thres` is the coefficient c of the pixel threshold fl(c s), and test_img was built for it.  ball (args.centre nullptr: the full
+// map): keyframe k sees only the points of its ball (args.centre[k], args.r2); on the fast path through the tile list of the
 // launch, which ball_tile_list_kernel builds here from the tile spheres and non-finite flags into `scratch` (3 ntiles words: out masks,
 // in masks, list).
 struct BallLaunch {
-    BallArgs args;                     // centre and r2 set by the caller; the rest is filled here
+    BallArgs args{};                   // centre and r2 set by ball_setup, centre moved to each launch's keyframes; the rest by project_map
     const float4* tiles = nullptr;
     const uint8_t* nonfinite = nullptr;
     long long ntiles = 0;
     uint32_t* scratch = nullptr;
+    std::vector<float4> h_centre;      // host copy of the centres: outlives their upload, the pass synchronises before it returns
 };
 
 static int project_map(ltr_ctx* ctx, PassPlan& p, const DevCloud& map, const DevPoses& poses, int k0, int nb, Proj mode, const uint32_t* rimg,
                        const uint32_t* test_img, float thres, bool adaptive, uint64_t* win, uint32_t* amin, const CullArgs& ca, const DeferredArgs& da,
-                       const BallLaunch* ball = nullptr) {
+                       const BallLaunch& ball = BallLaunch{}) {
     const bool cand = mode == Proj::kScanMinusMap;
     adaptive = adaptive && cand;
-    const bool use_ball = ball && ball->args.centre;
+    const bool use_ball = ball.args.centre != nullptr;
     if (amin) {
         fill_u32_kernel<<<grid_for(nb * p.npx, 256, ctx->sm_count * 8), 256, 0, ctx->stream>>>(amin, 0x7f800000u, nb * p.npx);
         LTR_LAUNCH_CHECK(ctx);
@@ -408,11 +425,11 @@ static int project_map(ltr_ctx* ctx, PassPlan& p, const DevCloud& map, const Dev
     prof_begin(ctx);
     p.units.push_back(nb);
     if (!p.use_fast) {
-        const auto kern = use_ball ? (adaptive ? map_project_kernel<true, true, true> : cand ? map_project_kernel<true, false, true> : map_project_kernel<false, false, true>)
-                        : adaptive ? map_project_kernel<true, true> : cand ? map_project_kernel<true> : map_project_kernel<false>;
+        const auto kern = with_bools([cand](auto ad, auto in_ball) {
+            return cand ? map_project_kernel<true, ad, in_ball> : map_project_kernel<false, false, in_ball>;
+        }, adaptive, use_ball);
         kern<<<(unsigned)((map.n + 255) / 256), 256, (size_t)nb * 12 * sizeof(double), ctx->stream>>>(view(map), poses.d, k0, nb, ctx->d_ext,
-            ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, p.g, rimg, thres, win, use_ball ? ball->args.centre : nullptr,
-            use_ball ? ball->args.r2 : 0.0f);
+            ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, p.g, rimg, thres, win, ball.args.centre, ball.args.r2);
     } else {
         unsigned int* work = (unsigned int*)(ctx->d_counters + 4);
         LTR_CUDA(ctx, cudaMemsetAsync(work, 0, sizeof(unsigned int), ctx->stream));
@@ -423,31 +440,23 @@ static int project_map(ltr_ctx* ctx, PassPlan& p, const DevCloud& map, const Dev
         }
         BallArgs ba{};
         if (use_ball) {   // the launch's tile list; its count lives in counters[5], never read by the host
-            ba = ball->args;
-            uint32_t* s = ball->scratch;
+            ba = ball.args;
+            uint32_t* s = ball.scratch;
             unsigned int* count = (unsigned int*)(ctx->d_counters + 5);
-            ba.out_mask = s; ba.in_mask = s + ball->ntiles; ba.list = s + 2 * ball->ntiles; ba.count = count;
+            ba.out_mask = s; ba.in_mask = s + ball.ntiles; ba.list = s + 2 * ball.ntiles; ba.count = count;
             LTR_CUDA(ctx, cudaMemsetAsync(count, 0, sizeof(unsigned int), ctx->stream));
-            ball_tile_list_kernel<<<(unsigned)((ball->ntiles * 32 + 255) / 256), 256, 0, ctx->stream>>>(ball->tiles, ball->nonfinite, ball->ntiles, ba, nb,
-                s, s + ball->ntiles, s + 2 * ball->ntiles, count, ctx->d_counters);
+            ball_tile_list_kernel<<<(unsigned)((ball.ntiles * 32 + 255) / 256), 256, 0, ctx->stream>>>(ball.tiles, ball.nonfinite, ball.ntiles, ba, nb,
+                s, s + ball.ntiles, s + 2 * ball.ntiles, count, ctx->d_counters);
             LTR_LAUNCH_CHECK(ctx);
         }
-        // template arguments <candidates only, short elevation path, deferred, guard-padded test image, adaptive threshold, ball subset>
-        const FastKernel kern = use_ball
-            ? ((cand && p.fc.pad_ok) ? (adaptive ? map_project_fast_kernel<true, true, false, true, true, true> : map_project_fast_kernel<true, true, false, true, false, true>)
-               : with_el_direct(p.fc, [mode, adaptive](auto el) -> FastKernel {
-                     constexpr bool kEl = decltype(el)::value;
-                     return mode == Proj::kScanMinusMap ? (adaptive ? map_project_fast_kernel<true, kEl, false, false, true, true> : map_project_fast_kernel<true, kEl, false, false, false, true>)
-                          : mode == Proj::kTrueMin      ? map_project_fast_kernel<false, kEl, false, false, false, true>
-                                                        : map_project_fast_kernel<false, kEl, true, false, false, true>;
-                 }))
-            : (cand && p.fc.pad_ok) ? (adaptive ? map_project_fast_kernel<true, true, false, true, true> : map_project_fast_kernel<true, true, false, true>)
-            : with_el_direct(p.fc, [mode, adaptive](auto el) -> FastKernel {
-                  constexpr bool kEl = decltype(el)::value;
-                  return mode == Proj::kScanMinusMap ? (adaptive ? map_project_fast_kernel<true, kEl, false, false, true> : map_project_fast_kernel<true, kEl, false>)
-                       : mode == Proj::kTrueMin      ? map_project_fast_kernel<false, kEl, false>
-                                                     : map_project_fast_kernel<false, kEl, true>;
-              });
+        // template arguments <candidates only, short elevation path, deferred, guard-padded test image, adaptive threshold, ball subset>;
+        // the padded test image implies the short elevation path (FastCfg::pad_ok)
+        const auto kern = with_bools([mode, pad = cand && p.fc.pad_ok](auto el, auto ad, auto in_ball) {
+            return pad                         ? map_project_fast_kernel<true, true, false, true, ad, in_ball>
+                 : mode == Proj::kScanMinusMap ? map_project_fast_kernel<true, el, false, false, ad, in_ball>
+                 : mode == Proj::kTrueMin      ? map_project_fast_kernel<false, el, false, false, false, in_ball>
+                                               : map_project_fast_kernel<false, el, true, false, false, in_ball>;
+        }, p.fc.el_direct != 0, adaptive, use_ball);
         kern<<<fast_grid(ctx, map.n), kFastThreads, fast_smem_bytes(), ctx->stream>>>(view(map), make_kf_batch(poses, k0, nb), poses.d, k0, nb, ctx->d_ext,
             ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, p.g, p.fc, rimg, cand ? test_img : amin, thres, win, amin, ca, ctx->d_counters, work, da, ba);
         if (deferred) {
@@ -461,6 +470,38 @@ static int project_map(ltr_ctx* ctx, PassPlan& p, const DevCloud& map, const Dev
     return LTR_OK;
 }
 
+// Fills `bl` with the balls of radius `radius` around the keyframes [kf_begin, kf_end): their f32 centres and, on the fast path, the pass's
+// tile spheres, a non-finite flag per tile and the launches' tile-list scratch.  Centres, flags and scratch share one new scratch block
+// *block.  PCL's radiusSearch hands FLANN radius^2 as a float; an r2 that rounds to 0 admits no point.
+static int ball_setup(ltr_ctx* ctx, const PassPlan& p, const DevCloud& map, const DevPoses& poses, int kf_begin, int kf_end, float radius,
+                      const float4* spheres, void** block, BallLaunch* bl) {
+    const int K = kf_end - kf_begin;
+    const long long ntiles = tile_count(map.n);
+    bl->h_centre.resize((size_t)K);
+    for (int k = 0; k < K; ++k) {   // the pose's translation column (pose rows at 12..23 of DevPoses::h), rounded to f32
+        const double* T = &poses.h[(size_t)(kf_begin + k) * 24 + 12];
+        bl->h_centre[(size_t)k] = make_float4((float)T[3], (float)T[7], (float)T[11], 0.0f);
+    }
+    const size_t c_bytes = ((size_t)K * sizeof(float4) + 255) / 256 * 256;
+    const size_t w_bytes = p.use_fast ? ((size_t)ntiles * 3 * sizeof(uint32_t) + 255) / 256 * 256 : 0;
+    LTR_TRY(dev_alloc(ctx, block, c_bytes + w_bytes + (p.use_fast ? (size_t)ntiles : 0)));
+    char* b = (char*)*block;
+    LTR_CUDA(ctx, cudaMemcpyAsync(b, bl->h_centre.data(), (size_t)K * sizeof(float4), cudaMemcpyHostToDevice, ctx->stream));
+    bl->args.centre = (const float4*)b;
+    bl->args.r2 = (float)((double)radius * (double)radius);
+    if (p.use_fast) {
+        uint8_t* nonfinite = (uint8_t*)(b + c_bytes + w_bytes);
+        LTR_CUDA(ctx, cudaMemsetAsync(nonfinite, 0, (size_t)ntiles, ctx->stream));
+        tile_nonfinite_kernel<<<(unsigned)((map.n + 255) / 256), 256, 0, ctx->stream>>>(view(map), nonfinite);
+        LTR_LAUNCH_CHECK(ctx);
+        bl->tiles = spheres;
+        bl->nonfinite = nonfinite;
+        bl->ntiles = ntiles;
+        bl->scratch = (uint32_t*)(b + c_bytes);
+    }
+    return LTR_OK;
+}
+
 // scan2RangeImg of the keyframes [kf0, kf0 + n) of `scans` into n images at rimg, through the fast pixel evaluation on the fast path
 static int scan_rimg(ltr_ctx* ctx, const PassPlan& p, const DevScanSet& scans, int kf0, int n, uint32_t* rimg) {
     fill_u32_kernel<<<grid_for(n * p.npx, 256, ctx->sm_count * 8), 256, 0, ctx->stream>>>(rimg, kNoPointBits, n * p.npx);
@@ -469,7 +510,7 @@ static int scan_rimg(ltr_ctx* ctx, const PassPlan& p, const DevScanSet& scans, i
     if (npts == 0) return LTR_OK;
     const unsigned blocks = (unsigned)((npts + 255) / 256);
     if (p.use_fast) {
-        const auto kern = with_el_direct(p.fc, [](auto el) { return scan_rimg_fast_kernel<decltype(el)::value>; });
+        const auto kern = with_bools([](auto el) { return scan_rimg_fast_kernel<el>; }, p.fc.el_direct != 0);
         kern<<<blocks, 256, 0, ctx->stream>>>(view(scans.pts), scans.d_off, kf0, n, p.g, p.fc, rimg);
     } else {
         scan_rimg_kernel<<<blocks, 256, 0, ctx->stream>>>(view(scans.pts), scans.d_off, kf0, n, p.g, rimg);
@@ -537,7 +578,7 @@ static int build_scan_images(ltr_ctx* ctx, const PassPlan& p, const DevScanSet& 
             LTR_LAUNCH_CHECK(ctx);
         }
         if (timg) {
-            const auto kern = coeff != 0.0f ? scan_test_image_kernel<true> : scan_test_image_kernel<false>;
+            const auto kern = with_bools([](auto ad) { return scan_test_image_kernel<ad>; }, coeff != 0.0f);
             kern<<<grid_for(n * timg_px, 256, fill_blocks), 256, 0, ctx->stream>>>(ri, timg + (size_t)c0 * timg_px, n, g.rows, g.cols, pad ? p.fc.pad_g : 0,
                                                                                   pad ? 1 : 0, shortcut, coeff);
             LTR_LAUNCH_CHECK(ctx);
@@ -682,15 +723,11 @@ int ltr_scan_images_release(ltr_ctx* ctx, int32_t free_storage) {
     return LTR_OK;
 }
 
-// adaptive_c != 0: the pixel threshold is fl(adaptive_c s) (ltr_remove_pass_adaptive) and diff_thres is not used.
-// ball_r2 != 0: keyframe k sees only the map points within the ball of squared radius ball_r2 around its pose's f32 translation
-// (ltr_remove_pass_ball; a negative value: no point is in any ball).
+// One run of remove_pass; allow_deferred: the true minimum may take the deferred mode.
 static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end,
-                            int32_t mode, float res_alpha, float diff_thres, float adaptive_c, float ball_r2, int32_t accumulate, int64_t* n_dynamic,
+                            int32_t mode, float res_alpha, float thres, bool adaptive, float ball_radius, int32_t accumulate, int64_t* n_dynamic,
                             bool allow_deferred, bool* overflowed) {
     *overflowed = false;
-    const bool adaptive = adaptive_c != 0.0f;
-    const float thres = adaptive ? adaptive_c : diff_thres;   // the kernels' `thres`: the constant, or the coefficient
     DevCloud* map;
     DevScanSet* scans;
     DevPoses* poses;
@@ -717,8 +754,7 @@ static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, 
     DeferredArgs da{};
     if (use_deferred && run) LTR_TRY(deferred_alloc(ctx, B, npx, &p_def, &da));
     // tile culling (project_cull.cuh): scan-minus-map variants only, one keyframe per lane -> launches of at most 32 keyframes
-    CullArgs ca;
-    std::memset(&ca, 0, sizeof(ca));
+    CullArgs ca{};
     // the sliding-window maxima cost 5 stores per pixel and keyframe: below one map point per pixel they cost more than the culling saves
     // (the small ND / PD candidate maps), so those passes project every pair
     const bool use_cull = p.use_fast && cand && ctx->cfg.fast_path >= 2 && B <= 32 && map->n >= kTilePts && map->n >= npx;
@@ -727,62 +763,27 @@ static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, 
     // scan-minus-map with the short elevation path and a 360 degree field of view: the test image is guard-padded (FastCfg::pad_*) and always built;
     // so is the adaptive threshold's (scan_test_image_kernel)
     const bool pad = p.use_fast && cand && p.fc.pad_ok;
-    const float timg_coeff = cand ? adaptive_c : 0.0f;
+    const float timg_coeff = cand && adaptive ? thres : 0.0f;
     const bool need_timg = p.use_fast && cand && (shortcut || pad || adaptive);
     const int64_t timg_px = pad ? (int64_t)p.fc.pad_npx : npx;
     // the scan-side images come from a kept set built over the whole range (scan_images_get) or, without one, are built per launch
     ScanImagesPin pin(ctx);
     ScanImageSet* set = nullptr;
     if (run) LTR_TRY(scan_images_get(ctx, p, *scans, *poses, kf_begin, kf_end, use_cull, need_timg, pad, timg_coeff, &set));
+    // the tile spheres bound culling's tiles and classify the fast path's ball tiles
+    const bool use_ball = ball_radius != 0.0f && run;
+    if (use_cull || (use_ball && p.use_fast)) LTR_TRY(tile_spheres(ctx, *map, &p_tiles));
     if (use_cull) {
         ca.enabled = 1;
-        ca.ntiles = (map->n + kTilePts - 1) / kTilePts;
-        ca.pyr_stride = (unsigned)(kPyrLevels * npx);
-        LTR_TRY(dev_alloc(ctx, &p_tiles, (size_t)ca.ntiles * sizeof(float4)));
-        if (!set) LTR_TRY(dev_alloc(ctx, &p_pyr, (size_t)B * ca.pyr_stride * sizeof(float)));
         ca.tiles = (const float4*)p_tiles;
-        tile_sphere_kernel<<<(unsigned)((ca.ntiles * 32 + 255) / 256), 256, 0, ctx->stream>>>(view(*map), (float4*)p_tiles, ca.ntiles);
-        LTR_LAUNCH_CHECK(ctx);
+        ca.ntiles = tile_count(map->n);
+        ca.pyr_stride = (unsigned)(kPyrLevels * npx);
+        if (!set) LTR_TRY(dev_alloc(ctx, &p_pyr, (size_t)B * ca.pyr_stride * sizeof(float)));
     }
-    // ball subset: the centres of the pass's keyframes and, on the fast path, the tile spheres (shared with culling), a non-finite flag per
-    // tile and the per-launch tile classification (BallLaunch)
     BallLaunch bl;
-    void *p_ball = nullptr;
+    void* p_ball = nullptr;
     ScratchGuard g_ball(ctx, &p_ball);
-    std::vector<float4> centre;   // outlives the copy below: the pass synchronises before it returns
-    if (ball_r2 != 0.0f && run) {
-        const int K = kf_end - kf_begin;
-        const long long ntiles = (map->n + kTilePts - 1) / kTilePts;
-        centre.resize((size_t)K);
-        for (int k = 0; k < K; ++k) {   // the pose's translation column (pose rows at 12..23 of DevPoses::h), rounded to f32
-            const double* T = &poses->h[(size_t)(kf_begin + k) * 24 + 12];
-            centre[(size_t)k] = make_float4((float)T[3], (float)T[7], (float)T[11], 0.0f);
-        }
-        const size_t c_bytes = ((size_t)K * sizeof(float4) + 255) / 256 * 256;
-        const size_t w_bytes = p.use_fast ? ((size_t)ntiles * 3 * sizeof(uint32_t) + 255) / 256 * 256 : 0;
-        const size_t t_bytes = (p.use_fast && !use_cull) ? (size_t)ntiles * sizeof(float4) : 0;
-        const size_t f_bytes = p.use_fast ? (size_t)ntiles : 0;
-        LTR_TRY(dev_alloc(ctx, &p_ball, c_bytes + w_bytes + t_bytes + f_bytes));
-        char* b = (char*)p_ball;
-        LTR_CUDA(ctx, cudaMemcpyAsync(b, centre.data(), (size_t)K * sizeof(float4), cudaMemcpyHostToDevice, ctx->stream));
-        bl.args.centre = (const float4*)b;
-        bl.args.r2 = ball_r2;
-        if (p.use_fast) {
-            bl.ntiles = ntiles;
-            bl.scratch = (uint32_t*)(b + c_bytes);
-            float4* tiles = use_cull ? (float4*)p_tiles : (float4*)(b + c_bytes + w_bytes);
-            if (!use_cull) {
-                tile_sphere_kernel<<<(unsigned)((ntiles * 32 + 255) / 256), 256, 0, ctx->stream>>>(view(*map), tiles, ntiles);
-                LTR_LAUNCH_CHECK(ctx);
-            }
-            uint8_t* nonfinite = (uint8_t*)(b + c_bytes + w_bytes + t_bytes);
-            LTR_CUDA(ctx, cudaMemsetAsync(nonfinite, 0, (size_t)ntiles, ctx->stream));
-            tile_nonfinite_kernel<<<(unsigned)((map->n + 255) / 256), 256, 0, ctx->stream>>>(view(*map), nonfinite);
-            LTR_LAUNCH_CHECK(ctx);
-            bl.tiles = tiles;
-            bl.nonfinite = nonfinite;
-        }
-    }
+    if (use_ball) LTR_TRY(ball_setup(ctx, p, *map, *poses, kf_begin, kf_end, ball_radius, (const float4*)p_tiles, &p_ball, &bl));
     LTR_TRY(pass_begin(ctx, p));
     if (run) {
         void *p_rimg = nullptr, *p_win = nullptr;
@@ -812,11 +813,10 @@ static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, 
                 test_img = need_timg ? l_timg : l_rimg;
                 if (use_cull) ca.pyr = (const float*)p_pyr;
             }
-            BallLaunch* blk = nullptr;
-            if (bl.args.centre) { blk = &bl; bl.args.centre = (const float4*)p_ball + (k0 - kf_begin); }
-            LTR_TRY(project_map(ctx, p, *map, *poses, k0, nb, proj, rimg, test_img, thres, adaptive, win, amin, ca, da, blk));
+            if (use_ball) bl.args.centre = (const float4*)p_ball + (k0 - kf_begin);
+            LTR_TRY(project_map(ctx, p, *map, *poses, k0, nb, proj, rimg, test_img, thres, adaptive, win, amin, ca, da, bl));
             const unsigned rb = (unsigned)((nb * npx + 255) / 256);
-            const auto resolve = cand ? (adaptive ? resolve_kernel<true, true> : resolve_kernel<true>) : (adaptive ? resolve_kernel<false, true> : resolve_kernel<false>);
+            const auto resolve = with_bools([](auto c, auto ad) { return resolve_kernel<c, ad>; }, cand, adaptive);
             resolve<<<rb, 256, 0, ctx->stream>>>(rimg, win, nb * npx, thres, map->flags);
             LTR_LAUNCH_CHECK(ctx);
         }
@@ -835,28 +835,32 @@ static int remove_pass_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, 
     return LTR_OK;
 }
 
+// The remove pass of the three entry points.  adaptive: `thres` is the coefficient c of the pixel threshold fl(c s), else the constant
+// threshold.  ball_radius > 0: keyframe k sees only the map points within that radius of its pose's f32 translation (ball_setup); 0: the
+// full map.  ND (true per-pixel minimum) runs in the deferred mode of project_fast.cuh unless the flags accumulate into earlier ones (a run
+// whose overflow list filled up would have to be undone).
+static int remove_pass(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end, int32_t mode,
+                       float res_alpha, float thres, bool adaptive, float ball_radius, int32_t accumulate, int64_t* n_dynamic) {
+    // NaN fails both comparisons
+    if (adaptive && !(thres > 0.0f && thres < 1.0f)) return fail(ctx, LTR_ERR_INVALID, "adaptive coefficient %g outside (0, 1)", (double)thres);
+    return with_deferred_retry([&](bool allow_deferred, bool* overflowed) {
+        return remove_pass_impl(ctx, map_h, scans_h, poses_h, kf_begin, kf_end, mode, res_alpha, thres, adaptive, ball_radius, accumulate, n_dynamic,
+                                allow_deferred && !accumulate, overflowed);
+    });
+}
+
 int ltr_remove_pass(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end,
                     int32_t mode, float res_alpha, float diff_thres, int32_t accumulate, int64_t* n_dynamic) {
     ApiTrace tr__(ctx, "ltr_remove_pass");
     if (!ctx) return LTR_ERR_INVALID;
-    // ND (true per-pixel minimum) runs in the deferred mode of project_fast.cuh unless the flags accumulate into earlier ones (a run whose
-    // overflow list filled up would have to be undone)
-    return with_deferred_retry([&](bool allow_deferred, bool* overflowed) {
-        return remove_pass_impl(ctx, map_h, scans_h, poses_h, kf_begin, kf_end, mode, res_alpha, diff_thres, 0.0f, 0.0f, accumulate, n_dynamic,
-                                allow_deferred && !accumulate, overflowed);
-    });
+    return remove_pass(ctx, map_h, scans_h, poses_h, kf_begin, kf_end, mode, res_alpha, diff_thres, false, 0.0f, accumulate, n_dynamic);
 }
 
 int ltr_remove_pass_adaptive(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end,
                              int32_t mode, float res_alpha, float adaptive_coeff, int32_t accumulate, int64_t* n_dynamic) {
     ApiTrace tr__(ctx, "ltr_remove_pass_adaptive");
     if (!ctx) return LTR_ERR_INVALID;
-    // NaN fails both comparisons
-    if (!(adaptive_coeff > 0.0f && adaptive_coeff < 1.0f)) return fail(ctx, LTR_ERR_INVALID, "adaptive coefficient %g outside (0, 1)", (double)adaptive_coeff);
-    return with_deferred_retry([&](bool allow_deferred, bool* overflowed) {
-        return remove_pass_impl(ctx, map_h, scans_h, poses_h, kf_begin, kf_end, mode, res_alpha, 0.0f, adaptive_coeff, 0.0f, accumulate, n_dynamic,
-                                allow_deferred && !accumulate, overflowed);
-    });
+    return remove_pass(ctx, map_h, scans_h, poses_h, kf_begin, kf_end, mode, res_alpha, adaptive_coeff, true, 0.0f, accumulate, n_dynamic);
 }
 
 int ltr_remove_pass_ball(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end,
@@ -865,15 +869,9 @@ int ltr_remove_pass_ball(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, ltr
     if (!ctx) return LTR_ERR_INVALID;
     // NaN fails every comparison
     if (!(ball_radius > 0.0f && ball_radius <= 3.4028235e38f)) return fail(ctx, LTR_ERR_INVALID, "ball radius %g is not finite and > 0", (double)ball_radius);
-    if (adaptive_coeff != 0.0f && !(adaptive_coeff > 0.0f && adaptive_coeff < 1.0f))
-        return fail(ctx, LTR_ERR_INVALID, "adaptive coefficient %g outside (0, 1)", (double)adaptive_coeff);
-    // PCL's radiusSearch hands FLANN radius^2 as a float; an r2 that rounds to 0 admits no point (-1 stands for it: 0 means "no ball")
-    float r2 = (float)((double)ball_radius * (double)ball_radius);
-    if (r2 == 0.0f) r2 = -1.0f;
-    return with_deferred_retry([&](bool allow_deferred, bool* overflowed) {
-        return remove_pass_impl(ctx, map_h, scans_h, poses_h, kf_begin, kf_end, mode, res_alpha, diff_thres, adaptive_coeff, r2, accumulate, n_dynamic,
-                                allow_deferred && !accumulate, overflowed);
-    });
+    const bool adaptive = adaptive_coeff != 0.0f;   // else the constant threshold diff_thres
+    return remove_pass(ctx, map_h, scans_h, poses_h, kf_begin, kf_end, mode, res_alpha, adaptive ? adaptive_coeff : diff_thres, adaptive, ball_radius,
+                       accumulate, n_dynamic);
 }
 
 // An overflowed run (*overflowed) frees its output again.
@@ -908,17 +906,14 @@ static int parse_projected_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_poses poses_h
         // deferred mode: the tiles are claimed near to far from each launch's keyframes (DeferredArgs::order); their bounding spheres
         // are computed once per call
         const bool use_order = use_deferred && mapc.n >= kTilePts;
-        const long long ntiles = (mapc.n + kTilePts - 1) / kTilePts;
+        const long long ntiles = tile_count(mapc.n);
         uint64_t* keys = nullptr;
         if (use_order) {
-            LTR_TRY(dev_alloc(ctx, &p_tiles, (size_t)ntiles * sizeof(float4)));
+            LTR_TRY(tile_spheres(ctx, mapc, &p_tiles));
             LTR_TRY(dev_alloc(ctx, &p_keys, (size_t)ntiles * 2 * sizeof(uint64_t)));
             keys = (uint64_t*)p_keys;
-            tile_sphere_kernel<<<(unsigned)((ntiles * 32 + 255) / 256), 256, 0, ctx->stream>>>(view(mapc), (float4*)p_tiles, ntiles);
-            LTR_LAUNCH_CHECK(ctx);
         }
-        CullArgs no_cull;
-        std::memset(&no_cull, 0, sizeof(no_cull));
+        const CullArgs no_cull{};
         LTR_TRY(dev_alloc(ctx, &p_list, (size_t)K * npx * sizeof(uint32_t)));
         const int nchunk = (int)((npx + kParseChunk - 1) / kParseChunk);
         LTR_TRY(dev_alloc(ctx, &p_cnt, ((size_t)K + (size_t)B * nchunk) * sizeof(unsigned int)));
@@ -1078,7 +1073,7 @@ int ltr_debug_fast_project(ltr_ctx* ctx, const float* xyz, int64_t n, const doub
     float* d_xyz = (float*)p;
     float* d_out = d_xyz + 3 * n;
     LTR_CUDA(ctx, cudaMemcpyAsync(d_xyz, xyz, (size_t)n * 12, cudaMemcpyHostToDevice, ctx->stream));
-    const auto kern = with_el_direct(fc, [](auto el) { return debug_fast_kernel<decltype(el)::value>; });
+    const auto kern = with_bools([](auto el) { return debug_fast_kernel<el>; }, fc.el_direct != 0);
     kern<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(d_xyz, n, pp.d_fast, pp.d, ctx->d_ext, ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order,
                                                                plan.g, fc, d_out);
     LTR_LAUNCH_CHECK(ctx);
