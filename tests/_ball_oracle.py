@@ -42,8 +42,10 @@ def members(xyz, c, radius):
         return sq_dist(xyz, c) < radius2(radius)
 
 
-def remove_pass(map_xyzi, scans_xyzi, offsets, poses, inv_poses, mode, alpha, radius, thres=0.1, coeff=0.0):
-    """flags (N,) uint8: the OR over the keyframes of the single-keyframe pass on the keyframe's ball subset."""
+def remove_pass(map_xyzi, scans_xyzi, offsets, poses, inv_poses, mode, alpha, radius, thres=0.1, coeff=0.0, lidar2base=oracle.IDENTITY,
+                order=0):
+    """flags (N,) uint8: the OR over the keyframes of the single-keyframe pass on the keyframe's ball subset.  The ball is centred on the
+    pose (the base), whatever the extrinsic; lidar2base and the transform order only reach the single-keyframe pass's projection."""
     m = np.ascontiguousarray(map_xyzi, F32)
     s = np.ascontiguousarray(scans_xyzi, F32)
     flags = np.zeros(len(m), np.uint8)
@@ -55,8 +57,8 @@ def remove_pass(map_xyzi, scans_xyzi, offsets, poses, inv_poses, mode, alpha, ra
         scan = s[offsets[k]:offsets[k + 1]]
         off = np.array([0, len(scan)], np.int64)
         if coeff:
-            f = _adaptive_oracle.remove_pass(m[idx], scan, off, inv_poses[k:k + 1], mode, alpha, coeff)
+            f = _adaptive_oracle.remove_pass(m[idx], scan, off, inv_poses[k:k + 1], mode, alpha, coeff, lidar2base=lidar2base, order=order)
         else:
-            f = oracle.remove_pass(m[idx], scan, off, inv_poses[k:k + 1], mode, alpha, thres)
+            f = oracle.remove_pass(m[idx], scan, off, inv_poses[k:k + 1], mode, alpha, thres, lidar2base=lidar2base, order=order)
         flags[idx[f != 0]] = 1
     return flags

@@ -66,9 +66,15 @@ def rollback(live, deltas, i, k, thr):
     return V(concat(set_minus(live, pd, k, thr), nd))
 
 
-def merged_map(scans, poses, leaf=LEAF):
-    """mergeAndDownsample(scans, leaf) with the identity extrinsic: every keyframe moved by its pose, concatenated, voxelised."""
-    parts = [oracle.transform(np.asarray(s, np.float32).reshape(-1, 4), p) for s, p in zip(scans, poses)]
+def merged_map(scans, poses, leaf=LEAF, lidar2base=oracle.IDENTITY, order=0):
+    """mergeAndDownsample(scans, leaf): every keyframe moved by lidar2base, then by its pose, in the given transform order, concatenated,
+    voxelised.  An identity lidar2base is skipped, as the library skips it (ltr_merge_scans_global passes no extrinsic then); applying it
+    would not be a no-op for -0.0 coordinates."""
+    ident = np.array_equal(np.asarray(lidar2base, np.float64), np.eye(4))
+    parts = []
+    for s, p in zip(scans, poses):
+        s = np.asarray(s, np.float32).reshape(-1, 4)
+        parts.append(oracle.transform(s if ident else oracle.transform(s, lidar2base, order), p, order))
     return oracle.voxel(np.concatenate(parts) if parts else np.zeros((0, 4), np.float32), leaf)
 
 
