@@ -90,11 +90,11 @@ static bool load_keyframes(LoadedSession& s, size_t k0, size_t k1, std::string* 
     return true;
 }
 
-static bool save_cloud(Removerter& R, ltr_cloud h, const std::string& path, bool octree_layout) {
+static bool save_cloud(Removerter& R, const CloudOwner& h, const std::string& path, bool octree_layout) {
     int64_t n = 0;
-    if (ltr_cloud_size(R.ctx, h, &n) != LTR_OK) return false;
+    if (ltr_cloud_size(R.ctx, h.get(), &n) != LTR_OK) return false;
     std::vector<float> buf((size_t)n * 4 + 4);
-    if (ltr_cloud_download(R.ctx, h, buf.data(), n, &n) != LTR_OK) return false;
+    if (ltr_cloud_download(R.ctx, h.get(), buf.data(), n, &n) != LTR_OK) return false;
     HostCloud c((size_t)n);
     if (n) std::memcpy(c.data(), buf.data(), (size_t)n * 16);
     std::string err;
@@ -102,12 +102,12 @@ static bool save_cloud(Removerter& R, ltr_cloud h, const std::string& path, bool
     return true;
 }
 
-static bool save_scans(Removerter& R, ltr_scanset s, const std::vector<std::string>& names, const std::string& dir, bool octree_layout) {  // saveScans (:1632-1650)
+static bool save_scans(Removerter& R, const ScanSetOwner& s, const std::vector<std::string>& names, const std::string& dir, bool octree_layout) {  // saveScans (:1632-1650)
     int32_t K = 0; int64_t total = 0;
-    if (s < 0 || ltr_scanset_info(R.ctx, s, &K, &total) != LTR_OK) return false;
+    if (s.get() < 0 || ltr_scanset_info(R.ctx, s.get(), &K, &total) != LTR_OK) return false;
     std::vector<float> buf((size_t)total * 4 + 4);
     std::vector<int64_t> off((size_t)K + 1);
-    if (ltr_scanset_download(R.ctx, s, buf.data(), total, off.data()) != LTR_OK) return false;
+    if (ltr_scanset_download(R.ctx, s.get(), buf.data(), total, off.data()) != LTR_OK) return false;
     for (int k = 0; k < K; ++k) {
         HostCloud c((size_t)(off[k + 1] - off[k]));
         if (!c.empty()) std::memcpy(c.data(), buf.data() + 4 * off[k], c.size() * 16);
@@ -395,15 +395,13 @@ int main(int argc, char** argv) {
             }
             if (save_map_pcd && R.owns(X)) {   // saveMapPointcloudByMergingCleanedScans: collective over the ranks holding the session
                 const std::string tag = sess == 0 ? "Central" : "Query";
-                ltr_cloud ms = -1, md = -1;
-                ck(R.mergeAndDownsample(X, X.scans_static_, 0.05f, &ms), "merge static scans");
-                ck(R.mergeAndDownsample(X, X.scans_dynamic_, 0.05f, &md), "merge dynamic scans");
+                CloudOwner ms, md;
+                ck(R.mergeAndDownsample(X, X.scans_static_.get(), 0.05f, &ms), "merge static scans");
+                ck(R.mergeAndDownsample(X, X.scans_dynamic_.get(), 0.05f, &md), "merge dynamic scans");
                 if (group_leader) {
                     ok &= save_cloud(R, ms, save_dir + "map_static/" + tag + "StaticScansMergedMapGlobal.pcd", true);
                     ok &= save_cloud(R, md, save_dir + "map_dynamic/" + tag + "DynamicScansMergedMapGlobal.pcd", true);
                 }
-                ltr_cloud_free(R.ctx, ms);
-                ltr_cloud_free(R.ctx, md);
             }
         }
     }

@@ -128,11 +128,11 @@ int ltr_knn_split_per_keyframe(ltr_ctx* ctx, ltr_scanset query_h, ltr_scanset ta
     if (T.pts.n > 0) LTR_TRY(finite_extent(ctx, T.pts, "target", mn, mx));
     if (Q.pts.n == 0) {
         const std::vector<int64_t> off((size_t)K + 1, 0);
-        if (out_near) LTR_TRY(scanset_new(ctx, off, out_near));
-        if (out_far) {
-            const int rc = scanset_new(ctx, off, out_far);
-            if (rc != LTR_OK) { if (out_near) ltr_scanset_free(ctx, *out_near); return rc; }
-        }
+        ScanSetOwner o_near, o_far;
+        if (out_near) LTR_TRY(scanset_new(ctx, off, &o_near));
+        if (out_far) LTR_TRY(scanset_new(ctx, off, &o_far));
+        if (out_near) *out_near = o_near.release();
+        if (out_far) *out_far = o_far.release();
         return LTR_OK;
     }
     void* flags = nullptr;

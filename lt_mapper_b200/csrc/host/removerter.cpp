@@ -29,7 +29,7 @@ struct StageTimer {
     ~StageTimer() { if (R.ctx) ltr_synchronize(R.ctx); R.timing[key] += now_s() - t0; }
 };
 
-std::map<std::string, ltr_cloud*> Session::cloud_names() {
+std::map<std::string, CloudOwner*> Session::cloud_names() {
     return {{"map_global_orig_", &map_global_orig_}, {"map_global_curr_", &map_global_curr_},
             {"map_global_curr_static_", &map_global_curr_static_}, {"map_global_curr_dynamic_", &map_global_curr_dynamic_},
             {"map_global_updated_", &map_global_updated_}, {"map_global_updated_strong_", &map_global_updated_strong_},
@@ -37,7 +37,7 @@ std::map<std::string, ltr_cloud*> Session::cloud_names() {
             {"map_global_pd_", &map_global_pd_}, {"map_global_pd_orig_", &map_global_pd_orig_},
             {"map_global_pd_strong_", &map_global_pd_strong_}, {"map_global_pd_weak_", &map_global_pd_weak_}};
 }
-std::map<std::string, ltr_scanset*> Session::scanset_names() {
+std::map<std::string, ScanSetOwner*> Session::scanset_names() {
     return {{"keyframe_scans_", &keyframe_scans_}, {"keyframe_scans_static_projected_", &keyframe_scans_static_projected_},
             {"keyframe_scans_dynamic_", &keyframe_scans_dynamic_}, {"scans_knn_coexist_", &scans_knn_coexist_},
             {"scans_knn_diff_", &scans_knn_diff_}, {"keyframe_scans_updated_", &keyframe_scans_updated_},
@@ -50,10 +50,6 @@ std::map<std::string, ltr_scanset*> Session::scanset_names() {
 Removerter::Removerter(const ltrh_params& p) : P(p) {
     central_sess_.sess_type_ = "Central"; central_sess_.id = 0;
     query_sess_.sess_type_ = "Query"; query_sess_.id = 1;
-}
-
-Removerter::~Removerter() {
-    if (ctx) { free_deltas(); ltr_destroy(ctx); }
 }
 
 int Removerter::fail(int code, const std::string& msg) { err = msg; return code; }
@@ -84,40 +80,31 @@ int Removerter::init() {
     cfg.keyframe_batch = P.keyframe_batch;
     cfg.fast_path = P.fast_path;
     const int rc = ltr_create(&ctx, &cfg);
+    ctx_owner_.reset(ctx);
     if (rc != LTR_OK) err = ltr_last_error(nullptr);
     if (const char* e = std::getenv("LTR_DIST_VOXEL_MIN")) dist_voxel_min = std::atoll(e);   // tests force the distributed path on small clouds
     return rc;
 }
 
-int Removerter::set(ltr_cloud* slot, ltr_cloud v) {
-    if (*slot >= 0 && *slot != v) CK(ltr_cloud_free(ctx, *slot));
-    *slot = v;
-    return LTR_OK;
-}
-int Removerter::set(ltr_scanset* slot, ltr_scanset v, bool) {
-    if (*slot >= 0 && *slot != v) CK(ltr_scanset_free(ctx, *slot));
-    *slot = v;
-    return LTR_OK;
-}
-int Removerter::assign(ltr_cloud* dst, ltr_cloud src) {
+int Removerter::assign(CloudOwner* dst, ltr_cloud src) {
     ltr_cloud c;
     if (src < 0) { CK(ltr_cloud_alloc(ctx, 0, &c)); }
     else CK(ltr_cloud_copy(ctx, src, &c));
-    return set(dst, c);
+    *dst = CloudOwner(ctx, c);
+    return LTR_OK;
 }
-int Removerter::append(ltr_cloud* dst, ltr_cloud src) {
-    if (*dst < 0) return assign(dst, src);
+int Removerter::append(CloudOwner* dst, ltr_cloud src) {
+    if (dst->get() < 0) return assign(dst, src);
     if (src < 0) return LTR_OK;
     ltr_cloud c;
-    CK(ltr_cloud_concat(ctx, *dst, src, &c));
-    return set(dst, c);
+    CK(ltr_cloud_concat(ctx, dst->get(), src, &c));
+    *dst = CloudOwner(ctx, c);
+    return LTR_OK;
 }
 int Removerter::save(const std::string& name, ltr_cloud c) {
     ltr_cloud copy;
     CK(ltr_cloud_copy(ctx, c, &copy));
-    auto it = saved.find(name);
-    if (it != saved.end()) { CK(ltr_cloud_free(ctx, it->second)); it->second = copy; }
-    else saved[name] = copy;
+    saved[name] = CloudOwner(ctx, copy);
     return LTR_OK;
 }
 
@@ -156,86 +143,93 @@ int Removerter::reduce_flags(ltr_cloud map, const Session& over) {
     return ltr_nccl_allreduce_flags(ctx, nccl_group[over.id], map) == LTR_OK ? LTR_OK : fail(LTR_ERR_CUDA, ltr_last_error(ctx));
 }
 
-int Removerter::gather_cloud(const Session& over, ltr_cloud* cloud) {
+int Removerter::gather_cloud(const Session& over, CloudOwner* cloud) {
     if (!sharded()) return LTR_OK;
+    const ltr_cloud local = cloud->get();
     ltr_cloud g;
-    CK(ltr_nccl_allgather_clouds(ctx, nccl_group[over.id], 1, cloud, &g));
-    return set(cloud, g);
+    CK(ltr_nccl_allgather_clouds(ctx, nccl_group[over.id], 1, &local, &g));
+    *cloud = CloudOwner(ctx, g);
+    return LTR_OK;
 }
 
-int Removerter::exchange_with_partner(int n_send, const ltr_cloud* send, int n_recv, ltr_cloud* recv) {
+int Removerter::exchange_with_partner(int n_send, const ltr_cloud* send, int n_recv, CloudOwner* recv) {
     if (!split) return fail(LTR_ERR_INVALID, "exchange_with_partner outside session-split mode");
-    return ltr_nccl_exchange_clouds(ctx, nccl_world, partner(), n_send, send, n_recv, recv) == LTR_OK ? LTR_OK : fail(LTR_ERR_CUDA, ltr_last_error(ctx));
+    std::vector<ltr_cloud> got((size_t)n_recv);
+    if (ltr_nccl_exchange_clouds(ctx, nccl_world, partner(), n_send, send, n_recv, got.data()) != LTR_OK) return fail(LTR_ERR_CUDA, ltr_last_error(ctx));
+    for (int i = 0; i < n_recv; ++i) recv[i] = CloudOwner(ctx, got[i]);
+    return LTR_OK;
 }
 
 int Removerter::load_session(int sess, const float* xyzi, const int64_t* offsets, const double* poses, const double* inv_poses, int K) {
     ltr_scanset ss;
     CK(ltr_scanset_upload(ctx, xyzi, offsets, K, &ss));
-    return load_session_scans(sess, ss, poses, inv_poses, K);
+    return load_session_scans(sess, ScanSetOwner(ctx, ss), poses, inv_poses, K);
 }
 
 int Removerter::load_session_raw(int sess, const float* xyzi, const int64_t* offsets, const double* poses, const double* inv_poses, int K,
                                  int32_t* n_overflowed) {
     ltr_scanset raw, ss;
     CK(ltr_scanset_upload(ctx, xyzi, offsets, K, &raw));
-    const int rc = ltr_voxel_grid_per_keyframe(ctx, raw, P.downsample_voxel_size, &ss, n_overflowed);   // Session.cpp:284-289
-    ltr_scanset_free(ctx, raw);
-    CK(rc);
-    return load_session_scans(sess, ss, poses, inv_poses, K);
+    ScanSetOwner raw_owner(ctx, raw);
+    CK(ltr_voxel_grid_per_keyframe(ctx, raw, P.downsample_voxel_size, &ss, n_overflowed));   // Session.cpp:284-289
+    raw_owner.reset();
+    return load_session_scans(sess, ScanSetOwner(ctx, ss), poses, inv_poses, K);
 }
 
 // the common tail of both loads: the device scan set `ss` and the uploaded poses become the session's keyframes
-int Removerter::load_session_scans(int sess, ltr_scanset ss, const double* poses, const double* inv_poses, int K) {
+int Removerter::load_session_scans(int sess, ScanSetOwner ss, const double* poses, const double* inv_poses, int K) {
     Session& S = sess == 0 ? central_sess_ : query_sess_;
     ltr_poses ps;
     CK(ltr_poses_upload(ctx, poses, inv_poses, K, &ps));
-    CK(set(&S.keyframe_scans_, ss, true));
-    if (S.keyframe_poses_ >= 0) CK(ltr_poses_free(ctx, S.keyframe_poses_));
-    S.keyframe_poses_ = ps;
+    S.keyframe_scans_ = std::move(ss);
+    S.keyframe_poses_ = PosesOwner(ctx, ps);
     S.num_keyframes_ = K;
     return LTR_OK;
 }
 
-int Removerter::octreeDownsampling(ltr_cloud* cloud, float leaf) {
+int Removerter::octreeDownsampling(CloudOwner* cloud, float leaf) {
     ltr_cloud v;
-    CK(ltr_voxel_centroid(ctx, *cloud, leaf, &v));
-    return set(cloud, v);
+    CK(ltr_voxel_centroid(ctx, cloud->get(), leaf, &v));
+    *cloud = CloudOwner(ctx, v);
+    return LTR_OK;
 }
 
-int Removerter::octreeDownsamplingAppended(ltr_cloud* cloud, float leaf) {
+int Removerter::octreeDownsamplingAppended(CloudOwner* cloud, float leaf) {
     int64_t n = 0;
-    CK(ltr_cloud_size(ctx, *cloud, &n));
+    CK(ltr_cloud_size(ctx, cloud->get(), &n));
     if (!sharded() || n < dist_voxel_min) return octreeDownsampling(cloud, leaf);
     const int g = nccl_group[0];            // the rank's own group (both entries are the same communicator)
     int32_t r = 0, w = 1;
     CK(ltr_nccl_info(ctx, g, &r, &w));
     ltr_cloud part, v;
-    CK(ltr_cloud_slice(ctx, *cloud, n * r / w, n * (r + 1) / w, &part));
-    const int rc = ltr_nccl_voxel_centroid_merged(ctx, g, part, leaf, &v);
-    ltr_cloud_free(ctx, part);
-    if (rc != LTR_OK) return fail(rc, ltr_last_error(ctx));
-    return set(cloud, v);
-}
-
-int Removerter::voxeliseMerged(Session& s, ltr_cloud merged, float leaf, ltr_cloud* out) {
-    CK(sharded() ? ltr_nccl_voxel_centroid_merged(ctx, nccl_group[s.id], merged, leaf, out) : ltr_voxel_centroid(ctx, merged, leaf, out));
+    CK(ltr_cloud_slice(ctx, cloud->get(), n * r / w, n * (r + 1) / w, &part));
+    CloudOwner part_owner(ctx, part);
+    CK(ltr_nccl_voxel_centroid_merged(ctx, g, part, leaf, &v));
+    part_owner.reset();
+    *cloud = CloudOwner(ctx, v);
     return LTR_OK;
 }
 
-int Removerter::mergeAndDownsample(Session& s, ltr_scanset scans, float leaf, ltr_cloud* out) {
+int Removerter::voxeliseMerged(Session& s, ltr_cloud merged, float leaf, CloudOwner* out) {
+    ltr_cloud v;
+    CK(sharded() ? ltr_nccl_voxel_centroid_merged(ctx, nccl_group[s.id], merged, leaf, &v) : ltr_voxel_centroid(ctx, merged, leaf, &v));
+    *out = CloudOwner(ctx, v);
+    return LTR_OK;
+}
+
+int Removerter::mergeAndDownsample(Session& s, ltr_scanset scans, float leaf, CloudOwner* out) {
     ltr_cloud m;
-    CK(ltr_merge_scans_global(ctx, scans, s.keyframe_poses_, &m));      // this rank's keyframes
-    const int rc = voxeliseMerged(s, m, leaf, out);
-    ltr_cloud_free(ctx, m);
-    return rc;
+    CK(ltr_merge_scans_global(ctx, scans, s.keyframe_poses_.get(), &m));      // this rank's keyframes
+    CloudOwner merged(ctx, m);
+    return voxeliseMerged(s, m, leaf, out);
 }
 
 int Removerter::precleaningKeyframes(float radius) {
     for (Session* s : {&central_sess_, &query_sess_}) {
         if (!owns(*s)) continue;
         ltr_scanset c;
-        CK(ltr_preclean(ctx, s->keyframe_scans_, radius, &c));
-        CK(set(&s->keyframe_scans_, c, true));
+        CK(ltr_preclean(ctx, s->keyframe_scans_.get(), radius, &c));
+        s->keyframe_scans_ = ScanSetOwner(ctx, c);
     }
     return LTR_OK;
 }
@@ -243,13 +237,14 @@ int Removerter::precleaningKeyframes(float radius) {
 int Removerter::makeGlobalMap(Session& s) {
     // with several ranks the voxelised map comes from the distributed voxeliser (each rank sorts its key range of the ~10^8 raw points);
     // map_global_orig_ keeps its meaning (the merged raw cloud of ALL keyframes) through a gather afterwards, in keyframe == rank order
-    ltr_cloud orig, curr;
-    CK(ltr_merge_scans_global(ctx, s.keyframe_scans_, s.keyframe_poses_, &orig));   // _sess.mergeScansWithinGlobalCoord() (:218), this rank's keyframes
-    CK(voxeliseMerged(s, orig, P.downsample_voxel_size, &curr));                    // :225
+    ltr_cloud merged;
+    CK(ltr_merge_scans_global(ctx, s.keyframe_scans_.get(), s.keyframe_poses_.get(), &merged));   // _sess.mergeScansWithinGlobalCoord() (:218), this rank's keyframes
+    CloudOwner orig(ctx, merged), curr;
+    CK(voxeliseMerged(s, orig.get(), P.downsample_voxel_size, &curr));                    // :225
     CK(gather_cloud(s, &orig));
-    CK(set(&s.map_global_orig_, orig));
-    CK(set(&s.map_global_curr_, curr));
-    CK(save("OriginalNoisy" + s.sess_type_ + "MapGlobal", s.map_global_curr_));       // :231
+    s.map_global_orig_ = std::move(orig);
+    s.map_global_curr_ = std::move(curr);
+    CK(save("OriginalNoisy" + s.sess_type_ + "MapGlobal", s.map_global_curr_.get()));       // :231
     return LTR_OK;
 }
 int Removerter::makeGlobalMap() {
@@ -261,65 +256,65 @@ int Removerter::makeGlobalMap() {
 // partitionCurrentMap / ForND / ForPD (:801-828, 771-799, 740-768) and the statements of removeOnce / revertOnce / iremoveOnceForND /
 // removeOnceForPD that follow it: the kept side (dynamic for revertOnce, static for the others) replaces its slot, is voxelised and becomes
 // the new *map; the other side is appended to its slot and voxelised.  Only the HD passes' appended maps go through the distributed voxeliser.
-int Removerter::partitionCurrentMapGeneric(ltr_cloud* map, Session& source, ltr_scanset scans, int mode, float res, const char* what,
-                                           bool keep_dynamic, ltr_cloud* stat, ltr_cloud* dyn) {
+int Removerter::partitionCurrentMapGeneric(CloudOwner* map, Session& source, ltr_scanset scans, int mode, float res, const char* what,
+                                           bool keep_dynamic, CloudOwner* stat, CloudOwner* dyn) {
     int64_t n_map = 0;
-    CK(ltr_cloud_size(ctx, *map, &n_map));
+    CK(ltr_cloud_size(ctx, map->get(), &n_map));
     // n_dynamic is taken from the partition below (after the cross-rank flag union), so no count is requested here
     if (mapBallRadius_ != 0.0f && mode == LTR_MODE_HD)   // removeOnce / revertOnce on the ball subsets (Removerter.cpp:617-624, commented out)
-        CK(ltr_remove_pass_ball(ctx, *map, scans, source.keyframe_poses_, 0, source.num_keyframes_, mode, res, 0.1f, adaptiveThresholdCoeff_,
+        CK(ltr_remove_pass_ball(ctx, map->get(), scans, source.keyframe_poses_.get(), 0, source.num_keyframes_, mode, res, 0.1f, adaptiveThresholdCoeff_,
                                 mapBallRadius_, 0, nullptr));
     else if (adaptiveThresholdCoeff_ != 0.0f)   // Removerter.cpp:396 in place of :398, for every variant
-        CK(ltr_remove_pass_adaptive(ctx, *map, scans, source.keyframe_poses_, 0, source.num_keyframes_, mode, res, adaptiveThresholdCoeff_, 0, nullptr));
+        CK(ltr_remove_pass_adaptive(ctx, map->get(), scans, source.keyframe_poses_.get(), 0, source.num_keyframes_, mode, res, adaptiveThresholdCoeff_, 0, nullptr));
     else
-        CK(ltr_remove_pass(ctx, *map, scans, source.keyframe_poses_, 0, source.num_keyframes_, mode, res, 0.1f, 0, nullptr));
-    CK(reduce_flags(*map, source));
+        CK(ltr_remove_pass(ctx, map->get(), scans, source.keyframe_poses_.get(), 0, source.num_keyframes_, mode, res, 0.1f, 0, nullptr));
+    CK(reduce_flags(map->get(), source));
     ltr_cloud st, dy;
-    CK(ltr_apply_partition(ctx, *map, &st, &dy));
+    CK(ltr_apply_partition(ctx, map->get(), &st, &dy));
+    CloudOwner kept(ctx, st), appended(ctx, dy);
     int64_t n_dyn = 0;
     CK(ltr_cloud_size(ctx, dy, &n_dyn));
     log.push_back(PassLog{what, n_map, n_dyn, -1, -1});
 
-    ltr_cloud *kept_slot = stat, *appended_slot = dyn;
-    ltr_cloud kept = st, appended = dy;
+    CloudOwner *kept_slot = stat, *appended_slot = dyn;
     if (keep_dynamic) { std::swap(kept_slot, appended_slot); std::swap(kept, appended); }
-    CK(set(kept_slot, kept));
+    *kept_slot = std::move(kept);
     CK(octreeDownsampling(kept_slot, 0.05f));
-    CK(assign(map, *kept_slot));
-    CK(append(appended_slot, appended));
-    CK(ltr_cloud_free(ctx, appended));
+    CK(assign(map, kept_slot->get()));
+    CK(append(appended_slot, appended.get()));
+    appended.reset();
     CK(mode == LTR_MODE_HD ? octreeDownsamplingAppended(appended_slot, 0.05f) : octreeDownsampling(appended_slot, 0.05f));
-    CK(ltr_cloud_size(ctx, *stat, &log.back().n_static_after));
-    CK(ltr_cloud_size(ctx, *dyn, &log.back().n_dynamic_after));
+    CK(ltr_cloud_size(ctx, stat->get(), &log.back().n_static_after));
+    CK(ltr_cloud_size(ctx, dyn->get(), &log.back().n_dynamic_after));
     return LTR_OK;
 }
 
 // keep static :894-895, voxelise :896, map :899-900, append dynamic :902, voxelise :903
 int Removerter::removeOnce(Session& t, Session& s, float res) {
-    return partitionCurrentMapGeneric(&t.map_global_curr_, s, s.keyframe_scans_, LTR_MODE_HD, res, "removeOnce", false,
+    return partitionCurrentMapGeneric(&t.map_global_curr_, s, s.keyframe_scans_.get(), LTR_MODE_HD, res, "removeOnce", false,
                                       &t.map_global_curr_static_, &t.map_global_curr_dynamic_);
 }
 
 // keep dynamic :919-920, voxelise :921, map :924-925, append static :927, voxelise :928
 int Removerter::revertOnce(Session& t, Session& s, float res) {
-    return partitionCurrentMapGeneric(&t.map_global_curr_, s, s.keyframe_scans_, LTR_MODE_HD, res, "revertOnce", true,
+    return partitionCurrentMapGeneric(&t.map_global_curr_, s, s.keyframe_scans_.get(), LTR_MODE_HD, res, "revertOnce", true,
                                       &t.map_global_curr_static_, &t.map_global_curr_dynamic_);
 }
 
 // keep strong :843-844, voxelise :845, map :848-849, append weak :851, voxelise :852
 int Removerter::iremoveOnceForND(Session& t, Session& s, float res) {
-    return partitionCurrentMapGeneric(&t.map_global_nd_, s, s.keyframe_scans_static_projected_, LTR_MODE_ND, res, "iremoveOnceForND", false,
+    return partitionCurrentMapGeneric(&t.map_global_nd_, s, s.keyframe_scans_static_projected_.get(), LTR_MODE_ND, res, "iremoveOnceForND", false,
                                       &t.map_global_nd_strong_, &t.map_global_nd_weak_);
 }
 
 // keep strong :868-869, voxelise :870, map :873-874, append weak :876, voxelise :878
 int Removerter::removeOnceForPD(Session& t, Session& s, float res) {
-    return partitionCurrentMapGeneric(&t.map_global_pd_, s, s.keyframe_scans_static_projected_, LTR_MODE_PD, res, "removeOnceForPD", false,
+    return partitionCurrentMapGeneric(&t.map_global_pd_, s, s.keyframe_scans_static_projected_.get(), LTR_MODE_PD, res, "removeOnceForPD", false,
                                       &t.map_global_pd_strong_, &t.map_global_pd_weak_);
 }
 
 int Removerter::resetCurrrentMapAsDynamic(Session& s, bool as_dynamic) {
-    return assign(&s.map_global_curr_, as_dynamic ? s.map_global_curr_dynamic_ : s.map_global_curr_static_);  // :714-732
+    return assign(&s.map_global_curr_, (as_dynamic ? s.map_global_curr_dynamic_ : s.map_global_curr_static_).get());  // :714-732
 }
 
 int Removerter::selfRemovert(Session& s) {
@@ -337,8 +332,9 @@ int Removerter::selfRemovert(Session& s) {
 
 int Removerter::extractHighDynPointsViaKnnDiff(Session& s, ltr_cloud target_map) {
     ltr_scanset di;
-    CK(ltr_knn_diff(ctx, s.keyframe_scans_, s.keyframe_poses_, 0, target_map, P.num_nn_points_within, P.dist_nn_points_within, nullptr, &di));
-    return set(&s.keyframe_scans_dynamic_, di, true);
+    CK(ltr_knn_diff(ctx, s.keyframe_scans_.get(), s.keyframe_poses_.get(), 0, target_map, P.num_nn_points_within, P.dist_nn_points_within, nullptr, &di));
+    s.keyframe_scans_dynamic_ = ScanSetOwner(ctx, di);
+    return LTR_OK;
 }
 
 int Removerter::removeHighDynamicPoints() {
@@ -351,22 +347,21 @@ int Removerter::removeHighDynamicPoints() {
     }
     if (P.extract_high_dyn_knn) {
         StageTimer t(*this, "hd_knn");
-        if (owns(C)) CK(extractHighDynPointsViaKnnDiff(C, C.map_global_curr_static_));  // :1591
-        if (owns(Q)) CK(extractHighDynPointsViaKnnDiff(Q, Q.map_global_curr_static_));  // :1592
-        ltr_cloud c = -1, q = -1;
-        if (owns(C)) CK(mergeAndDownsample(C, C.keyframe_scans_dynamic_, 0.05f, &c));  // :1594, :1597
-        if (owns(Q)) CK(mergeAndDownsample(Q, Q.keyframe_scans_dynamic_, 0.05f, &q));  // :1595, :1598
-        if (owns(C)) { CK(save("central_sess_high_dyn", c)); CK(ltr_cloud_free(ctx, c)); }  // :1600
-        if (owns(Q)) { CK(save("query_sess_high_dyn", q)); CK(ltr_cloud_free(ctx, q)); }    // :1601
+        if (owns(C)) CK(extractHighDynPointsViaKnnDiff(C, C.map_global_curr_static_.get()));  // :1591
+        if (owns(Q)) CK(extractHighDynPointsViaKnnDiff(Q, Q.map_global_curr_static_.get()));  // :1592
+        CloudOwner c, q;
+        if (owns(C)) CK(mergeAndDownsample(C, C.keyframe_scans_dynamic_.get(), 0.05f, &c));  // :1594, :1597
+        if (owns(Q)) CK(mergeAndDownsample(Q, Q.keyframe_scans_dynamic_.get(), 0.05f, &q));  // :1595, :1598
+        if (owns(C)) { CK(save("central_sess_high_dyn", c.get())); c.reset(); }  // :1600
+        if (owns(Q)) { CK(save("query_sess_high_dyn", q.get())); q.reset(); }    // :1601
     }
     if (split) {
         // Step 2 reads the OTHER session's static map (Removerter.cpp:1416, 1418): hand mine to my partner, take theirs
         StageTimer t(*this, "exchange");
         Session& mine = owns(C) ? C : Q;
         Session& other = owns(C) ? Q : C;
-        ltr_cloud got = -1;
-        CK(exchange_with_partner(1, &mine.map_global_curr_static_, 1, &got));
-        CK(set(&other.map_global_curr_static_, got));
+        const ltr_cloud send = mine.map_global_curr_static_.get();
+        CK(exchange_with_partner(1, &send, 1, &other.map_global_curr_static_));
     }
     return LTR_OK;
 }
@@ -377,25 +372,27 @@ int Removerter::removeHighDynamicPoints() {
 int Removerter::scansideRemovalForEachScan(Session& map_sess, Session& scan_sess, int criterion) {
     StageTimer t(*this, "scanside");
     if (!owns(scan_sess)) return LTR_OK;
-    if (map_sess.map_global_curr_static_ < 0) return fail(LTR_ERR_INVALID, "scansideRemovalForEachScan: no static map of the " + map_sess.sess_type_ + " session (run Steps 1-2 first)");
-    if (scan_sess.keyframe_scans_ < 0) return fail(LTR_ERR_INVALID, "scansideRemovalForEachScan: no keyframe scans of the " + scan_sess.sess_type_ + " session");
+    if (map_sess.map_global_curr_static_.get() < 0) return fail(LTR_ERR_INVALID, "scansideRemovalForEachScan: no static map of the " + map_sess.sess_type_ + " session (run Steps 1-2 first)");
+    if (scan_sess.keyframe_scans_.get() < 0) return fail(LTR_ERR_INVALID, "scansideRemovalForEachScan: no keyframe scans of the " + scan_sess.sess_type_ + " session");
     ltr_scanset st, dy;
-    CK(ltr_scanside_split(ctx, scan_sess.keyframe_scans_, scan_sess.keyframe_poses_, 0, map_sess.map_global_curr_static_, criterion,
+    CK(ltr_scanside_split(ctx, scan_sess.keyframe_scans_.get(), scan_sess.keyframe_poses_.get(), 0, map_sess.map_global_curr_static_.get(), criterion,
                           P.num_nn_points_within, P.dist_nn_points_within, &st, &dy));   // :1302-1309
-    CK(set(&scan_sess.scans_static_, st, true));
-    return set(&scan_sess.scans_dynamic_, dy, true);
+    scan_sess.scans_static_ = ScanSetOwner(ctx, st);
+    scan_sess.scans_dynamic_ = ScanSetOwner(ctx, dy);
+    return LTR_OK;
 }
 
-int Removerter::parseScansViaProjection(Session& s, ltr_cloud map, ltr_scanset* vec_to_store) {
+int Removerter::parseScansViaProjection(Session& s, ltr_cloud map, ScanSetOwner* vec_to_store) {
     ltr_scanset out;
-    CK(ltr_parse_projected(ctx, map, s.keyframe_poses_, 0, s.num_keyframes_, Session::kReprojectionAlpha, &out));
-    return set(vec_to_store, out, true);
+    CK(ltr_parse_projected(ctx, map, s.keyframe_poses_.get(), 0, s.num_keyframes_, Session::kReprojectionAlpha, &out));
+    *vec_to_store = ScanSetOwner(ctx, out);
+    return LTR_OK;
 }
 
 int Removerter::parseStaticScansViaProjection() {
     StageTimer t(*this, "parse_static");
-    if (owns(central_sess_)) CK(parseScansViaProjection(central_sess_, central_sess_.map_global_curr_, &central_sess_.keyframe_scans_static_projected_));  // Session.cpp:305-308
-    if (owns(query_sess_)) CK(parseScansViaProjection(query_sess_, query_sess_.map_global_curr_, &query_sess_.keyframe_scans_static_projected_));
+    if (owns(central_sess_)) CK(parseScansViaProjection(central_sess_, central_sess_.map_global_curr_.get(), &central_sess_.keyframe_scans_static_projected_));  // Session.cpp:305-308
+    if (owns(query_sess_)) CK(parseScansViaProjection(query_sess_, query_sess_.map_global_curr_.get(), &query_sess_.keyframe_scans_static_projected_));
     return LTR_OK;
 }
 
@@ -404,54 +401,56 @@ int Removerter::extractLowDynPointsViaKnnDiff(Session& s, ltr_cloud target_map) 
     s.clear_icp_stats();
     if (!useICPrefinement_) {
         // Session.cpp:395-402 (0.4 m downsample + ICP target) only feed the refinement, which the reference switches off (Session.cpp:551)
-        CK(ltr_knn_diff(ctx, s.keyframe_scans_static_projected_, s.keyframe_poses_, 0, target_map, P.num_nn_points_within, P.dist_nn_points_within, &co, &di));
+        CK(ltr_knn_diff(ctx, s.keyframe_scans_static_projected_.get(), s.keyframe_poses_.get(), 0, target_map, P.num_nn_points_within, P.dist_nn_points_within, &co, &di));
     } else {
         // Session.cpp:394-402: the ICP target is the other session's map at 0.4 m; partitionLowDynamicPointsOfScanByKnn (:549-584) registers
         // every keyframe to it and keeps the registered scan iff getFitnessScore() < 1.0.  Multi-GPU: this rank's keyframe block against
         // its replica of the target map, no collective.
         int32_t K = 0;
         int64_t npts = 0;
-        CK(ltr_scanset_info(ctx, s.keyframe_scans_static_projected_, &K, &npts));
+        CK(ltr_scanset_info(ctx, s.keyframe_scans_static_projected_.get(), &K, &npts));
         s.icp_T16_.resize((size_t)K * 16); s.icp_fitness_.resize((size_t)K); s.icp_iterations_.resize((size_t)K); s.icp_exit_.resize((size_t)K);
         s.icp_accepted_.resize((size_t)K);
-        ltr_cloud tgt = -1;
+        ltr_cloud tgt;
         CK(ltr_voxel_centroid(ctx, target_map, 0.4f, &tgt));   // Session.cpp:400
-        const int rc = ltr_icp_refine(ctx, s.keyframe_scans_static_projected_, s.keyframe_poses_, 0, tgt, nullptr, s.icp_T16_.data(), s.icp_fitness_.data(),
-                                      s.icp_iterations_.data(), s.icp_exit_.data());
-        ltr_cloud_free(ctx, tgt);
-        CK(rc);
+        CloudOwner tgt_owner(ctx, tgt);
+        CK(ltr_icp_refine(ctx, s.keyframe_scans_static_projected_.get(), s.keyframe_poses_.get(), 0, tgt, nullptr, s.icp_T16_.data(), s.icp_fitness_.data(),
+                          s.icp_iterations_.data(), s.icp_exit_.data()));
+        tgt_owner.reset();
         for (int32_t k = 0; k < K; ++k) s.icp_accepted_[(size_t)k] = s.icp_fitness_[(size_t)k] < 1.0 ? 1 : 0;   // Session.cpp:571
-        CK(ltr_knn_diff_refined(ctx, s.keyframe_scans_static_projected_, s.keyframe_poses_, 0, target_map, P.num_nn_points_within,
+        CK(ltr_knn_diff_refined(ctx, s.keyframe_scans_static_projected_.get(), s.keyframe_poses_.get(), 0, target_map, P.num_nn_points_within,
                                 P.dist_nn_points_within, s.icp_T16_.data(), s.icp_accepted_.data(), &co, &di));
     }
-    CK(set(&s.scans_knn_coexist_, co, true));
-    CK(set(&s.scans_knn_diff_, di, true));
+    s.scans_knn_coexist_ = ScanSetOwner(ctx, co);
+    s.scans_knn_diff_ = ScanSetOwner(ctx, di);
     return LTR_OK;
 }
 
 int Removerter::constructGlobalNDMap(Session& s) {
-    ltr_cloud m;
-    CK(mergeAndDownsample(s, s.scans_knn_diff_, 0.05f, &m));   // Session.cpp:432-434
-    return set(&s.map_global_nd_, m);
+    CloudOwner m;
+    CK(mergeAndDownsample(s, s.scans_knn_diff_.get(), 0.05f, &m));   // Session.cpp:432-434
+    s.map_global_nd_ = std::move(m);
+    return LTR_OK;
 }
 
 int Removerter::constructGlobalPDMap(Session& s) {
-    ltr_cloud m;
-    CK(mergeAndDownsample(s, s.scans_knn_diff_, 0.05f, &m));   // Session.cpp:439-441
-    CK(set(&s.map_global_pd_, m));
-    return assign(&s.map_global_pd_orig_, s.map_global_pd_);  // Session.cpp:444
+    CloudOwner m;
+    CK(mergeAndDownsample(s, s.scans_knn_diff_.get(), 0.05f, &m));   // Session.cpp:439-441
+    s.map_global_pd_ = std::move(m);
+    return assign(&s.map_global_pd_orig_, s.map_global_pd_.get());  // Session.cpp:444
 }
 
 int Removerter::removeWeakNDMapPointsHavingStrongNDInNear(Session& s) {
     int64_t n_strong = 0;
-    CK(ltr_cloud_size(ctx, s.map_global_nd_strong_, &n_strong));
+    CK(ltr_cloud_size(ctx, s.map_global_nd_strong_.get(), &n_strong));
     if (n_strong == 0) return LTR_OK;  // Session.cpp:454-455
     ltr_cloud near_, far_;
     // hard-coded k = 2, threshold 1.0 (Session.cpp:468-469)
-    CK(ltr_knn_split_cloud(ctx, s.map_global_nd_weak_, s.map_global_nd_strong_, 2, 1.0f, &near_, &far_));
+    CK(ltr_knn_split_cloud(ctx, s.map_global_nd_weak_.get(), s.map_global_nd_strong_.get(), 2, 1.0f, &near_, &far_));
+    CloudOwner near_owner(ctx, near_), far_owner(ctx, far_);
     CK(append(&s.map_global_nd_strong_, near_));  // Session.cpp:482 (+=)
-    CK(ltr_cloud_free(ctx, near_));
-    CK(set(&s.map_global_nd_weak_, far_));        // Session.cpp:483 (=)
+    near_owner.reset();
+    s.map_global_nd_weak_ = std::move(far_owner);  // Session.cpp:483 (=)
     return LTR_OK;
 }
 
@@ -474,8 +473,8 @@ int Removerter::detectLowDynamicPoints() {
     Session& Q = query_sess_;
     {
         StageTimer t(*this, "ld_knn");
-        if (owns(C)) CK(extractLowDynPointsViaKnnDiff(C, Q.map_global_curr_static_));  // :1416
-        if (owns(Q)) CK(extractLowDynPointsViaKnnDiff(Q, C.map_global_curr_static_));  // :1418
+        if (owns(C)) CK(extractLowDynPointsViaKnnDiff(C, Q.map_global_curr_static_.get()));  // :1416
+        if (owns(Q)) CK(extractLowDynPointsViaKnnDiff(Q, C.map_global_curr_static_.get()));  // :1418
     }
     {
         StageTimer t(*this, "ld_filter");
@@ -483,55 +482,57 @@ int Removerter::detectLowDynamicPoints() {
         if (split) {
             // :1427 is independent of :1421-1424, so the query side builds its PD map now and the two maps cross over
             if (owns(Q)) CK(constructGlobalPDMap(Q));
-            ltr_cloud got = -1;
+            CloudOwner got;
             // the sender drops its copy: from here on the member lives only where its filter passes run
             if (owns(C)) {
-                CK(exchange_with_partner(1, &C.map_global_nd_, 1, &got));
-                CK(set(&C.map_global_nd_, -1));
-                CK(set(&Q.map_global_pd_, got)); CK(assign(&Q.map_global_pd_orig_, Q.map_global_pd_));   // Session.cpp:444
+                const ltr_cloud send = C.map_global_nd_.get();
+                CK(exchange_with_partner(1, &send, 1, &got));
+                C.map_global_nd_.reset();
+                Q.map_global_pd_ = std::move(got); CK(assign(&Q.map_global_pd_orig_, Q.map_global_pd_.get()));   // Session.cpp:444
             } else {
-                CK(exchange_with_partner(1, &Q.map_global_pd_, 1, &got));
-                CK(set(&Q.map_global_pd_, -1)); CK(set(&Q.map_global_pd_orig_, -1));
-                CK(set(&C.map_global_nd_, got));
+                const ltr_cloud send = Q.map_global_pd_.get();
+                CK(exchange_with_partner(1, &send, 1, &got));
+                Q.map_global_pd_.reset(); Q.map_global_pd_orig_.reset();
+                C.map_global_nd_ = std::move(got);
             }
         }
         if (owns(Q)) {
-            if (C.map_global_nd_weak_ < 0) CK(assign(&C.map_global_nd_weak_, -1));
+            if (C.map_global_nd_weak_.get() < 0) CK(assign(&C.map_global_nd_weak_, -1));
             CK(filterStrongND(C, Q));                           // :1423
             CK(removeWeakNDMapPointsHavingStrongNDInNear(C));   // :1424
         }
         if (!split) CK(constructGlobalPDMap(Q));                // :1427
         if (owns(C)) {
-            if (Q.map_global_pd_weak_ < 0) CK(assign(&Q.map_global_pd_weak_, -1));
+            if (Q.map_global_pd_weak_.get() < 0) CK(assign(&Q.map_global_pd_weak_, -1));
             CK(filterStrongPD(Q, C));                           // :1429
             // revertStrongPDMapPointsHavingWeakPDInNear: empty TODO in the reference (Session.cpp:447-450)
-            CK(assign(&C.map_global_pd_, Q.map_global_pd_));                  // :1434
-            CK(assign(&C.map_global_pd_orig_, Q.map_global_pd_orig_));        // :1435
-            CK(assign(&C.map_global_pd_strong_, Q.map_global_pd_strong_));    // :1436
+            CK(assign(&C.map_global_pd_, Q.map_global_pd_.get()));                  // :1434
+            CK(assign(&C.map_global_pd_orig_, Q.map_global_pd_orig_.get()));        // :1435
+            CK(assign(&C.map_global_pd_strong_, Q.map_global_pd_strong_.get()));    // :1436
         }
     }
     {
         // always-on "save merged maps for visual debug" block (:1442-1480) including its in-place re-downsampling.
         // With several ranks the four merged clouds are voxelised without being gathered (mergeAndDownsample).
         StageTimer t(*this, "ld_merge_viz");
-        ltr_cloud qco = -1, cco = -1, qdi = -1, cdi = -1;
-        if (owns(Q)) CK(mergeAndDownsample(Q, Q.scans_knn_coexist_, 0.05f, &qco));   // :1443-1444
-        if (owns(C)) CK(mergeAndDownsample(C, C.scans_knn_coexist_, 0.05f, &cco));   // :1448-1449
-        if (owns(Q)) CK(mergeAndDownsample(Q, Q.scans_knn_diff_, 0.05f, &qdi));      // :1453-1454
-        if (owns(C)) CK(mergeAndDownsample(C, C.scans_knn_diff_, 0.05f, &cdi));      // :1458-1459
-        if (owns(Q)) { CK(save("union_map_queryside", qco)); CK(ltr_cloud_free(ctx, qco)); }     // :1446
-        if (owns(C)) { CK(save("union_map_centralside", cco)); CK(ltr_cloud_free(ctx, cco)); }   // :1451
-        if (owns(Q)) { CK(save("pd_map", qdi)); CK(ltr_cloud_free(ctx, qdi)); }                  // :1456
-        if (owns(C)) { CK(save("nd_map", cdi)); CK(ltr_cloud_free(ctx, cdi)); }                  // :1461
+        CloudOwner qco, cco, qdi, cdi;
+        if (owns(Q)) CK(mergeAndDownsample(Q, Q.scans_knn_coexist_.get(), 0.05f, &qco));   // :1443-1444
+        if (owns(C)) CK(mergeAndDownsample(C, C.scans_knn_coexist_.get(), 0.05f, &cco));   // :1448-1449
+        if (owns(Q)) CK(mergeAndDownsample(Q, Q.scans_knn_diff_.get(), 0.05f, &qdi));      // :1453-1454
+        if (owns(C)) CK(mergeAndDownsample(C, C.scans_knn_diff_.get(), 0.05f, &cdi));      // :1458-1459
+        if (owns(Q)) { CK(save("union_map_queryside", qco.get())); qco.reset(); }     // :1446
+        if (owns(C)) { CK(save("union_map_centralside", cco.get())); cco.reset(); }   // :1451
+        if (owns(Q)) { CK(save("pd_map", qdi.get())); qdi.reset(); }                  // :1456
+        if (owns(C)) { CK(save("nd_map", cdi.get())); cdi.reset(); }                  // :1461
         if (owns(Q)) {   // the ND members live where filterStrongND ran
             int64_t n = 0;
-            CK(ltr_cloud_size(ctx, C.map_global_nd_strong_, &n));
-            if (n != 0) { CK(octreeDownsampling(&C.map_global_nd_strong_, 0.05f)); CK(save("strong_nd_map", C.map_global_nd_strong_)); }   // :1463-1468
-            CK(octreeDownsampling(&C.map_global_nd_weak_, 0.05f)); CK(save("weak_nd_map", C.map_global_nd_weak_));                          // :1470-1472
+            CK(ltr_cloud_size(ctx, C.map_global_nd_strong_.get(), &n));
+            if (n != 0) { CK(octreeDownsampling(&C.map_global_nd_strong_, 0.05f)); CK(save("strong_nd_map", C.map_global_nd_strong_.get())); }   // :1463-1468
+            CK(octreeDownsampling(&C.map_global_nd_weak_, 0.05f)); CK(save("weak_nd_map", C.map_global_nd_weak_.get()));                          // :1470-1472
         }
         if (owns(C)) {   // the PD members live where filterStrongPD ran
-            CK(octreeDownsampling(&Q.map_global_pd_strong_, 0.05f)); CK(save("strong_pd_map", Q.map_global_pd_strong_));   // :1474-1476
-            CK(octreeDownsampling(&Q.map_global_pd_weak_, 0.05f)); CK(save("weak_pd_map", Q.map_global_pd_weak_));         // :1478-1480
+            CK(octreeDownsampling(&Q.map_global_pd_strong_, 0.05f)); CK(save("strong_pd_map", Q.map_global_pd_strong_.get()));   // :1474-1476
+            CK(octreeDownsampling(&Q.map_global_pd_weak_, 0.05f)); CK(save("weak_pd_map", Q.map_global_pd_weak_.get()));         // :1478-1480
         }
     }
     return LTR_OK;
@@ -540,53 +541,53 @@ int Removerter::detectLowDynamicPoints() {
 int Removerter::updateCurrentMap() {
     Session& C = central_sess_;
     Session& Q = query_sess_;
-    ltr_cloud uq = -1, uc = -1, upd = -1, strong = -1;
-    if (owns(Q)) CK(mergeAndDownsample(Q, Q.scans_knn_coexist_, 0.05f, &uq));  // :1489-1490
+    CloudOwner uq, uc, upd, strong;
+    if (owns(Q)) CK(mergeAndDownsample(Q, Q.scans_knn_coexist_.get(), 0.05f, &uq));  // :1489-1490
     if (split) {
         // Step 3 runs on the owners of the central keyframes; the query side hands over what it holds of the central session
         if (owns(Q)) {
-            const ltr_cloud send[3] = {uq, C.map_global_nd_weak_, C.map_global_nd_strong_};
+            const ltr_cloud send[3] = {uq.get(), C.map_global_nd_weak_.get(), C.map_global_nd_strong_.get()};
             CK(exchange_with_partner(3, send, 0, nullptr));
-            CK(ltr_cloud_free(ctx, uq));
+            uq.reset();
             return LTR_OK;
         }
-        ltr_cloud got[3] = {-1, -1, -1};
+        CloudOwner got[3];
         CK(exchange_with_partner(0, nullptr, 3, got));
-        uq = got[0];
-        CK(set(&C.map_global_nd_weak_, got[1]));
-        CK(set(&C.map_global_nd_strong_, got[2]));
+        uq = std::move(got[0]);
+        C.map_global_nd_weak_ = std::move(got[1]);
+        C.map_global_nd_strong_ = std::move(got[2]);
     }
-    CK(mergeAndDownsample(C, C.scans_knn_coexist_, 0.05f, &uc));  // :1492-1493
-    CK(assign(&upd, uq));                       // :1495
-    CK(append(&upd, uc));                       // :1496
-    CK(append(&upd, C.map_global_nd_weak_));    // :1500
-    CK(assign(&strong, upd));                   // :1505
-    CK(append(&strong, C.map_global_pd_strong_));  // :1506
-    CK(octreeDownsampling(&strong, 0.05f));     // :1507
-    CK(append(&upd, C.map_global_pd_orig_));    // :1511
-    CK(octreeDownsampling(&upd, 0.05f));        // :1512
-    CK(set(&C.map_global_updated_, upd)); CK(save("updated_map", upd));                      // :1516-1517
-    CK(set(&C.map_global_updated_strong_, strong)); CK(save("updated_map_strong", strong));  // :1519-1520
-    CK(ltr_cloud_free(ctx, uq));
-    CK(ltr_cloud_free(ctx, uc));
+    CK(mergeAndDownsample(C, C.scans_knn_coexist_.get(), 0.05f, &uc));  // :1492-1493
+    CK(assign(&upd, uq.get()));                       // :1495
+    CK(append(&upd, uc.get()));                       // :1496
+    CK(append(&upd, C.map_global_nd_weak_.get()));    // :1500
+    CK(assign(&strong, upd.get()));                   // :1505
+    CK(append(&strong, C.map_global_pd_strong_.get()));  // :1506
+    CK(octreeDownsampling(&strong, 0.05f));           // :1507
+    CK(append(&upd, C.map_global_pd_orig_.get()));    // :1511
+    CK(octreeDownsampling(&upd, 0.05f));              // :1512
+    C.map_global_updated_ = std::move(upd); CK(save("updated_map", C.map_global_updated_.get()));                      // :1516-1517
+    C.map_global_updated_strong_ = std::move(strong); CK(save("updated_map_strong", C.map_global_updated_strong_.get()));  // :1519-1520
+    uq.reset();
+    uc.reset();
     return LTR_OK;
 }
 
 int Removerter::parseUpdatedStaticScansViaProjection() {
     Session& C = central_sess_;
     if (!owns(C)) return LTR_OK;
-    CK(parseScansViaProjection(C, C.map_global_updated_, &C.keyframe_scans_updated_));
-    CK(parseScansViaProjection(C, C.map_global_updated_strong_, &C.keyframe_scans_updated_strong_));
+    CK(parseScansViaProjection(C, C.map_global_updated_.get(), &C.keyframe_scans_updated_));
+    CK(parseScansViaProjection(C, C.map_global_updated_strong_.get(), &C.keyframe_scans_updated_strong_));
     return LTR_OK;
 }
 
 int Removerter::parseLDScansViaProjection() {
     Session& C = central_sess_;
     if (!owns(C)) return LTR_OK;
-    CK(parseScansViaProjection(C, C.map_global_pd_orig_, &C.keyframe_scans_pd_));
-    CK(parseScansViaProjection(C, C.map_global_pd_strong_, &C.keyframe_scans_strong_pd_));
-    CK(parseScansViaProjection(C, C.map_global_nd_weak_, &C.keyframe_scans_weak_nd_));
-    CK(parseScansViaProjection(C, C.map_global_nd_strong_, &C.keyframe_scans_strong_nd_));
+    CK(parseScansViaProjection(C, C.map_global_pd_orig_.get(), &C.keyframe_scans_pd_));
+    CK(parseScansViaProjection(C, C.map_global_pd_strong_.get(), &C.keyframe_scans_strong_pd_));
+    CK(parseScansViaProjection(C, C.map_global_nd_weak_.get(), &C.keyframe_scans_weak_nd_));
+    CK(parseScansViaProjection(C, C.map_global_nd_strong_.get(), &C.keyframe_scans_strong_nd_));
     return LTR_OK;
 }
 
@@ -594,12 +595,15 @@ int Removerter::updateScansScanwise() {
     Session& C = central_sess_;
     if (!owns(C)) return LTR_OK;
     ltr_scanset a, b, v;
-    CK(ltr_scanset_concat_per_keyframe(ctx, C.keyframe_scans_updated_, C.keyframe_scans_weak_nd_, &a));  // Session.cpp:367-370
-    CK(ltr_scanset_concat_per_keyframe(ctx, a, C.keyframe_scans_pd_, &b));                               // Session.cpp:371
-    CK(ltr_voxel_centroid_per_keyframe(ctx, b, 0.05f, &v));                                              // Session.cpp:374
-    CK(ltr_scanset_free(ctx, a));
-    CK(ltr_scanset_free(ctx, b));
-    return set(&C.keyframe_scans_updated_, v, true);                                                    // Session.cpp:377
+    CK(ltr_scanset_concat_per_keyframe(ctx, C.keyframe_scans_updated_.get(), C.keyframe_scans_weak_nd_.get(), &a));  // Session.cpp:367-370
+    ScanSetOwner a_owner(ctx, a);
+    CK(ltr_scanset_concat_per_keyframe(ctx, a, C.keyframe_scans_pd_.get(), &b));                                     // Session.cpp:371
+    ScanSetOwner b_owner(ctx, b);
+    CK(ltr_voxel_centroid_per_keyframe(ctx, b, 0.05f, &v));                                                          // Session.cpp:374
+    a_owner.reset();
+    b_owner.reset();
+    C.keyframe_scans_updated_ = ScanSetOwner(ctx, v);                                                                // Session.cpp:377
+    return LTR_OK;
 }
 
 int Removerter::run_step0() {
@@ -630,24 +634,17 @@ int Removerter::reset_to_step0() {
         s->clear_icp_stats();   // Step 2's results
         auto it = saved.find("OriginalNoisy" + s->sess_type_ + "MapGlobal");
         if (!owns(*s)) {   // session-split: everything held of the other session was derived after Step 0
-            for (auto& kv : s->cloud_names()) if (*kv.second >= 0) { CK(ltr_cloud_free(ctx, *kv.second)); *kv.second = -1; }
+            for (auto& kv : s->cloud_names()) kv.second->reset();
             continue;
         }
         if (it == saved.end()) return fail(LTR_ERR_INVALID, "reset_to_step0: Step 0 has not run");
-        for (auto& kv : s->cloud_names()) {
-            if (kv.first == "map_global_orig_" || kv.first == "map_global_curr_") continue;
-            if (*kv.second >= 0) { CK(ltr_cloud_free(ctx, *kv.second)); *kv.second = -1; }
-        }
-        for (auto& kv : s->scanset_names()) {
-            if (kv.first == "keyframe_scans_") continue;
-            if (*kv.second >= 0) { CK(ltr_scanset_free(ctx, *kv.second)); *kv.second = -1; }
-        }
-        CK(assign(&s->map_global_curr_, it->second));
+        for (auto& kv : s->cloud_names()) if (kv.first != "map_global_orig_" && kv.first != "map_global_curr_") kv.second->reset();
+        for (auto& kv : s->scanset_names()) if (kv.first != "keyframe_scans_") kv.second->reset();
+        CK(assign(&s->map_global_curr_, it->second.get()));
     }
     for (auto it = saved.begin(); it != saved.end();) {
-        if (it->first.rfind("OriginalNoisy", 0) == 0) { ++it; continue; }
-        CK(ltr_cloud_free(ctx, it->second));
-        it = saved.erase(it);
+        if (it->first.rfind("OriginalNoisy", 0) == 0) ++it;
+        else it = saved.erase(it);
     }
     log.clear();
     timing.clear();
@@ -663,29 +660,22 @@ int Removerter::reset_to_step0() {
 // runs Steps 0-3 again.  Ranks that do not own the central session hold none of its scans and only release.
 int Removerter::cascade_promote_updated() {
     Session& C = central_sess_;
-    if (owns(C) && C.keyframe_scans_updated_ < 0) return fail(LTR_ERR_INVALID, "cascade: Step 3 has not run (no keyframe_scans_updated_)");
+    if (owns(C) && C.keyframe_scans_updated_.get() < 0) return fail(LTR_ERR_INVALID, "cascade: Step 3 has not run (no keyframe_scans_updated_)");
     ltr_scanset promoted = -1;
-    if (owns(C)) CK(ltr_voxel_grid_per_keyframe(ctx, C.keyframe_scans_updated_, P.downsample_voxel_size, &promoted, nullptr));
+    if (owns(C)) CK(ltr_voxel_grid_per_keyframe(ctx, C.keyframe_scans_updated_.get(), P.downsample_voxel_size, &promoted, nullptr));
+    ScanSetOwner promoted_owner(ctx, promoted);
     // with delta maps on, this generation's delta (what Step 3 added and removed, in each keyframe's frame) moves out of the session into
-    // deltas_ before the release below, so that it stays owned even if a free fails
-    if (deltaMaps_) {
-        std::pair<ltr_scanset, ltr_scanset> delta{-1, -1};
-        if (owns(C)) {
-            delta = {C.keyframe_scans_pd_, C.keyframe_scans_strong_nd_};
-            C.keyframe_scans_pd_ = C.keyframe_scans_strong_nd_ = -1;
-        }
-        deltas_.push_back(delta);
-    }
+    // deltas_ before the release below; ranks without central keyframes hold neither and record an empty pair
+    if (deltaMaps_) deltas_.emplace_back(std::move(C.keyframe_scans_pd_), std::move(C.keyframe_scans_strong_nd_));
     for (Session* s : {&central_sess_, &query_sess_}) {
-        for (auto& kv : s->cloud_names()) if (*kv.second >= 0) { CK(ltr_cloud_free(ctx, *kv.second)); *kv.second = -1; }
-        for (auto& kv : s->scanset_names()) if (*kv.second >= 0) { CK(ltr_scanset_free(ctx, *kv.second)); *kv.second = -1; }
+        for (auto& kv : s->cloud_names()) kv.second->reset();
+        for (auto& kv : s->scanset_names()) kv.second->reset();
         s->clear_icp_stats();
     }
-    for (auto& kv : saved) CK(ltr_cloud_free(ctx, kv.second));
     saved.clear();
-    if (query_sess_.keyframe_poses_ >= 0) { CK(ltr_poses_free(ctx, query_sess_.keyframe_poses_)); query_sess_.keyframe_poses_ = -1; }
+    query_sess_.keyframe_poses_.reset();
     query_sess_.num_keyframes_ = 0;
-    if (owns(C)) C.keyframe_scans_ = promoted;
+    C.keyframe_scans_ = std::move(promoted_owner);
     log.clear();
     timing.clear();
     return LTR_OK;
@@ -703,88 +693,76 @@ int Removerter::cascade_promote_updated() {
 // generations and restores V((L (-) PD) ++ ND) from the live central scans L.  Multi-GPU: each rank works on its own central keyframe
 // block; only the restored map's mergeAndDownsample crosses ranks.  Ranks without central keyframes record placeholders and return.
 // ---------------------------------------------------------------------------------------------------------------
-int Removerter::free_deltas() {
-    for (auto& g : deltas_) {
-        if (g.first >= 0) CK(ltr_scanset_free(ctx, g.first));
-        if (g.second >= 0) CK(ltr_scanset_free(ctx, g.second));
-    }
-    deltas_.clear();
-    return LTR_OK;
-}
-
 int Removerter::set_delta_maps(bool on) {
-    if (!on) CK(free_deltas());
+    if (!on) deltas_.clear();
     deltaMaps_ = on;
     return LTR_OK;
 }
 
 int Removerter::delta_load(const float* pd_xyzi, const int64_t* pd_off, const float* nd_xyzi, const int64_t* nd_off) {
     if (!deltaMaps_) return fail(LTR_ERR_INVALID, "delta_load: delta maps are off (ltrh_set_delta_maps)");
-    std::pair<ltr_scanset, ltr_scanset> g{-1, -1};
+    std::pair<ScanSetOwner, ScanSetOwner> g;
     if (owns(central_sess_)) {
         if (!pd_off || !nd_off) return fail(LTR_ERR_INVALID, "delta_load: null offsets");
-        CK(ltr_scanset_upload(ctx, pd_xyzi, pd_off, central_sess_.num_keyframes_, &g.first));
-        const int rc = ltr_scanset_upload(ctx, nd_xyzi, nd_off, central_sess_.num_keyframes_, &g.second);
-        if (rc != LTR_OK) { err = ltr_last_error(ctx); ltr_scanset_free(ctx, g.first); return rc; }
+        ltr_scanset pd, nd;
+        CK(ltr_scanset_upload(ctx, pd_xyzi, pd_off, central_sess_.num_keyframes_, &pd));
+        g.first = ScanSetOwner(ctx, pd);
+        CK(ltr_scanset_upload(ctx, nd_xyzi, nd_off, central_sess_.num_keyframes_, &nd));
+        g.second = ScanSetOwner(ctx, nd);
     }
-    deltas_.push_back(g);
+    deltas_.push_back(std::move(g));
     return LTR_OK;
 }
 
-int Removerter::copy_scanset(ltr_scanset s, ltr_scanset* out) {
+int Removerter::copy_scanset(ltr_scanset s, ScanSetOwner* out) {
     int32_t K = 0;
     CK(ltr_scanset_info(ctx, s, &K, nullptr));
     const std::vector<int64_t> zero((size_t)K + 1, 0);
-    ltr_scanset empty;
+    ltr_scanset empty, c;
     CK(ltr_scanset_upload(ctx, nullptr, zero.data(), K, &empty));
-    const int rc = ltr_scanset_concat_per_keyframe(ctx, s, empty, out);
-    ltr_scanset_free(ctx, empty);
-    CK(rc);
+    ScanSetOwner empty_owner(ctx, empty);
+    CK(ltr_scanset_concat_per_keyframe(ctx, s, empty, &c));
+    *out = ScanSetOwner(ctx, c);
     return LTR_OK;
 }
 
-int Removerter::set_difference(ltr_scanset a, ltr_scanset b, ltr_scanset* out) {
-    CK(ltr_knn_split_per_keyframe(ctx, a, b, P.num_nn_points_within, P.dist_nn_points_within, nullptr, out));
+int Removerter::set_difference(ltr_scanset a, ltr_scanset b, ScanSetOwner* out) {
+    ltr_scanset d;
+    CK(ltr_knn_split_per_keyframe(ctx, a, b, P.num_nn_points_within, P.dist_nn_points_within, nullptr, &d));
+    *out = ScanSetOwner(ctx, d);
     return LTR_OK;
 }
 
-int Removerter::concat_voxelise(ltr_scanset a, ltr_scanset b, ltr_scanset* out) {
-    ltr_scanset c = -1;
-    int rc = ltr_scanset_concat_per_keyframe(ctx, a, b, &c);
-    ltr_scanset_free(ctx, a);
-    ltr_scanset_free(ctx, b);
-    if (rc == LTR_OK) {
-        rc = ltr_voxel_centroid_per_keyframe(ctx, c, 0.05f, out);   // Session.cpp:374
-        ltr_scanset_free(ctx, c);
-    }
-    CK(rc);
+int Removerter::concat_voxelise(ScanSetOwner a, ScanSetOwner b, ScanSetOwner* out) {
+    ltr_scanset c, v;
+    CK(ltr_scanset_concat_per_keyframe(ctx, a.get(), b.get(), &c));
+    a.reset();
+    b.reset();
+    ScanSetOwner cat(ctx, c);
+    CK(ltr_voxel_centroid_per_keyframe(ctx, c, 0.05f, &v));   // Session.cpp:374
+    *out = ScanSetOwner(ctx, v);
     return LTR_OK;
 }
 
-// (PD, ND) composed over the generations [i, j), i < j; new handles
-int Removerter::compose(int i, int j, ltr_scanset* pd_out, ltr_scanset* nd_out) {
-    ltr_scanset pd = -1, nd = -1;
-    CK(copy_scanset(deltas_[(size_t)i].first, &pd));
-    int rc = copy_scanset(deltas_[(size_t)i].second, &nd);
-    for (int g = i + 1; g < j && rc == LTR_OK; ++g) {
-        const ltr_scanset pdg = deltas_[(size_t)g].first, ndg = deltas_[(size_t)g].second;
-        ltr_scanset a = -1, b = -1, c = -1, d = -1, nd2 = -1, pd2 = -1;
-        if ((rc = set_difference(nd, pdg, &a)) != LTR_OK) break;
-        if ((rc = set_difference(ndg, pd, &b)) != LTR_OK) { ltr_scanset_free(ctx, a); break; }
-        if ((rc = set_difference(pd, ndg, &c)) != LTR_OK) { ltr_scanset_free(ctx, a); ltr_scanset_free(ctx, b); break; }
-        if ((rc = set_difference(pdg, nd, &d)) != LTR_OK) { ltr_scanset_free(ctx, a); ltr_scanset_free(ctx, b); ltr_scanset_free(ctx, c); break; }
-        if ((rc = concat_voxelise(a, b, &nd2)) != LTR_OK) { ltr_scanset_free(ctx, c); ltr_scanset_free(ctx, d); break; }
-        if ((rc = concat_voxelise(c, d, &pd2)) != LTR_OK) { ltr_scanset_free(ctx, nd2); break; }
-        ltr_scanset_free(ctx, pd); ltr_scanset_free(ctx, nd);
-        pd = pd2; nd = nd2;
+// (PD, ND) composed over the generations [i, j), i < j; *pd_out and *nd_out are replaced only on success
+int Removerter::compose(int i, int j, ScanSetOwner* pd_out, ScanSetOwner* nd_out) {
+    ScanSetOwner pd, nd;
+    CK(copy_scanset(deltas_[(size_t)i].first.get(), &pd));
+    CK(copy_scanset(deltas_[(size_t)i].second.get(), &nd));
+    for (int g = i + 1; g < j; ++g) {
+        const ltr_scanset pdg = deltas_[(size_t)g].first.get(), ndg = deltas_[(size_t)g].second.get();
+        ScanSetOwner a, b, c, d, nd2, pd2;
+        CK(set_difference(nd.get(), pdg, &a));
+        CK(set_difference(ndg, pd.get(), &b));
+        CK(set_difference(pd.get(), ndg, &c));
+        CK(set_difference(pdg, nd.get(), &d));
+        CK(concat_voxelise(std::move(a), std::move(b), &nd2));
+        CK(concat_voxelise(std::move(c), std::move(d), &pd2));
+        pd = std::move(pd2);
+        nd = std::move(nd2);
     }
-    if (rc != LTR_OK) {
-        if (pd >= 0) ltr_scanset_free(ctx, pd);
-        if (nd >= 0) ltr_scanset_free(ctx, nd);
-        return rc;
-    }
-    *pd_out = pd;
-    *nd_out = nd;
+    *pd_out = std::move(pd);
+    *nd_out = std::move(nd);
     return LTR_OK;
 }
 
@@ -795,10 +773,7 @@ int Removerter::compose_changes(int i, int j) {
                                                                ") is not a non-empty range of the " + std::to_string(T) + " recorded generations");
     Session& C = central_sess_;
     if (!owns(C)) return LTR_OK;
-    ltr_scanset pd, nd;
-    CK(compose(i, j, &pd, &nd));
-    CK(set(&C.composed_pd_, pd, true));
-    return set(&C.composed_nd_, nd, true);
+    return compose(i, j, &C.composed_pd_, &C.composed_nd_);
 }
 
 int Removerter::rollback(int i) {
@@ -807,24 +782,21 @@ int Removerter::rollback(int i) {
     if (i < 0 || i > T) return fail(LTR_ERR_INVALID, "rollback: generation " + std::to_string(i) + " outside [0, " + std::to_string(T) + "]");
     Session& C = central_sess_;
     if (!owns(C)) return LTR_OK;
-    if (C.keyframe_scans_ < 0) return fail(LTR_ERR_INVALID, "rollback: no central keyframe scans");
-    ltr_scanset restored = -1;
+    if (C.keyframe_scans_.get() < 0) return fail(LTR_ERR_INVALID, "rollback: no central keyframe scans");
+    ScanSetOwner restored;
     if (i == T) {
-        CK(copy_scanset(C.keyframe_scans_, &restored));
+        CK(copy_scanset(C.keyframe_scans_.get(), &restored));
     } else {
-        ltr_scanset pd, nd, kept = -1;
+        ScanSetOwner pd, nd, kept;
         CK(compose(i, T, &pd, &nd));
-        const int rc = set_difference(C.keyframe_scans_, pd, &kept);
-        ltr_scanset_free(ctx, pd);
-        if (rc != LTR_OK) { ltr_scanset_free(ctx, nd); return rc; }
-        CK(concat_voxelise(kept, nd, &restored));
+        CK(set_difference(C.keyframe_scans_.get(), pd.get(), &kept));
+        pd.reset();
+        CK(concat_voxelise(std::move(kept), std::move(nd), &restored));
     }
-    CK(set(&C.keyframe_scans_restored_, restored, true));
-    ltr_cloud m;
-    CK(mergeAndDownsample(C, C.keyframe_scans_restored_, 0.05f, &m));
-    const int rc = save("restored_map", m);
-    ltr_cloud_free(ctx, m);
-    return rc;
+    C.keyframe_scans_restored_ = std::move(restored);
+    CloudOwner m;
+    CK(mergeAndDownsample(C, C.keyframe_scans_restored_.get(), 0.05f, &m));
+    return save("restored_map", m.get());
 }
 
 }  // namespace ltremovert_b200
@@ -984,14 +956,14 @@ int ltrh_cloud(ltrh_removerter* r, const char* name, int32_t sess, ltr_cloud* ou
     if (n.rfind("saved:", 0) == 0) {
         auto it = R.saved.find(n.substr(6));
         if (it == R.saved.end()) { R.err = "no saved cloud " + n; return LTR_ERR_INVALID; }
-        *out = it->second;
+        *out = it->second.get();
         return LTR_OK;
     }
     Session& S = sess == 0 ? R.central_sess_ : R.query_sess_;
     auto m = S.cloud_names();
     auto it = m.find(n);
-    if (it == m.end() || *it->second < 0) { R.err = "no cloud " + n; return LTR_ERR_INVALID; }
-    *out = *it->second;
+    if (it == m.end() || it->second->get() < 0) { R.err = "no cloud " + n; return LTR_ERR_INVALID; }
+    *out = it->second->get();
     return LTR_OK;
 }
 int ltrh_scanset(ltrh_removerter* r, const char* name, int32_t sess, ltr_scanset* out) {
@@ -999,8 +971,8 @@ int ltrh_scanset(ltrh_removerter* r, const char* name, int32_t sess, ltr_scanset
     Session& S = sess == 0 ? R.central_sess_ : R.query_sess_;
     auto m = S.scanset_names();
     auto it = m.find(name);
-    if (it == m.end() || *it->second < 0) { R.err = std::string("no scanset ") + name; return LTR_ERR_INVALID; }
-    *out = *it->second;
+    if (it == m.end() || it->second->get() < 0) { R.err = std::string("no scanset ") + name; return LTR_ERR_INVALID; }
+    *out = it->second->get();
     return LTR_OK;
 }
 double ltrh_timing(ltrh_removerter* r, const char* key) {

@@ -6,12 +6,18 @@
 #pragma once
 #include <cstdint>
 #include <map>
+#include <memory>
 #include <string>
 #include <utility>
 #include <vector>
 #include "../../../include/ltr_removert.h"
+#include "../handle_owner.h"
 
 namespace ltremovert_b200 {
+
+using ltr::CloudOwner;
+using ltr::PosesOwner;
+using ltr::ScanSetOwner;
 
 void invert4x4_public(const double* m, double* out);   // general 4x4 inverse by cofactors (removerter.cpp)
 
@@ -25,17 +31,17 @@ public:
     std::string sess_type_;
     int id = 0;                                        // 0 = central, 1 = query
     int num_keyframes_ = 0;                            // this rank's keyframes
-    ltr_poses keyframe_poses_ = -1;                    // keyframe_poses_ + keyframe_inverse_poses_ (Session.h:36-37)
+    PosesOwner keyframe_poses_;                        // keyframe_poses_ + keyframe_inverse_poses_ (Session.h:36-37)
     // per-keyframe clouds (Session.h:40-56)
-    ltr_scanset keyframe_scans_ = -1, keyframe_scans_static_projected_ = -1, keyframe_scans_dynamic_ = -1;
-    ltr_scanset scans_knn_coexist_ = -1, scans_knn_diff_ = -1;
-    ltr_scanset keyframe_scans_updated_ = -1, keyframe_scans_updated_strong_ = -1, keyframe_scans_pd_ = -1,
-                keyframe_scans_strong_pd_ = -1, keyframe_scans_strong_nd_ = -1, keyframe_scans_weak_nd_ = -1;
+    ScanSetOwner keyframe_scans_, keyframe_scans_static_projected_, keyframe_scans_dynamic_;
+    ScanSetOwner scans_knn_coexist_, scans_knn_diff_;
+    ScanSetOwner keyframe_scans_updated_, keyframe_scans_updated_strong_, keyframe_scans_pd_, keyframe_scans_strong_pd_, keyframe_scans_strong_nd_,
+                 keyframe_scans_weak_nd_;
     // scan-side removal of this session's scans (the commented central_/query_scans_{static,dynamic}_ of Removerter.h)
-    ltr_scanset scans_static_ = -1, scans_dynamic_ = -1;
+    ScanSetOwner scans_static_, scans_dynamic_;
     // LT-map change composition (DESIGN.md §5.3) on the central session: the composed delta of ltrh_compose_changes and the scans of
     // ltrh_rollback, per keyframe of this rank
-    ltr_scanset composed_pd_ = -1, composed_nd_ = -1, keyframe_scans_restored_ = -1;
+    ScanSetOwner composed_pd_, composed_nd_, keyframe_scans_restored_;
     // ICP refinement of the last extractLowDynPointsViaKnnDiff with useICPrefinement_ on (ltr_icp_refine), per keyframe of this rank
     std::vector<float> icp_T16_;
     std::vector<double> icp_fitness_;
@@ -43,19 +49,18 @@ public:
     std::vector<uint8_t> icp_accepted_;
     void clear_icp_stats() { icp_T16_.clear(); icp_fitness_.clear(); icp_iterations_.clear(); icp_exit_.clear(); icp_accepted_.clear(); }
     // maps (Session.h:67-87)
-    ltr_cloud map_global_orig_ = -1, map_global_curr_ = -1, map_global_curr_static_ = -1, map_global_curr_dynamic_ = -1;
-    ltr_cloud map_global_updated_ = -1, map_global_updated_strong_ = -1;
-    ltr_cloud map_global_nd_ = -1, map_global_nd_strong_ = -1, map_global_nd_weak_ = -1;
-    ltr_cloud map_global_pd_ = -1, map_global_pd_orig_ = -1, map_global_pd_strong_ = -1, map_global_pd_weak_ = -1;
+    CloudOwner map_global_orig_, map_global_curr_, map_global_curr_static_, map_global_curr_dynamic_;
+    CloudOwner map_global_updated_, map_global_updated_strong_;
+    CloudOwner map_global_nd_, map_global_nd_strong_, map_global_nd_weak_;
+    CloudOwner map_global_pd_, map_global_pd_orig_, map_global_pd_strong_, map_global_pd_weak_;
 
-    std::map<std::string, ltr_cloud*> cloud_names();
-    std::map<std::string, ltr_scanset*> scanset_names();
+    std::map<std::string, CloudOwner*> cloud_names();
+    std::map<std::string, ScanSetOwner*> scanset_names();
 };
 
 class Removerter {
 public:
     explicit Removerter(const ltrh_params& p);
-    ~Removerter();
     int init();  // creates the device context; returns ltr_status
 
     // ---- reference call graph (Removerter.cpp) ----
@@ -92,22 +97,22 @@ public:
     int rollback(int i);
 
     // ---- Session methods (Session.cpp) ----
-    int parseScansViaProjection(Session& s, ltr_cloud map, ltr_scanset* vec_to_store);     // Session.cpp:348-360
+    int parseScansViaProjection(Session& s, ltr_cloud map, ScanSetOwner* vec_to_store);    // Session.cpp:348-360
     int extractLowDynPointsViaKnnDiff(Session& s, ltr_cloud target_map);                   // Session.cpp:393-427, 549-584
     int extractHighDynPointsViaKnnDiff(Session& s, ltr_cloud target_map);                  // Session.cpp:487-504
     int constructGlobalNDMap(Session& s);                                                  // Session.cpp:430-435
     int constructGlobalPDMap(Session& s);                                                  // Session.cpp:437-445
     int removeWeakNDMapPointsHavingStrongNDInNear(Session& s);                             // Session.cpp:452-484
-    int octreeDownsampling(ltr_cloud* cloud, float leaf);                                  // utility.cpp:204-219, in place
+    int octreeDownsampling(CloudOwner* cloud, float leaf);                                 // utility.cpp:204-219, in place
     // the same for a freshly appended cloud ("*a += *b", never in octree order): with several ranks every rank contributes its slice of
     // the (replicated) cloud to the distributed voxeliser, so each sorts 1/G of it instead of all of it
-    int octreeDownsamplingAppended(ltr_cloud* cloud, float leaf);
+    int octreeDownsamplingAppended(CloudOwner* cloud, float leaf);
     // octreeDownsampling of the cloud merged over ALL keyframes of s, given this rank's part `merged` (not consumed): with several
     // ranks the parts are voxelised together without being gathered (ltr_nccl_voxel_centroid_merged)
-    int voxeliseMerged(Session& s, ltr_cloud merged, float leaf, ltr_cloud* out);
+    int voxeliseMerged(Session& s, ltr_cloud merged, float leaf, CloudOwner* out);
     // mergeScansWithinGlobalCoordUtil (utility.cpp:170-192) followed by octreeDownsampling of the result, the only way the path
     // consumes a merged cloud apart from map_global_orig_
-    int mergeAndDownsample(Session& s, ltr_scanset scans, float leaf, ltr_cloud* out);
+    int mergeAndDownsample(Session& s, ltr_scanset scans, float leaf, CloudOwner* out);
 
     // ---- plumbing ----
     int load_session(int sess, const float* xyzi, const int64_t* offsets, const double* poses, const double* inv_poses, int K);
@@ -115,10 +120,8 @@ public:
     // n_overflowed (optional) = scans the filter returned unchanged
     int load_session_raw(int sess, const float* xyzi, const int64_t* offsets, const double* poses, const double* inv_poses, int K,
                          int32_t* n_overflowed = nullptr);
-    int set(ltr_cloud* slot, ltr_cloud v);         // frees what the slot held, then stores v
-    int set(ltr_scanset* slot, ltr_scanset v, bool);
-    int assign(ltr_cloud* dst, ltr_cloud src);     // "*dst = *src" (deep copy)
-    int append(ltr_cloud* dst, ltr_cloud src);     // "*dst += *src"
+    int assign(CloudOwner* dst, ltr_cloud src);    // "*dst = *src" (deep copy)
+    int append(CloudOwner* dst, ltr_cloud src);    // "*dst += *src"
     int save(const std::string& name, ltr_cloud c);  // stands for pcl::io::savePCDFileBinary: keeps a device copy by name
     // ---- multi-GPU (SURVEY.md section 8e; see "Parallel decomposition" in removerter.cpp) ----
     int comm_init_nccl(const uint8_t* id128, int rank, int world, int split_sessions);   // native NCCL transport (ltr_nccl_*)
@@ -127,19 +130,21 @@ public:
     bool sharded() const { return group_world > 1; }
     int partner() const { return (rank + world / 2) % world; }
     int reduce_flags(ltr_cloud map, const Session& over);               // OR of the dynamic flags over the ranks that own `over`'s keyframes
-    int gather_cloud(const Session& over, ltr_cloud* cloud);            // *cloud <- rank-ordered concatenation over those ranks
-    int exchange_with_partner(int n_send, const ltr_cloud* send, int n_recv, ltr_cloud* recv);   // split mode only
+    int gather_cloud(const Session& over, CloudOwner* cloud);           // *cloud <- rank-ordered concatenation over those ranks
+    int exchange_with_partner(int n_send, const ltr_cloud* send, int n_recv, CloudOwner* recv);  // split mode only
     int fail(int code, const std::string& msg);
 
+    // declared first, so that the context is destroyed after every member that owns a handle in it
+    std::unique_ptr<ltr_ctx, void (*)(ltr_ctx*)> ctx_owner_{nullptr, ltr_destroy};
+    ltr_ctx* ctx = nullptr;   // ctx_owner_.get()
     ltrh_params P;
     bool useICPrefinement_ = false;   // Session.cpp:551 (`bool useICPrefinement { false }`), set by ltrh_set_icp_refinement
     float adaptiveThresholdCoeff_ = 0.0f;   // Removerter.cpp:395-396 (`adaptive_coeff`, commented out); 0: the constant 0.1 (:398), set by ltrh_set_adaptive_threshold
     bool deltaMaps_ = false;   // ltrh_set_delta_maps: cascade_promote_updated records each generation's delta in deltas_
-    // per generation (PD_g, ND_g) = (keyframe_scans_pd_, keyframe_scans_strong_nd_) of this rank's central keyframes; -1 on ranks without
-    // central keyframes, so that every rank counts the same generations
-    std::vector<std::pair<ltr_scanset, ltr_scanset>> deltas_;
+    // per generation (PD_g, ND_g) = (keyframe_scans_pd_, keyframe_scans_strong_nd_) of this rank's central keyframes; empty on ranks
+    // without central keyframes, so that every rank counts the same generations
+    std::vector<std::pair<ScanSetOwner, ScanSetOwner>> deltas_;
     float mapBallRadius_ = 0.0f;   // Removerter.h:46-48 (`kUseSubsetMapCloud` off, `kBallSize` 80 m); 0: the full map, set by ltrh_set_map_ball
-    ltr_ctx* ctx = nullptr;
     int rank = 0, world = 1;
     bool split = false;       // session-split: ranks [0, world/2) own the central keyframes, the others the query keyframes
     int nccl_world = -1;      // ltr_nccl communicator handles: everyone, ...
@@ -150,20 +155,19 @@ public:
     // every rank; LTR_DIST_VOXEL_MIN turns it on (the multi-rank tests do).
     int64_t dist_voxel_min = INT64_MAX;
     Session central_sess_, query_sess_;
-    std::map<std::string, ltr_cloud> saved;
+    std::map<std::string, CloudOwner> saved;
     std::map<std::string, double> timing;
     std::vector<PassLog> log;
     std::string err;
 
 private:
-    int load_session_scans(int sess, ltr_scanset ss, const double* poses, const double* inv_poses, int K);
-    int free_deltas();
-    int copy_scanset(ltr_scanset s, ltr_scanset* out);
-    int set_difference(ltr_scanset a, ltr_scanset b, ltr_scanset* out);          // a (-) b: the far part of a against b, per keyframe
-    int concat_voxelise(ltr_scanset a, ltr_scanset b, ltr_scanset* out);         // V(a ++ b), consumes a and b
-    int compose(int i, int j, ltr_scanset* pd, ltr_scanset* nd);
-    int partitionCurrentMapGeneric(ltr_cloud* map, Session& source, ltr_scanset scans, int mode, float res, const char* what,
-                                   bool keep_dynamic, ltr_cloud* stat, ltr_cloud* dyn);
+    int load_session_scans(int sess, ScanSetOwner ss, const double* poses, const double* inv_poses, int K);
+    int copy_scanset(ltr_scanset s, ScanSetOwner* out);
+    int set_difference(ltr_scanset a, ltr_scanset b, ScanSetOwner* out);         // a (-) b: the far part of a against b, per keyframe
+    int concat_voxelise(ScanSetOwner a, ScanSetOwner b, ScanSetOwner* out);      // V(a ++ b)
+    int compose(int i, int j, ScanSetOwner* pd, ScanSetOwner* nd);
+    int partitionCurrentMapGeneric(CloudOwner* map, Session& source, ltr_scanset scans, int mode, float res, const char* what,
+                                   bool keep_dynamic, CloudOwner* stat, CloudOwner* dyn);
 };
 
 }  // namespace ltremovert_b200

@@ -375,9 +375,9 @@ int ltr_icp_refine(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t
         for (int j = 0; j < 16; ++j) hT[16 * (size_t)k + j] = (j % 5 == 0) ? 1.0f : 0.0f;
     if (scans.pts.n > 0) {
         // 1. the global scans and their per-keyframe 0.4 m centroids
-        ScanSetOwner g_glob(ctx), g_src(ctx);
-        LTR_TRY(scanset_new(ctx, scans.h_off, &g_glob.h));
-        const DevCloud g = ctx->scansets[g_glob.h].pts;
+        ScanSetOwner g_glob;
+        LTR_TRY(scanset_new(ctx, scans.h_off, &g_glob));
+        const DevCloud g = ctx->scansets[g_glob.get()].pts;
         // scan_global as ltr_knn_diff moves it: base2lidar, then the pose
         LTR_TRY(scans_to_global(ctx, scans, 0, scans.pts.n, poses.d + (size_t)pose_offset * 24, ctx->ext_identity ? nullptr : ctx->d_ext, g.x(),
                                 g.y(), g.z(), g.i()));
@@ -385,9 +385,11 @@ int ltr_icp_refine(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t
             float mn[3], mx[3];
             LTR_TRY(finite_extent(ctx, g, "scan", mn, mx));
         }
-        LTR_TRY(ltr_voxel_centroid_per_keyframe(ctx, g_glob.h, P.source_leaf, &g_src.h));
+        ltr_scanset h_src;
+        LTR_TRY(ltr_voxel_centroid_per_keyframe(ctx, g_glob.get(), P.source_leaf, &h_src));
+        ScanSetOwner g_src(ctx, h_src);
         g_glob.reset();
-        const DevScanSet src = ctx->scansets[g_src.h];
+        const DevScanSet src = ctx->scansets[g_src.get()];
         // 2. the target's grid levels, all of them: every iteration searches them
         Pyramid pyr(ctx);
         pyr.init(view(tgt), nullptr, 1, tmn, tmx);

@@ -247,19 +247,23 @@ int ltr_knn_split_cloud(ltr_ctx* ctx, ltr_cloud query_h, ltr_cloud target_h, int
     void* t_block = nullptr;
     ScratchGuard g_grid(ctx, &t_block);
     if (q.n > 0) LTR_TRY(knn_target_build(ctx, target, k, thr, &t, &t_block));   // before the outputs exist, so that a rejected target leaks nothing
-    LTR_TRY(cloud_new(ctx, q.n, out_near));
-    LTR_TRY(cloud_new(ctx, q.n, out_far));
-    if (q.n == 0) return LTR_OK;
-    void* p = nullptr;
-    ScratchGuard g_p(ctx, &p);
-    LTR_TRY(dev_alloc(ctx, &p, (size_t)q.n));
-    LTR_TRY(knn_target_label(ctx, t, view(q), k, thr, (uint8_t*)p));
-    g_grid.release();
-    DevCloud o0 = ctx->clouds[*out_near], o1 = ctx->clouds[*out_far];
-    int64_t nf = 0;
-    LTR_TRY(stable_partition_by_flag(ctx, q, (const uint8_t*)p, &nf, &o0, &o1));
-    ctx->clouds[*out_near].n = o0.n;
-    ctx->clouds[*out_far].n = o1.n;
+    CloudOwner near_, far_;
+    LTR_TRY(cloud_new(ctx, q.n, &near_));
+    LTR_TRY(cloud_new(ctx, q.n, &far_));
+    if (q.n > 0) {
+        void* p = nullptr;
+        ScratchGuard g_p(ctx, &p);
+        LTR_TRY(dev_alloc(ctx, &p, (size_t)q.n));
+        LTR_TRY(knn_target_label(ctx, t, view(q), k, thr, (uint8_t*)p));
+        g_grid.release();
+        DevCloud o0 = ctx->clouds[near_.get()], o1 = ctx->clouds[far_.get()];
+        int64_t nf = 0;
+        LTR_TRY(stable_partition_by_flag(ctx, q, (const uint8_t*)p, &nf, &o0, &o1));
+        ctx->clouds[near_.get()].n = o0.n;
+        ctx->clouds[far_.get()].n = o1.n;
+    }
+    *out_near = near_.release();
+    *out_far = far_.release();
     return LTR_OK;
 }
 

@@ -81,7 +81,7 @@ void dev_free(ltr_ctx* ctx, void* p) {
     }
 }
 
-int cloud_new(ltr_ctx* ctx, int64_t n, ltr_cloud* out) {
+int cloud_new(ltr_ctx* ctx, int64_t n, CloudOwner* out) {
     if (n < 0) return fail(ctx, LTR_ERR_INVALID, "negative cloud size");
     int slot = -1;
     for (size_t i = 0; i < ctx->clouds.size(); ++i) if (!ctx->clouds[i].used) { slot = (int)i; break; }
@@ -92,7 +92,7 @@ int cloud_new(ltr_ctx* ctx, int64_t n, ltr_cloud* out) {
     LTR_TRY(dev_alloc(ctx, &p, (size_t)c.cap * 4 * sizeof(float)));
     c.base = (float*)p;
     ctx->clouds[slot] = c;
-    *out = slot;
+    *out = CloudOwner(ctx, slot);
     return LTR_OK;
 }
 int cloud_get(ltr_ctx* ctx, ltr_cloud h, DevCloud** c) {
@@ -100,7 +100,7 @@ int cloud_get(ltr_ctx* ctx, ltr_cloud h, DevCloud** c) {
     *c = &ctx->clouds[h];
     return LTR_OK;
 }
-void cloud_release(ltr_ctx* ctx, DevCloud* c) {
+static void cloud_release(ltr_ctx* ctx, DevCloud* c) {
     if (!c->borrowed) dev_free(ctx, c->base);
     dev_free(ctx, c->flags);
     *c = DevCloud();
@@ -113,7 +113,7 @@ int cloud_ensure_flags(ltr_ctx* ctx, DevCloud* c) {
     LTR_CUDA(ctx, cudaMemsetAsync(c->flags, 0, (size_t)c->cap, ctx->stream));
     return LTR_OK;
 }
-int scanset_new(ltr_ctx* ctx, const std::vector<int64_t>& off, ltr_scanset* out) {
+int scanset_new(ltr_ctx* ctx, const std::vector<int64_t>& off, ScanSetOwner* out) {
     const int K = (int)off.size() - 1;
     if (K < 0) return fail(ctx, LTR_ERR_INVALID, "scanset needs K+1 offsets");
     for (int k = 0; k < K; ++k) if (off[k + 1] < off[k]) return fail(ctx, LTR_ERR_INVALID, "scanset offsets must be non-decreasing");
@@ -134,7 +134,7 @@ int scanset_new(ltr_ctx* ctx, const std::vector<int64_t>& off, ltr_scanset* out)
     LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // `off` may be a temporary
     p_pts = nullptr; p_off = nullptr;
     ctx->scansets[slot] = s;
-    *out = slot;
+    *out = ScanSetOwner(ctx, slot);
     return LTR_OK;
 }
 int scanset_get(ltr_ctx* ctx, ltr_scanset h, DevScanSet** s) {
@@ -350,13 +350,19 @@ int ltr_memory_stats(const ltr_ctx* ctx, int64_t* stats3) {
 int ltr_cloud_upload(ltr_ctx* ctx, const float* xyzi, int64_t n, ltr_cloud* out) {
     ApiTrace tr__(ctx, "ltr_cloud_upload");
     if (!ctx || !out || (n > 0 && !xyzi)) return fail(ctx, LTR_ERR_INVALID, "null argument");
-    LTR_TRY(cloud_new(ctx, n, out));
-    return upload_points(ctx, xyzi, ctx->clouds[*out]);
+    CloudOwner o;
+    LTR_TRY(cloud_new(ctx, n, &o));
+    LTR_TRY(upload_points(ctx, xyzi, ctx->clouds[o.get()]));
+    *out = o.release();
+    return LTR_OK;
 }
 int ltr_cloud_alloc(ltr_ctx* ctx, int64_t n, ltr_cloud* out) {
     ApiTrace tr__(ctx, "ltr_cloud_alloc");
     if (!ctx || !out) return fail(ctx, LTR_ERR_INVALID, "null argument");
-    return cloud_new(ctx, n, out);
+    CloudOwner o;
+    LTR_TRY(cloud_new(ctx, n, &o));
+    *out = o.release();
+    return LTR_OK;
 }
 int ltr_cloud_size(ltr_ctx* ctx, ltr_cloud c, int64_t* n) {
     DevCloud* dc;
@@ -384,11 +390,13 @@ int ltr_cloud_copy(ltr_ctx* ctx, ltr_cloud src, ltr_cloud* out) {
     DevCloud* s;
     LTR_TRY(cloud_get(ctx, src, &s));
     const DevCloud sc = *s;
-    LTR_TRY(cloud_new(ctx, sc.n, out));
-    DevCloud& d = ctx->clouds[*out];
+    CloudOwner o;
+    LTR_TRY(cloud_new(ctx, sc.n, &o));
+    DevCloud& d = ctx->clouds[o.get()];
     if (sc.n > 0) {
         LTR_CUDA(ctx, cudaMemcpy2DAsync(d.base, (size_t)d.cap * 4, sc.base, (size_t)sc.cap * 4, (size_t)sc.n * 4, 4, cudaMemcpyDeviceToDevice, ctx->stream));
     }
+    *out = o.release();
     return LTR_OK;
 }
 int ltr_cloud_slice(ltr_ctx* ctx, ltr_cloud src, int64_t begin, int64_t end, ltr_cloud* out) {
@@ -411,10 +419,12 @@ int ltr_cloud_concat(ltr_ctx* ctx, ltr_cloud a, ltr_cloud b, ltr_cloud* out) {
     LTR_TRY(cloud_get(ctx, a, &pa));
     LTR_TRY(cloud_get(ctx, b, &pb));
     const DevCloud ca = *pa, cb = *pb;
-    LTR_TRY(cloud_new(ctx, ca.n + cb.n, out));
-    DevCloud& d = ctx->clouds[*out];
+    CloudOwner o;
+    LTR_TRY(cloud_new(ctx, ca.n + cb.n, &o));
+    DevCloud& d = ctx->clouds[o.get()];
     if (ca.n > 0) LTR_CUDA(ctx, cudaMemcpy2DAsync(d.base, (size_t)d.cap * 4, ca.base, (size_t)ca.cap * 4, (size_t)ca.n * 4, 4, cudaMemcpyDeviceToDevice, ctx->stream));
     if (cb.n > 0) LTR_CUDA(ctx, cudaMemcpy2DAsync(d.base + ca.n, (size_t)d.cap * 4, cb.base, (size_t)cb.cap * 4, (size_t)cb.n * 4, 4, cudaMemcpyDeviceToDevice, ctx->stream));
+    *out = o.release();
     return LTR_OK;
 }
 int ltr_cloud_device_ptrs(ltr_ctx* ctx, ltr_cloud c, float** x, float** y, float** z, float** i, int64_t* n) {
@@ -433,8 +443,11 @@ int ltr_scanset_upload(ltr_ctx* ctx, const float* xyzi, const int64_t* offsets, 
     if (!ctx || !out || !offsets || K < 0) return fail(ctx, LTR_ERR_INVALID, "bad argument");
     std::vector<int64_t> off(offsets, offsets + K + 1);
     if (off[K] > 0 && !xyzi) return fail(ctx, LTR_ERR_INVALID, "null points");
-    LTR_TRY(scanset_new(ctx, off, out));
-    return upload_points(ctx, xyzi, ctx->scansets[*out].pts);
+    ScanSetOwner o;
+    LTR_TRY(scanset_new(ctx, off, &o));
+    LTR_TRY(upload_points(ctx, xyzi, ctx->scansets[o.get()].pts));
+    *out = o.release();
+    return LTR_OK;
 }
 int ltr_scanset_info(ltr_ctx* ctx, ltr_scanset s, int32_t* K, int64_t* total) {
     DevScanSet* ss;
@@ -467,9 +480,11 @@ int ltr_scanset_flatten(ltr_ctx* ctx, ltr_scanset s, ltr_cloud* out) {
     DevScanSet* ss;
     LTR_TRY(scanset_get(ctx, s, &ss));
     const DevCloud sc = ss->pts;
-    LTR_TRY(cloud_new(ctx, sc.n, out));
-    DevCloud& d = ctx->clouds[*out];
+    CloudOwner o;
+    LTR_TRY(cloud_new(ctx, sc.n, &o));
+    DevCloud& d = ctx->clouds[o.get()];
     if (sc.n > 0) LTR_CUDA(ctx, cudaMemcpy2DAsync(d.base, (size_t)d.cap * 4, sc.base, (size_t)sc.cap * 4, (size_t)sc.n * 4, 4, cudaMemcpyDeviceToDevice, ctx->stream));
+    *out = o.release();
     return LTR_OK;
 }
 int ltr_scanset_concat_per_keyframe(ltr_ctx* ctx, ltr_scanset a, ltr_scanset b, ltr_scanset* out) {
@@ -483,13 +498,15 @@ int ltr_scanset_concat_per_keyframe(ltr_ctx* ctx, ltr_scanset a, ltr_scanset b, 
     for (int k = 0; k < K; ++k) off[k + 1] = off[k] + (pa->h_off[k + 1] - pa->h_off[k]) + (pb->h_off[k + 1] - pb->h_off[k]);
     const DevCloud ca = pa->pts, cb = pb->pts;
     const std::vector<int64_t> oa = pa->h_off, ob = pb->h_off;
-    LTR_TRY(scanset_new(ctx, off, out));
-    DevCloud& d = ctx->scansets[*out].pts;
+    ScanSetOwner o;
+    LTR_TRY(scanset_new(ctx, off, &o));
+    DevCloud& d = ctx->scansets[o.get()].pts;
     for (int k = 0; k < K; ++k) {
         const int64_t na = oa[k + 1] - oa[k], nb = ob[k + 1] - ob[k];
         if (na > 0) LTR_CUDA(ctx, cudaMemcpy2DAsync(d.base + off[k], (size_t)d.cap * 4, ca.base + oa[k], (size_t)ca.cap * 4, (size_t)na * 4, 4, cudaMemcpyDeviceToDevice, ctx->stream));
         if (nb > 0) LTR_CUDA(ctx, cudaMemcpy2DAsync(d.base + off[k] + na, (size_t)d.cap * 4, cb.base + ob[k], (size_t)cb.cap * 4, (size_t)nb * 4, 4, cudaMemcpyDeviceToDevice, ctx->stream));
     }
+    *out = o.release();
     return LTR_OK;
 }
 
@@ -506,18 +523,19 @@ int ltr_poses_upload(ltr_ctx* ctx, const double* poses, const double* inv_poses,
         std::memcpy(&p.h[(size_t)k * 24], inv_poses + (size_t)k * 16, 12 * sizeof(double));
         std::memcpy(&p.h[(size_t)k * 24 + 12], poses + (size_t)k * 16, 12 * sizeof(double));
     }
-    void* d;
-    LTR_TRY(dev_alloc(ctx, &d, (size_t)K * 24 * sizeof(double)));
-    p.d = (double*)d;
+    void *p_d = nullptr, *p_fast = nullptr;
+    ScratchGuard g_d(ctx, &p_d), g_fast(ctx, &p_fast);   // disarmed once the handle owns both blocks
+    LTR_TRY(dev_alloc(ctx, &p_d, (size_t)K * 24 * sizeof(double)));
+    p.d = (double*)p_d;
     if (K > 0) LTR_CUDA(ctx, cudaMemcpyAsync(p.d, p.h.data(), (size_t)K * 24 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     p.h_fast.resize((size_t)K * 16);
     for (int k = 0; k < K; ++k) make_kf_fast(&p.h[(size_t)k * 24], ctx->cfg.base2lidar, ctx->ext_identity, &p.h_fast[(size_t)k * 16]);
-    LTR_TRY(dev_alloc(ctx, &d, (size_t)K * 16 * sizeof(float)));
-    p.d_fast = (float*)d;
+    LTR_TRY(dev_alloc(ctx, &p_fast, (size_t)K * 16 * sizeof(float)));
+    p.d_fast = (float*)p_fast;
     if (K > 0) LTR_CUDA(ctx, cudaMemcpyAsync(p.d_fast, p.h_fast.data(), (size_t)K * 16 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    p_d = p_fast = nullptr;
     ctx->poses[slot] = p;
-    LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     *out = slot;
     return LTR_OK;
 }

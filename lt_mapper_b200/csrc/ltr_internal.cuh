@@ -9,6 +9,7 @@
 #include <map>
 #include <chrono>
 #include "../../include/ltr_b200.h"
+#include "handle_owner.h"
 
 namespace ltr {
 
@@ -189,27 +190,12 @@ struct ScratchGuard {
     ScratchGuard& operator=(const ScratchGuard&) = delete;
 };
 
-// Owns an ltr_cloud / ltr_scanset handle (h, -1: none) and frees it on every exit path; reset() frees it now.
-template <int (*Free)(ltr_ctx*, int32_t)>
-struct HandleOwner {
-    ltr_ctx* ctx;
-    int32_t h;
-    explicit HandleOwner(ltr_ctx* c, int32_t handle = -1) : ctx(c), h(handle) {}
-    ~HandleOwner() { reset(); }
-    void reset() { if (h >= 0) { Free(ctx, h); h = -1; } }
-    HandleOwner(const HandleOwner&) = delete;
-    HandleOwner& operator=(const HandleOwner&) = delete;
-};
-using CloudOwner = HandleOwner<ltr_cloud_free>;
-using ScanSetOwner = HandleOwner<ltr_scanset_free>;
-
-int cloud_new(ltr_ctx* ctx, int64_t n, ltr_cloud* out);          // uninitialised cloud of n points
+int cloud_new(ltr_ctx* ctx, int64_t n, CloudOwner* out);         // uninitialised cloud of n points
 int cloud_get(ltr_ctx* ctx, ltr_cloud h, DevCloud** c);
-int scanset_new(ltr_ctx* ctx, const std::vector<int64_t>& off, ltr_scanset* out);  // allocates points + uploads offsets
+int scanset_new(ltr_ctx* ctx, const std::vector<int64_t>& off, ScanSetOwner* out);  // allocates points + uploads offsets
 int scanset_get(ltr_ctx* ctx, ltr_scanset h, DevScanSet** s);
 int poses_get(ltr_ctx* ctx, ltr_poses h, DevPoses** p);
 int cloud_ensure_flags(ltr_ctx* ctx, DevCloud* c);
-void cloud_release(ltr_ctx* ctx, DevCloud* c);
 
 inline int64_t round_cap(int64_t n) { return ((n > 0 ? n : 1) + 63) / 64 * 64; }
 inline PtrView view(const DevCloud& c) { return PtrView{c.x(), c.y(), c.z(), c.i(), c.n}; }
@@ -237,7 +223,7 @@ int nccl_comm_info(ltr_ctx* ctx, int comm, int* rank, int* world);
 int nccl_allreduce_u32(ltr_ctx* ctx, int comm, uint32_t* dev, size_t count, int op /* 0 sum, 1 min, 2 max */);
 // `send` holds this rank's points grouped by destination rank (segment d has scount[d] points, segments back to back); *recv_out
 // receives, in source-rank order, what every rank sent to this one
-int nccl_alltoallv_cloud(ltr_ctx* ctx, int comm, const DevCloud& send, const std::vector<int64_t>& scount, ltr_cloud* recv_out);
+int nccl_alltoallv_cloud(ltr_ctx* ctx, int comm, const DevCloud& send, const std::vector<int64_t>& scount, CloudOwner* recv_out);
 
 // drops the held scan-image sets (all, or those built from the scan set / poses with that serial); free_storage also returns the slots'
 // storage blocks to the allocator (project.cu)

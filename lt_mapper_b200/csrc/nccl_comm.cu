@@ -108,7 +108,7 @@ int nccl_allreduce_u32(ltr_ctx* ctx, int comm, uint32_t* dev, size_t count, int 
     return LTR_OK;
 }
 
-int nccl_alltoallv_cloud(ltr_ctx* ctx, int comm, const DevCloud& send, const std::vector<int64_t>& scount, ltr_cloud* recv_out) {
+int nccl_alltoallv_cloud(ltr_ctx* ctx, int comm, const DevCloud& send, const std::vector<int64_t>& scount, CloudOwner* recv_out) {
     NcclComm* cp;
     LTR_TRY(comm_get(ctx, comm, &cp));
     const NcclComm cc = *cp;
@@ -120,7 +120,7 @@ int nccl_alltoallv_cloud(ltr_ctx* ctx, int comm, const DevCloud& send, const std
     for (int d = 0; d < G; ++d) sdispl[d + 1] = sdispl[d] + scount[d];
     for (int r = 0; r < G; ++r) rdispl[r + 1] = rdispl[r] + all[(size_t)r * G + cc.rank];
     LTR_TRY(cloud_new(ctx, rdispl[G], recv_out));
-    const DevCloud dst = ctx->clouds[*recv_out];
+    const DevCloud dst = ctx->clouds[recv_out->get()];
     const float* sp[4] = {send.x(), send.y(), send.z(), send.i()};
     float* dp[4] = {dst.x(), dst.y(), dst.z(), dst.i()};
     NcclApi* a = nccl_api();
@@ -259,8 +259,14 @@ int ltr_nccl_allgather_clouds(ltr_ctx* ctx, int32_t comm, int32_t count, const l
     LTR_TRY(comm_get(ctx, comm, &c));
     if (!local || !out || count < 1 || count > kMaxBatch) return fail(ctx, LTR_ERR_INVALID, "bad argument");
     const NcclComm cc = *c;
+    std::vector<CloudOwner> o((size_t)count);
     if (cc.world <= 1) {
-        for (int i = 0; i < count; ++i) LTR_TRY(ltr_cloud_copy(ctx, local[i], &out[i]));
+        for (int i = 0; i < count; ++i) {
+            ltr_cloud h;
+            LTR_TRY(ltr_cloud_copy(ctx, local[i], &h));
+            o[i] = CloudOwner(ctx, h);
+        }
+        for (int i = 0; i < count; ++i) out[i] = o[i].release();
         return LTR_OK;
     }
     int64_t mine[kMaxBatch];
@@ -271,12 +277,12 @@ int ltr_nccl_allgather_clouds(ltr_ctx* ctx, int32_t comm, int32_t count, const l
     std::vector<std::vector<int64_t>> displs((size_t)count, std::vector<int64_t>((size_t)cc.world + 1, 0));
     for (int i = 0; i < count; ++i) {
         for (int r = 0; r < cc.world; ++r) displs[i][r + 1] = displs[i][r] + all[(size_t)r * count + i];
-        LTR_TRY(cloud_new(ctx, displs[i][cc.world], &out[i]));
+        LTR_TRY(cloud_new(ctx, displs[i][cc.world], &o[i]));
     }
     LTR_NCCL(ctx, a, a->GroupStart());
     for (int i = 0; i < count; ++i) {
         const DevCloud src = ctx->clouds[local[i]];
-        const DevCloud dst = ctx->clouds[out[i]];
+        const DevCloud dst = ctx->clouds[o[i].get()];
         const float* sp[4] = {src.x(), src.y(), src.z(), src.i()};
         float* dp[4] = {dst.x(), dst.y(), dst.z(), dst.i()};
         for (int r = 0; r < cc.world; ++r) {
@@ -291,11 +297,12 @@ int ltr_nccl_allgather_clouds(ltr_ctx* ctx, int32_t comm, int32_t count, const l
     LTR_NCCL(ctx, a, a->GroupEnd());
     for (int i = 0; i < count; ++i) {
         const DevCloud src = ctx->clouds[local[i]];
-        const DevCloud dst = ctx->clouds[out[i]];
+        const DevCloud dst = ctx->clouds[o[i].get()];
         if (src.n > 0)
             LTR_CUDA(ctx, cudaMemcpy2DAsync(dst.base + displs[i][cc.rank], (size_t)dst.cap * 4, src.base, (size_t)src.cap * 4, (size_t)src.n * 4, 4,
                                             cudaMemcpyDeviceToDevice, ctx->stream));
     }
+    for (int i = 0; i < count; ++i) out[i] = o[i].release();
     return LTR_OK;
 }
 
@@ -321,7 +328,8 @@ int ltr_nccl_exchange_clouds(ltr_ctx* ctx, int32_t comm, int32_t peer, int32_t n
     // also on a send-only side: the pinned staging slots h[0, n_send) are reused by the next count exchange on this communicator,
     // which must not overwrite them before the asynchronous upload above has read them
     LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    for (int i = 0; i < n_recv; ++i) LTR_TRY(cloud_new(ctx, h[kMaxBatch + i], &recv[i]));
+    std::vector<CloudOwner> o((size_t)n_recv);
+    for (int i = 0; i < n_recv; ++i) LTR_TRY(cloud_new(ctx, h[kMaxBatch + i], &o[i]));
     LTR_NCCL(ctx, a, a->GroupStart());
     for (int i = 0; i < n_send; ++i) {
         const DevCloud s = ctx->clouds[send[i]];
@@ -329,11 +337,12 @@ int ltr_nccl_exchange_clouds(ltr_ctx* ctx, int32_t comm, int32_t peer, int32_t n
         if (s.n > 0) for (int k = 0; k < 4; ++k) LTR_NCCL(ctx, a, a->Send(sp[k], (size_t)s.n, ncclFloat32, peer, nccl_of(cc), ctx->stream));
     }
     for (int i = 0; i < n_recv; ++i) {
-        const DevCloud r = ctx->clouds[recv[i]];
+        const DevCloud r = ctx->clouds[o[i].get()];
         float* rp[4] = {r.x(), r.y(), r.z(), r.i()};
         if (r.n > 0) for (int k = 0; k < 4; ++k) LTR_NCCL(ctx, a, a->Recv(rp[k], (size_t)r.n, ncclFloat32, peer, nccl_of(cc), ctx->stream));
     }
     LTR_NCCL(ctx, a, a->GroupEnd());
+    for (int i = 0; i < n_recv; ++i) recv[i] = o[i].release();
     return LTR_OK;
 }
 

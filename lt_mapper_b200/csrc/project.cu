@@ -874,7 +874,7 @@ int ltr_remove_pass_ball(ltr_ctx* ctx, ltr_cloud map_h, ltr_scanset scans_h, ltr
                        accumulate, n_dynamic);
 }
 
-// An overflowed run (*overflowed) frees its output again.
+// An overflowed run (*overflowed) frees its output again and leaves *out unwritten.
 static int parse_projected_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_poses poses_h, int32_t kf_begin, int32_t kf_end, float res_alpha, ltr_scanset* out,
                                 bool allow_deferred, bool* overflowed) {
     *overflowed = false;
@@ -956,8 +956,9 @@ static int parse_projected_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_poses poses_h
         if (h_over) *overflowed = true;
         for (int k = 0; k < K; ++k) off[k + 1] = off[k] + cnt[k];
     }
-    LTR_TRY(scanset_new(ctx, off, out));
-    DevScanSet& os = ctx->scansets[*out];
+    ScanSetOwner o;
+    LTR_TRY(scanset_new(ctx, off, &o));
+    DevScanSet& os = ctx->scansets[o.get()];
     if (os.pts.n > 0) {
         parse_emit_kernel<<<(unsigned)((os.pts.n + 255) / 256), 256, 0, ctx->stream>>>(view(mapc), posc.d, kf_begin, os.d_off, K, (const uint32_t*)p_list,
             (int)npx, ctx->d_ext, ctx->ext_identity ? 1 : 0, ctx->cfg.transform_order, os.pts);
@@ -968,7 +969,7 @@ static int parse_projected_impl(ltr_ctx* ctx, ltr_cloud map_h, ltr_poses poses_h
     LTR_CUDA(ctx, cudaEventRecord(ctx->ev1, ctx->stream));
     LTR_CUDA(ctx, cudaEventSynchronize(ctx->ev1));
     pass_end(ctx, p, 4, 12.0 * (double)mapc.n, mapc.n, K);
-    if (*overflowed) return ltr_scanset_free(ctx, *out);
+    if (!*overflowed) *out = o.release();
     return LTR_OK;
 }
 
@@ -1066,6 +1067,7 @@ int ltr_debug_fast_project(ltr_ctx* ctx, const float* xyz, int64_t n, const doub
     double id[16];
     for (int i = 0; i < 16; ++i) id[i] = (i % 5 == 0) ? 1.0 : 0.0;
     LTR_TRY(ltr_poses_upload(ctx, id, inv_pose16, 1, &ph));
+    PosesOwner g_ph(ctx, ph);
     const DevPoses pp = ctx->poses[ph];
     void* p = nullptr;
     ScratchGuard g_p(ctx, &p);
@@ -1079,8 +1081,7 @@ int ltr_debug_fast_project(ltr_ctx* ctx, const float* xyz, int64_t n, const doub
     LTR_LAUNCH_CHECK(ctx);
     LTR_CUDA(ctx, cudaMemcpyAsync(out8, d_out, (size_t)n * 32, cudaMemcpyDeviceToHost, ctx->stream));
     LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    g_p.release();
-    return ltr_poses_free(ctx, ph);
+    return LTR_OK;
 }
 
 }  // extern "C"

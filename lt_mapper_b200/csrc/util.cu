@@ -812,7 +812,7 @@ static int voxel_distributed(ltr_ctx* ctx, int comm, const DevCloud& loc, float 
     VoxBox b;
     int hb = 0, shift = 0;
     LTR_TRY(dist_decide_box(ctx, h_mm, leaf, &empty, &b, &hb, &shift));
-    if (empty) return cloud_new(ctx, 0, out_h);    // every rank's cloud is empty
+    if (empty) { CloudOwner h; LTR_TRY(cloud_new(ctx, 0, &h)); *out_h = h.release(); return LTR_OK; }   // every rank's cloud is empty
     // B. local keys + prefix histogram, summed over the ranks
     uint32_t* d_hist_loc = d_mm + 8;
     uint32_t* d_hist_glb = d_hist_loc + kDistHistWords;
@@ -829,20 +829,20 @@ static int voxel_distributed(ltr_ctx* ctx, int comm, const DevCloud& loc, float 
     DestCuts cuts;
     std::vector<int64_t> scount;
     LTR_TRY(dist_plan(ctx, h_hist.data(), h_hist.data() + kDistHistWords, nbins, G, &cuts, &scount));
-    CloudOwner g_send(ctx), g_recv(ctx), g_slice(ctx);
-    LTR_TRY(cloud_new(ctx, lv.n, &g_send.h));
-    LTR_TRY(dist_stage_group(ctx, lv, p, shift, cuts, ctx->clouds[g_send.h]));
+    CloudOwner g_send, g_recv, g_slice;
+    LTR_TRY(cloud_new(ctx, lv.n, &g_send));
+    LTR_TRY(dist_stage_group(ctx, lv, p, shift, cuts, ctx->clouds[g_send.get()]));
     g_p.release();
-    LTR_TRY(nccl_alltoallv_cloud(ctx, comm, ctx->clouds[g_send.h], scount, &g_recv.h));
+    LTR_TRY(nccl_alltoallv_cloud(ctx, comm, ctx->clouds[g_send.get()], scount, &g_recv));
     g_send.reset();
     // D. my range, with the GLOBAL box
-    const DevCloud recv = ctx->clouds[g_recv.h];
-    LTR_TRY(cloud_new(ctx, recv.n, &g_slice.h));
-    DevCloud slice = ctx->clouds[g_slice.h];
+    const DevCloud recv = ctx->clouds[g_recv.get()];
+    LTR_TRY(cloud_new(ctx, recv.n, &g_slice));
+    DevCloud slice = ctx->clouds[g_slice.get()];
     LTR_TRY(voxel_view(ctx, view(recv), leaf, &slice, &b));
-    ctx->clouds[g_slice.h].n = slice.n;
+    ctx->clouds[g_slice.get()].n = slice.n;
     // slices in range order == octree order
-    const ltr_cloud local[1] = {g_slice.h};
+    const ltr_cloud local[1] = {g_slice.get()};
     return ltr_nccl_allgather_clouds(ctx, comm, 1, local, out_h);
 }
 
@@ -871,7 +871,7 @@ static int voxel_distributed_simulated(ltr_ctx* ctx, int G, const ltr_cloud* loc
     LTR_TRY(dist_decide_box(ctx, mm, leaf, &empty, &b, &hb, &shift));
     if (cuts_out) for (int j = 0; j < G - 1; ++j) cuts_out[j] = 0;
     if (send_counts) for (int j = 0; j < G * G; ++j) send_counts[j] = 0;
-    if (empty) return cloud_new(ctx, 0, out_h);
+    if (empty) { CloudOwner h; LTR_TRY(cloud_new(ctx, 0, &h)); *out_h = h.release(); return LTR_OK; }
     // B
     const int nbins = 1 << hb;
     std::vector<uint32_t> hl((size_t)G * kDistHistWords), hg((size_t)kDistHistWords, 0u);
@@ -889,20 +889,20 @@ static int voxel_distributed_simulated(ltr_ctx* ctx, int G, const ltr_cloud* loc
     for (int r = 0; r < G; ++r) LTR_TRY(dist_plan(ctx, &hl[(size_t)r * kDistHistWords], hg.data(), nbins, G, &cuts, &scount[(size_t)r]));
     std::deque<CloudOwner> send, recv, slice;
     for (int r = 0; r < G; ++r) {
-        send.emplace_back(ctx);
-        LTR_TRY(cloud_new(ctx, lv[(size_t)r].n, &send.back().h));
-        LTR_TRY(dist_stage_group(ctx, lv[(size_t)r], p_keys[(size_t)r], shift, cuts, ctx->clouds[send.back().h]));
+        send.emplace_back();
+        LTR_TRY(cloud_new(ctx, lv[(size_t)r].n, &send.back()));
+        LTR_TRY(dist_stage_group(ctx, lv[(size_t)r], p_keys[(size_t)r], shift, cuts, ctx->clouds[send.back().get()]));
     }
     guards.clear();
     for (int d = 0; d < G; ++d) {
         int64_t m = 0;
         for (int r = 0; r < G; ++r) m += scount[(size_t)r][(size_t)d];
-        recv.emplace_back(ctx);
-        LTR_TRY(cloud_new(ctx, m, &recv.back().h));
-        const DevCloud dst = ctx->clouds[recv.back().h];
+        recv.emplace_back();
+        LTR_TRY(cloud_new(ctx, m, &recv.back()));
+        const DevCloud dst = ctx->clouds[recv.back().get()];
         int64_t at = 0;
         for (int r = 0; r < G; ++r) {
-            const DevCloud src = ctx->clouds[send[(size_t)r].h];
+            const DevCloud src = ctx->clouds[send[(size_t)r].get()];
             int64_t from = 0;
             for (int e = 0; e < d; ++e) from += scount[(size_t)r][(size_t)e];
             const int64_t k = scount[(size_t)r][(size_t)d];
@@ -915,20 +915,20 @@ static int voxel_distributed_simulated(ltr_ctx* ctx, int G, const ltr_cloud* loc
     // D
     int64_t total = 0;
     for (int d = 0; d < G; ++d) {
-        const DevCloud rc = ctx->clouds[recv[(size_t)d].h];
-        slice.emplace_back(ctx);
-        LTR_TRY(cloud_new(ctx, rc.n, &slice.back().h));
-        DevCloud s = ctx->clouds[slice.back().h];
+        const DevCloud rc = ctx->clouds[recv[(size_t)d].get()];
+        slice.emplace_back();
+        LTR_TRY(cloud_new(ctx, rc.n, &slice.back()));
+        DevCloud s = ctx->clouds[slice.back().get()];
         LTR_TRY(voxel_view(ctx, view(rc), leaf, &s, &b));
-        ctx->clouds[slice.back().h].n = s.n;
+        ctx->clouds[slice.back().get()].n = s.n;
         total += s.n;
     }
-    CloudOwner g_out(ctx);
-    LTR_TRY(cloud_new(ctx, total, &g_out.h));
-    const DevCloud o = ctx->clouds[g_out.h];
+    CloudOwner g_out;
+    LTR_TRY(cloud_new(ctx, total, &g_out));
+    const DevCloud o = ctx->clouds[g_out.get()];
     int64_t at = 0;
     for (int d = 0; d < G; ++d) {
-        const DevCloud s = ctx->clouds[slice[(size_t)d].h];
+        const DevCloud s = ctx->clouds[slice[(size_t)d].get()];
         if (s.n > 0) LTR_CUDA(ctx, cudaMemcpy2DAsync(o.base + at, (size_t)o.cap * 4, s.base, (size_t)s.cap * 4, (size_t)s.n * 4, 4,
                                                      cudaMemcpyDeviceToDevice, ctx->stream));
         at += s.n;
@@ -936,8 +936,7 @@ static int voxel_distributed_simulated(ltr_ctx* ctx, int G, const ltr_cloud* loc
     LTR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     if (cuts_out) for (int j = 0; j < G - 1; ++j) cuts_out[j] = cuts.ub[j];
     if (send_counts) for (int r = 0; r < G; ++r) for (int d = 0; d < G; ++d) send_counts[r * G + d] = scount[(size_t)r][(size_t)d];
-    *out_h = g_out.h;
-    g_out.h = -1;
+    *out_h = g_out.release();
     return LTR_OK;
 }
 
@@ -984,13 +983,13 @@ int ScanSplit::init() {
 
 int ScanSplit::relocalise(int64_t base, int64_t n, const float* gx, const float* gy, const float* gz) {
     if (n == 0) return LTR_OK;
-    if (reloc_.h < 0) {
-        LTR_TRY(cloud_new(ctx_, scans_.pts.n, &reloc_.h));
-        LTR_CUDA(ctx_, cudaMemcpyAsync(ctx_->clouds[reloc_.h].i(), scans_.pts.i(), (size_t)scans_.pts.n * sizeof(float), cudaMemcpyDeviceToDevice,
+    if (reloc_.get() < 0) {
+        LTR_TRY(cloud_new(ctx_, scans_.pts.n, &reloc_));
+        LTR_CUDA(ctx_, cudaMemcpyAsync(ctx_->clouds[reloc_.get()].i(), scans_.pts.i(), (size_t)scans_.pts.n * sizeof(float), cudaMemcpyDeviceToDevice,
                                        ctx_->stream));
     }
     global_to_scans_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx_->stream>>>(gx, gy, gz, scans_.d_off, scans_.K, base, n, poses_,
-        ctx_->ext_identity ? nullptr : ctx_->d_ext, ctx_->cfg.transform_order, ctx_->clouds[reloc_.h]);
+        ctx_->ext_identity ? nullptr : ctx_->d_ext, ctx_->cfg.transform_order, ctx_->clouds[reloc_.get()]);
     LTR_LAUNCH_CHECK(ctx_);
     return LTR_OK;
 }
@@ -998,12 +997,15 @@ int ScanSplit::relocalise(int64_t base, int64_t n, const float* gx, const float*
 int ScanSplit::finish(ltr_scanset* out0, ltr_scanset* out1) {
     if (scans_.pts.n == 0) {
         const std::vector<int64_t> off((size_t)scans_.K + 1, 0);
-        if (out0) LTR_TRY(scanset_new(ctx_, off, out0));
-        if (out1) LTR_TRY(scanset_new(ctx_, off, out1));
+        ScanSetOwner o0, o1;
+        if (out0) LTR_TRY(scanset_new(ctx_, off, &o0));
+        if (out1) LTR_TRY(scanset_new(ctx_, off, &o1));
+        if (out0) *out0 = o0.release();
+        if (out1) *out1 = o1.release();
         return LTR_OK;
     }
     DevScanSet set = scans_;
-    set.pts = ctx_->clouds[reloc_.h];
+    set.pts = ctx_->clouds[reloc_.get()];
     return split_scanset_by_flag(ctx_, set, flags, out0, out1);
 }
 
@@ -1072,20 +1074,20 @@ int split_scanset_by_flag(ltr_ctx* ctx, const DevScanSet& in_ref, const uint8_t*
         off1[k + 1] = off1[k] + cnt[k];
         off0[k + 1] = off0[k] + (in.h_off[k + 1] - in.h_off[k]) - cnt[k];
     }
-    ltr_scanset h0, h1;
+    ScanSetOwner h0, h1;   // an output the caller does not take is freed on return
     const DevCloud src = in.pts;  // copy: the table may be reallocated by scanset_new
     LTR_TRY(scanset_new(ctx, off0, &h0));
     LTR_TRY(scanset_new(ctx, off1, &h1));
     // a global stable partition keeps keyframe order, so it lands exactly at the per-keyframe offsets
-    DevCloud o0 = ctx->scansets[h0].pts, o1 = ctx->scansets[h1].pts;
+    DevCloud o0 = ctx->scansets[h0.get()].pts, o1 = ctx->scansets[h1.get()].pts;
     if (src.n > 0) {
         // outputs may be smaller than src.n in capacity only by construction of sizes: they are exact
         int64_t nf = 0;
         LTR_TRY(stable_partition_by_flag(ctx, src, flags, &nf, &o0, &o1));
         if (nf != off1[in.K]) return fail(ctx, LTR_ERR_CUDA, "internal: partition count mismatch");
     }
-    if (out_unflagged) *out_unflagged = h0; else ltr_scanset_free(ctx, h0);
-    if (out_flagged) *out_flagged = h1; else ltr_scanset_free(ctx, h1);
+    if (out_unflagged) *out_unflagged = h0.release();
+    if (out_flagged) *out_flagged = h1.release();
     return LTR_OK;
 }
 
@@ -1101,11 +1103,12 @@ int ltr_voxel_centroid(ltr_ctx* ctx, ltr_cloud in, float leaf, ltr_cloud* out) {
     DevCloud* c;
     LTR_TRY(cloud_get(ctx, in, &c));
     const DevCloud src = *c;
-    LTR_TRY(cloud_new(ctx, src.n, out));
-    DevCloud o = ctx->clouds[*out];
-    const int rc = voxel_view(ctx, view(src), leaf, &o);
-    if (rc != LTR_OK) { cloud_release(ctx, &ctx->clouds[*out]); return rc; }
-    ctx->clouds[*out].n = o.n;
+    CloudOwner h;
+    LTR_TRY(cloud_new(ctx, src.n, &h));
+    DevCloud o = ctx->clouds[h.get()];
+    LTR_TRY(voxel_view(ctx, view(src), leaf, &o));
+    ctx->clouds[h.get()].n = o.n;
+    *out = h.release();
     return LTR_OK;
 }
 
@@ -1134,25 +1137,25 @@ int ltr_voxel_centroid_per_keyframe(ltr_ctx* ctx, ltr_scanset in, float leaf, lt
     const std::vector<int64_t> off = s->h_off;
     const int K = s->K;
     // worst case every point survives: voxelise into a scratch of the input layout, then compact
-    ltr_cloud scratch;
+    CloudOwner scratch;
     LTR_TRY(cloud_new(ctx, src.n, &scratch));
-    const DevCloud sc = ctx->clouds[scratch];
+    const DevCloud sc = ctx->clouds[scratch.get()];
     std::vector<int64_t> noff((size_t)K + 1, 0);
     for (int k = 0; k < K; ++k) {
         PtrView v{src.x() + off[k], src.y() + off[k], src.z() + off[k], src.i() + off[k], off[k + 1] - off[k]};
         DevCloud o = sc;
         o.base = sc.base + off[k];  // component stride stays sc.cap
-        const int rc = voxel_view(ctx, v, leaf, &o);
-        if (rc != LTR_OK) { ltr_cloud_free(ctx, scratch); return rc; }
+        LTR_TRY(voxel_view(ctx, v, leaf, &o));
         noff[k + 1] = noff[k] + o.n;
     }
-    LTR_TRY(scanset_new(ctx, noff, out));
-    DevCloud& d = ctx->scansets[*out].pts;
+    ScanSetOwner h;
+    LTR_TRY(scanset_new(ctx, noff, &h));
+    DevCloud& d = ctx->scansets[h.get()].pts;
     for (int k = 0; k < K; ++k) {
         const int64_t m = noff[k + 1] - noff[k];
         if (m > 0) LTR_CUDA(ctx, cudaMemcpy2DAsync(d.base + noff[k], (size_t)d.cap * 4, sc.base + off[k], (size_t)sc.cap * 4, (size_t)m * 4, 4, cudaMemcpyDeviceToDevice, ctx->stream));
     }
-    ltr_cloud_free(ctx, scratch);
+    *out = h.release();
     return LTR_OK;
 }
 
@@ -1166,10 +1169,13 @@ int ltr_merge_scans_global(ltr_ctx* ctx, ltr_scanset scans, ltr_poses poses, ltr
     if (p->K != s->K) return fail(ctx, LTR_ERR_INVALID, "pose count %d != keyframe count %d (Session.cpp:117)", p->K, s->K);
     const DevScanSet ss = *s;
     const DevPoses pp = *p;
-    LTR_TRY(cloud_new(ctx, ss.pts.n, out));
+    CloudOwner h;
+    LTR_TRY(cloud_new(ctx, ss.pts.n, &h));
     // mergeScansWithinGlobalCoordUtil (utility.cpp:170-192): lidar2base, then the pose
-    const DevCloud o = ctx->clouds[*out];
-    return scans_to_global(ctx, ss, 0, ss.pts.n, pp.d, ctx->ext_identity ? nullptr : ctx->d_ext + 12, o.x(), o.y(), o.z(), o.i());
+    const DevCloud o = ctx->clouds[h.get()];
+    LTR_TRY(scans_to_global(ctx, ss, 0, ss.pts.n, pp.d, ctx->ext_identity ? nullptr : ctx->d_ext + 12, o.x(), o.y(), o.z(), o.i()));
+    *out = h.release();
+    return LTR_OK;
 }
 
 int ltr_preclean(ltr_ctx* ctx, ltr_scanset scans, float radius, ltr_scanset* out) {
@@ -1229,13 +1235,16 @@ int ltr_apply_partition(ltr_ctx* ctx, ltr_cloud map, ltr_cloud* out_static, ltr_
     if (c->n == 1 || c->n == 2) return fail(ctx, LTR_ERR_UNSUPPORTED, "maps of 1 or 2 points hit undefined behaviour in the reference (utility.h:158-167)");
     LTR_TRY(cloud_ensure_flags(ctx, c));
     const DevCloud src = *c;
-    LTR_TRY(cloud_new(ctx, src.n, out_static));
-    LTR_TRY(cloud_new(ctx, src.n, out_dynamic));
-    DevCloud o0 = ctx->clouds[*out_static], o1 = ctx->clouds[*out_dynamic];
+    CloudOwner st, dy;
+    LTR_TRY(cloud_new(ctx, src.n, &st));
+    LTR_TRY(cloud_new(ctx, src.n, &dy));
+    DevCloud o0 = ctx->clouds[st.get()], o1 = ctx->clouds[dy.get()];
     int64_t nf = 0;
     LTR_TRY(stable_partition_by_flag(ctx, src, src.flags, &nf, &o0, &o1));
-    ctx->clouds[*out_static].n = o0.n;
-    ctx->clouds[*out_dynamic].n = o1.n;
+    ctx->clouds[st.get()].n = o0.n;
+    ctx->clouds[dy.get()].n = o1.n;
+    *out_static = st.release();
+    *out_dynamic = dy.release();
     return LTR_OK;
 }
 

@@ -420,7 +420,7 @@ static int voxel_grid_run(ltr_ctx* ctx, const PtrView& src, const std::vector<in
     max_chunk = std::max(max_chunk, std::min<int64_t>(off[K], env_points("LTR_VOXEL_GRID_CHUNK_POINTS", kVgChunkPoints, kVgChunkPoints)));
     void *p_ent = nullptr, *p_pos = nullptr, *p_segs = nullptr, *p_cnt = nullptr, *p_status = nullptr, *p_oo = nullptr;
     ScratchGuard g_ent(ctx, &p_ent), g_pos(ctx, &p_pos), g_segs(ctx, &p_segs), g_cnt(ctx, &p_cnt), g_status(ctx, &p_status), g_oo(ctx, &p_oo);
-    CloudOwner g_sc(ctx);
+    CloudOwner g_sc;
     const size_t nk = (size_t)std::max(K, 1);
     LTR_TRY(dev_alloc(ctx, &p_cnt, nk * sizeof(int64_t)));
     LTR_TRY(dev_alloc(ctx, &p_status, nk * sizeof(int32_t)));
@@ -429,9 +429,9 @@ static int voxel_grid_run(ltr_ctx* ctx, const PtrView& src, const std::vector<in
         LTR_TRY(dev_alloc(ctx, &p_ent, (size_t)max_chunk * sizeof(uint64_t)));
         LTR_TRY(dev_alloc(ctx, &p_pos, (size_t)max_chunk * 2 * sizeof(uint32_t)));
         LTR_TRY(dev_alloc(ctx, &p_segs, (size_t)max_chunk * sizeof(uint64_t)));
-        LTR_TRY(cloud_new(ctx, off[K], &g_sc.h));
+        LTR_TRY(cloud_new(ctx, off[K], &g_sc));
     }
-    const DevCloud sc = g_sc.h >= 0 ? ctx->clouds[g_sc.h] : DevCloud();
+    const DevCloud sc = g_sc.get() >= 0 ? ctx->clouds[g_sc.get()] : DevCloud();
     for (int k0 = 0; k0 < K;) {
         int k1 = k0 + 1;
         while (k1 < K && off[k1 + 1] - off[k0] <= max_chunk) ++k1;
@@ -481,14 +481,13 @@ int ltr_voxel_grid(ltr_ctx* ctx, ltr_cloud in, float leaf, ltr_cloud* out, int32
     LTR_TRY(dev_alloc(ctx, &p_off, 2 * sizeof(int64_t)));
     LTR_CUDA(ctx, cudaMemcpyAsync(p_off, off.data(), 2 * sizeof(int64_t), cudaMemcpyHostToDevice, ctx->stream));
     int32_t nov = 0;
-    ltr_cloud h = -1;
-    const int rc = voxel_grid_run(ctx, view(src), off, (const int64_t*)p_off, leaf, &nov, [&](const std::vector<int64_t>& oo, DevCloud* o) {
+    CloudOwner h;
+    LTR_TRY(voxel_grid_run(ctx, view(src), off, (const int64_t*)p_off, leaf, &nov, [&](const std::vector<int64_t>& oo, DevCloud* o) {
         LTR_TRY(cloud_new(ctx, oo[1], &h));
-        *o = ctx->clouds[h];
+        *o = ctx->clouds[h.get()];
         return (int)LTR_OK;
-    });
-    if (rc != LTR_OK) { if (h >= 0) ltr_cloud_free(ctx, h); return rc; }
-    *out = h;
+    }));
+    *out = h.release();
     if (overflowed) *overflowed = nov;
     return LTR_OK;
 }
@@ -499,14 +498,13 @@ int ltr_voxel_grid_per_keyframe(ltr_ctx* ctx, ltr_scanset in, float leaf, ltr_sc
     DevScanSet* s;
     LTR_TRY(scanset_get(ctx, in, &s));
     const DevScanSet ss = *s;   // copy: scanset_new may reallocate the handle table
-    ltr_scanset h = -1;
-    const int rc = voxel_grid_run(ctx, view(ss.pts), ss.h_off, ss.d_off, leaf, n_overflowed, [&](const std::vector<int64_t>& oo, DevCloud* o) {
+    ScanSetOwner h;
+    LTR_TRY(voxel_grid_run(ctx, view(ss.pts), ss.h_off, ss.d_off, leaf, n_overflowed, [&](const std::vector<int64_t>& oo, DevCloud* o) {
         LTR_TRY(scanset_new(ctx, oo, &h));
-        *o = ctx->scansets[h].pts;
+        *o = ctx->scansets[h.get()].pts;
         return (int)LTR_OK;
-    });
-    if (rc != LTR_OK) { if (h >= 0) ltr_scanset_free(ctx, h); return rc; }
-    *out = h;
+    }));
+    *out = h.release();
     return LTR_OK;
 }
 

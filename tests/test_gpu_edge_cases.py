@@ -153,10 +153,14 @@ def test_error_paths_release_their_scratch_memory(ctx):
     ss = ctx.scanset_upload(good[:1000], [0, 400, 1000])
     ps = ctx.poses_upload(np.stack([I4, I4]), np.stack([I4, I4]))
     tiny = ctx.cloud_upload(good[:0])                          # an empty kNN target is rejected (PCL asserts on an empty tree)
+    ss_bad = ctx.scanset_upload(bad[:2000], [0, 1000, 2000])   # the non-finite point lies in the second keyframe
     base = ctx.memory_stats()[0]
     for _ in range(3):
         with pytest.raises(ltr.LtrError):
             ctx.voxel_centroid(hb, 0.1)                       # fails after the output cloud, keys and scratch were allocated
+        with pytest.raises(ltr.LtrError) as e:
+            ctx.voxel_centroid_per_keyframe(ss_bad, 0.1)      # fails after the first keyframe was voxelised into the scratch cloud
+        assert e.value.code == -3
         with pytest.raises(ltr.LtrError):
             ctx.knn_diff(ss, ps, tiny, 2, 0.01)
         with pytest.raises(ltr.LtrError):
