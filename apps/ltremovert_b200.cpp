@@ -5,8 +5,8 @@
 // on the GPU through libltr_removert/libltr_b200, and writes the same output tree (Removerter.cpp:26-50, 231, 1446-1477,
 // 1517-1520, 1600-1601, 1607-1650).  No ROS, no PCL; rviz publishing is dropped (side effect only).
 //
-//   ltremovert_b200 --config params.yaml [--selfremovert] [--pcl110] [--no-split] [--clean-scans[=map|scan-minus-map]] [--icp-refinement]
-//                   [--adaptive-threshold[=c]] [--map-ball[=R]]
+//   ltremovert_b200 --config params.yaml [--selfremovert] [--pcl110] [--no-split] [--clean-scans[=map|scan-minus-map]]
+//                   [--clean-scans-between[=map|scan-minus-map]] [--icp-refinement] [--adaptive-threshold[=c]] [--map-ball[=R]]
 //     --selfremovert   run selfRemovert over remove_resolution_list (Removerter.cpp:1378-1393) instead of the shipped
 //                      single removeOnce(2.5) (Removerter.cpp:1584, 1587)
 //     --pcl110         PCL >= 1.10 transformPointCloud summation order (ltr_config.transform_order = 1)
@@ -16,6 +16,13 @@
 //                      input scan's name (saveCleanedScans, :1143-1195), and with saveMapPCD the merged, 0.05-voxelised maps of
 //                      saveMapPointcloudByMergingCleanedScans (:1197-1251) to map_static/ and map_dynamic/.  Off by default: without it
 //                      the output tree is the one the node writes.
+//     --clean-scans-between  after Step 3, scansideRemovalForEachScan (C,Q) and (Q,C) with isFineRegistration (Removerter.cpp:1256-1261,
+//                      1295-1297; removeDynamicPointsOfScanByKnnBtnSession, :950-1017, commented out in the reference): each keyframe is
+//                      registered to the other session's 0.4 m static map and split registered when its fitness is below 1.0, with the
+//                      criterion of --clean-scans.  Writes every keyframe's parts under the input scan's name to
+//                      scan_static/query_vs_central/ and scan_dynamic/query_vs_central/ (scan-level PD) and scan_static/central_vs_query/
+//                      and scan_dynamic/central_vs_query/ (scan-level ND); prints one summary line (keyframes accepted, median
+//                      iterations).  Combines with --clean-scans; off by default.
 //     --icp-refinement Step 2's kNN diff registers every keyframe to the other session's 0.4 m map first and keeps the registered scan
 //                      when its fitness is below 1.0 (partitionLowDynamicPointsOfScanByKnn's `useICPrefinement`, Session.cpp:549-584,
 //                      off in the reference); prints one summary line (keyframes accepted, median iterations).  The output tree keeps
@@ -31,8 +38,8 @@
 //                      (the changes since the first listed run) and composed/scans_restored/ (the central scans as the first listed run
 //                      found them) under save_pcd_directory, and with saveMapPCD composed/restored_map.pcd.  The yaml's query session
 //                      must still list (its scan directory and pose file are read for the keyframe selection), but none of its scans
-//                      is loaded.  The Step 0-3 options (--selfremovert, --clean-scans, --icp-refinement, --adaptive-threshold,
-//                      --map-ball) are rejected with it.  Every listed file is checked on every rank before any collective.
+//                      is loaded.  The Step 0-3 options (--selfremovert, --clean-scans, --clean-scans-between, --icp-refinement,
+//                      --adaptive-threshold, --map-ball) are rejected with it.  Every listed file is checked on every rank before any collective.
 //     --map-ball       every removeOnce / revertOnce projects, per keyframe, only the map points within R m of the keyframe's pose (the
 //                      reference's kUseSubsetMapCloud / kBallSize, Removerter.h:46-48, off there; takeGlobalMapSubsetWithinBall,
 //                      Removerter.cpp:415-427); R defaults to the reference's 80 and must be finite and > 0.  The ND / PD filter passes and
@@ -141,10 +148,12 @@ int main(int argc, char** argv) {
     std::string cfg_path;
     bool selfremovert = false, pcl110 = false, no_split = false;
     int clean_scans = -1;   // -1 off, else ltr_scanside_criterion
+    int clean_between = -1;   // the same for the registered (C,Q) / (Q,C) removal
     bool icp_refinement = false;
     float adaptive_c = 0.0f;   // 0: the constant threshold
     float ball_r = 0.0f;       // 0: the full map
-    const char* usage = "usage: %s --config params.yaml [--selfremovert] [--pcl110] [--no-split] [--clean-scans[=map|scan-minus-map]] [--icp-refinement]"
+    const char* usage = "usage: %s --config params.yaml [--selfremovert] [--pcl110] [--no-split] [--clean-scans[=map|scan-minus-map]]"
+                        " [--clean-scans-between[=map|scan-minus-map]] [--icp-refinement]"
                         " [--adaptive-threshold[=c], 0 < c < 1] [--map-ball[=R], R > 0] [--compose=<gen_dir>[,<gen_dir>...]]\n";
     std::vector<std::string> compose_dirs;   // --compose: output trees of earlier runs, oldest first
     for (int i = 1; i < argc; ++i) {
@@ -154,6 +163,8 @@ int main(int argc, char** argv) {
         else if (!std::strcmp(argv[i], "--no-split")) no_split = true;
         else if (!std::strcmp(argv[i], "--clean-scans") || !std::strcmp(argv[i], "--clean-scans=map")) clean_scans = LTR_SCANSIDE_MAP;
         else if (!std::strcmp(argv[i], "--clean-scans=scan-minus-map")) clean_scans = LTR_SCANSIDE_SCAN_MINUS_MAP;
+        else if (!std::strcmp(argv[i], "--clean-scans-between") || !std::strcmp(argv[i], "--clean-scans-between=map")) clean_between = LTR_SCANSIDE_MAP;
+        else if (!std::strcmp(argv[i], "--clean-scans-between=scan-minus-map")) clean_between = LTR_SCANSIDE_SCAN_MINUS_MAP;
         else if (!std::strcmp(argv[i], "--icp-refinement")) icp_refinement = true;
         else if (!std::strcmp(argv[i], "--adaptive-threshold")) adaptive_c = 0.05f;
         else if (!std::strcmp(argv[i], "--map-ball")) ball_r = 80.0f;
@@ -181,9 +192,9 @@ int main(int argc, char** argv) {
         else { std::fprintf(stderr, usage, argv[0]); return 2; }
     }
     if (cfg_path.empty()) { std::fprintf(stderr, usage, argv[0]); return 2; }
-    if (!compose_dirs.empty() && (selfremovert || clean_scans >= 0 || icp_refinement || adaptive_c != 0.0f || ball_r != 0.0f)) {
-        std::fprintf(stderr, "--compose runs no Step 0-3: --selfremovert, --clean-scans, --icp-refinement, --adaptive-threshold and --map-ball "
-                             "cannot be combined with it\n");
+    if (!compose_dirs.empty() && (selfremovert || clean_scans >= 0 || clean_between >= 0 || icp_refinement || adaptive_c != 0.0f || ball_r != 0.0f)) {
+        std::fprintf(stderr, "--compose runs no Step 0-3: --selfremovert, --clean-scans, --clean-scans-between, --icp-refinement, "
+                             "--adaptive-threshold and --map-ball cannot be combined with it\n");
         return 2;
     }
     const int rank = env_int("RANK", 0), world = std::max(1, env_int("WORLD_SIZE", 1));
@@ -333,17 +344,15 @@ int main(int argc, char** argv) {
     R.mapBallRadius_ = ball_r;   // checked above
     if (ball_r != 0.0f && rank == 0)
         std::printf(" Map ball: radius %g m, each removeOnce / revertOnce keyframe projects only the map points within it\n", (double)ball_r);
-    ck(R.run_step0(), "Step 0");
-    R.useICPrefinement_ = icp_refinement;
-    ck(R.run_step12(), "Step 1-2");
-    if (icp_refinement) {
-        // over both sessions and every rank: [0, kMaxIt] iteration histogram, accepted, keyframes
+    // one summary line of registrations over both sessions and every rank (a collective: every rank calls it)
+    auto icp_summary = [&](const char* what, const IcpStats& a, const IcpStats& b) {
+        // [0, kMaxIt] iteration histogram, accepted, keyframes
         constexpr int kMaxIt = 100;
         std::vector<int64_t> h(kMaxIt + 3, 0);
-        for (const Session* X : {&R.central_sess_, &R.query_sess_})
-            for (size_t k = 0; k < X->icp_iterations_.size(); ++k) {
-                h[(size_t)std::min(std::max(X->icp_iterations_[k], 0), kMaxIt)]++;
-                h[kMaxIt + 1] += X->icp_accepted_[k];
+        for (const IcpStats* X : {&a, &b})
+            for (size_t k = 0; k < X->iterations.size(); ++k) {
+                h[(size_t)std::min(std::max(X->iterations[k], 0), kMaxIt)]++;
+                h[kMaxIt + 1] += X->accepted[k];
                 h[kMaxIt + 2]++;
             }
         if (world > 1 && R.nccl_world >= 0) {
@@ -354,9 +363,13 @@ int main(int argc, char** argv) {
         int median = 0;
         for (int64_t seen = 0; median <= kMaxIt; ++median) { seen += h[(size_t)median]; if (2 * seen > h[kMaxIt + 2] - 1) break; }
         if (rank == 0)
-            std::printf(" ICP refinement: %lld of %lld keyframes accepted, median iterations %d\n", (long long)h[kMaxIt + 1], (long long)h[kMaxIt + 2],
+            std::printf(" %s: %lld of %lld keyframes accepted, median iterations %d\n", what, (long long)h[kMaxIt + 1], (long long)h[kMaxIt + 2],
                         h[kMaxIt + 2] ? median : 0);
-    }
+    };
+    ck(R.run_step0(), "Step 0");
+    R.useICPrefinement_ = icp_refinement;
+    ck(R.run_step12(), "Step 1-2");
+    if (icp_refinement) icp_summary("ICP refinement", R.central_sess_.icp_, R.query_sess_.icp_);
     ck(R.run_step3(), "Step 3");
     if (rank == 0) for (const auto& l : R.log)
         std::printf(" %-18s map %lld  dynamic %lld  -> static %lld  dynamic %lld\n", l.what.c_str(), (long long)l.n_map, (long long)l.n_dynamic,
@@ -404,6 +417,24 @@ int main(int argc, char** argv) {
                 }
             }
         }
+    }
+    if (clean_between >= 0) {
+        // (map, scan) = (C,Q): the query's scans against the central map, scan-level PD; (Q,C): the central's against the query map, ND
+        for (int scan_sess = 1; scan_sess >= 0; --scan_sess) {
+            Session& X = scan_sess == 0 ? R.central_sess_ : R.query_sess_;
+            Session& M = scan_sess == 0 ? R.query_sess_ : R.central_sess_;
+            const LoadedSession& L = scan_sess == 0 ? C : Q;
+            const std::string name = scan_sess == 0 ? "central_vs_query" : "query_vs_central";
+            ck(R.scansideRemovalForEachScan(M, X, clean_between, true), "scansideRemovalForEachScan (fine registration)");
+            if (R.owns(X)) {
+                const std::string ds = save_dir + "scan_static/" + name, dd = save_dir + "scan_dynamic/" + name;
+                fsmkdir(ds);
+                fsmkdir(dd);
+                ok &= save_scans(R, X.scans_static_, L.keyframe_names, ds, false);
+                ok &= save_scans(R, X.scans_dynamic_, L.keyframe_names, dd, false);
+            }
+        }
+        icp_summary("Scan-side registration", R.central_sess_.scanside_icp_, R.query_sess_.scanside_icp_);
     }
     if (world > 1 && R.nccl_world >= 0) ltr_nccl_barrier(R.ctx, R.nccl_world);   // nobody leaves before everybody's files are written
     if (rank == 0) std::printf(" outputs written to %s (%s)\n", save_dir.c_str(), ok ? "ok" : "WITH ERRORS");

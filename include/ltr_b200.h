@@ -270,6 +270,21 @@ int ltr_icp_refine(ltr_ctx* ctx, ltr_scanset scans, ltr_poses poses, int32_t pos
  * entries (the reference accepts iff fitness < 1.0, Session.cpp:571). */
 int ltr_knn_diff_refined(ltr_ctx* ctx, ltr_scanset scans, ltr_poses poses, int32_t pose_offset, ltr_cloud target, int32_t k, float thr,
                          const float* T16, const uint8_t* accepted, ltr_scanset* out_coexist, ltr_scanset* out_diff);
+/* The fine registration of scan-side removal between sessions (removeDynamicPointsOfScanByKnnBtnSession, Removerter.cpp:950-1017, and its
+ * isFineRegistration set-up, :1263-1268, 1295-1297, 1325-1331; commented out in the reference): ltr_icp_refine with step 1 replaced by the
+ * way ltr_scanside_split moves a scan, local2global(scan_k, pose, lidar2base) (utility.cpp:160-168).  Same arguments, outputs, errors and
+ * chunking as ltr_icp_refine; with the identity extrinsic the two return the same bytes. */
+int ltr_icp_refine_scanside(ltr_ctx* ctx, ltr_scanset scans, ltr_poses poses, int32_t pose_offset, ltr_cloud target_down,
+                            const ltr_icp_params* params, float* T16_out, double* fitness_out, int32_t* iterations_out, int32_t* exit_out);
+/* ltr_scanside_split with the fine registration applied (Removerter.cpp:950-1017 under the accept rule of Session.cpp:571-579): the
+ * global points of keyframe k with accepted[k] != 0 are moved by T16[16k..16k+16) in f32 (((m0 x + m1 y) + m2 z) + m3) before the finite
+ * check and both searches, so "scan minus map" averages over the registered scan; both parts hold the registered points, moved back with
+ * global2local.  A keyframe with accepted[k] == 0 gives exactly ltr_scanside_split's bytes (the commented reference would search with the
+ * registered points even then; DESIGN.md §5.4).  T16 and accepted are host arrays of K entries, NULL with K > 0 is LTR_ERR_INVALID; the
+ * other errors, the chunking and ltr_scanside_stats are those of ltr_scanside_split. */
+int ltr_scanside_split_refined(ltr_ctx* ctx, ltr_scanset scans, ltr_poses poses, int32_t pose_offset, ltr_cloud map, int32_t criterion,
+                               int32_t k, float thr, const float* T16, const uint8_t* accepted, ltr_scanset* out_static,
+                               ltr_scanset* out_dynamic);
 
 /* ---- multi-GPU exchange points (NCCL, on the context's stream; libnccl is dlopen'ed at first use) ----------------
  * The path shards by keyframe: every per-keyframe loop of the reference (Removerter.cpp:429-593, Session.cpp:348-427) runs on the

@@ -112,6 +112,14 @@ int ltrh_rollback(ltrh_removerter* r, int32_t i);
  * scan-level positive / negative differences.  Valid after ltrh_run_step12 until ltrh_reset_to_step0 or ltrh_cascade_promote_updated
  * (which release the results).  Multi-GPU: each rank splits its own keyframe block; no collective. */
 int ltrh_scanside_removal(ltrh_removerter* r, int32_t map_sess, int32_t scan_sess, int32_t criterion);
+/* scansideRemovalForEachScan with isFineRegistration (Removerter.cpp:1295-1297; removeDynamicPointsOfScanByKnnBtnSession, :950-1017, both
+ * commented out in the reference): every keyframe of scan_sess held by this rank is registered by ltr_icp_refine_scanside (the reference's
+ * parameters, ltr_icp_params_default) to ltr_voxel_centroid(map_sess's map_global_curr_static_, 0.4), accepted iff its fitness is below 1.0
+ * (:978), and split by ltr_scanside_split_refined against the full static map with num_nn_points_within / dist_nn_points_within.  Results
+ * as ltrh_scanside_removal ("scans_static_" / "scans_dynamic_" of scan_sess, the same lifetime), the registration through
+ * ltrh_scanside_icp_stats.  Any session pair is accepted; (C,Q) / (Q,C) are the ones the reference registers.  Multi-GPU: each rank
+ * registers and splits its own keyframe block against its replica of the map; no collective. */
+int ltrh_scanside_removal_registered(ltrh_removerter* r, int32_t map_sess, int32_t scan_sess, int32_t criterion);
 /* Session::partitionLowDynamicPointsOfScanByKnn's ICP refinement (Session.cpp:549-584; `useICPrefinement`, false in the reference and by
  * default here).  With on != 0 every later detectLowDynamicPoints (ltrh_run_step12) registers each keyframe to the other session's map at
  * 0.4 m (ltr_icp_refine with the reference's parameters) and runs the kNN diff on the registered scan when its fitness is below 1.0
@@ -136,6 +144,11 @@ int ltrh_set_map_ball(ltrh_removerter* r, float radius);
  * and the accepted flag (fitness < 1.0).  Any array may be NULL. */
 int ltrh_icp_stats(ltrh_removerter* r, int32_t sess, int32_t capacity, int32_t* K_out, float* T16, double* fitness, int32_t* iterations,
                    int32_t* exit_reason, uint8_t* accepted);
+/* The same for the registration of the last scan-side removal of session `sess`'s scans on this rank (ltrh_scanside_removal_registered):
+ * *K_out = 0 when that removal ran without registration (ltrh_scanside_removal), and after ltrh_reset_to_step0 or
+ * ltrh_cascade_promote_updated.  Kept apart from ltrh_icp_stats: neither call changes what the other reports. */
+int ltrh_scanside_icp_stats(ltrh_removerter* r, int32_t sess, int32_t capacity, int32_t* K_out, float* T16, double* fitness, int32_t* iterations,
+                            int32_t* exit_reason, uint8_t* accepted);
 /* a single member function of Removerter by name, e.g. "removeHighDynamicPoints" */
 int ltrh_stage(ltrh_removerter* r, const char* name);
 

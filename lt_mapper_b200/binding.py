@@ -44,7 +44,7 @@ EXPORTS = [
     "ltr_scanset_free", "ltr_scanset_concat_per_keyframe", "ltr_scanset_flatten", "ltr_poses_upload", "ltr_poses_free",
     "ltr_preclean", "ltr_merge_scans_global", "ltr_voxel_centroid", "ltr_voxel_centroid_per_keyframe", "ltr_voxel_grid", "ltr_voxel_grid_per_keyframe", "ltr_remove_pass", "ltr_remove_pass_adaptive", "ltr_remove_pass_ball", "ltr_scan_images_release",
     "ltr_flags_device_ptr", "ltr_flags_download", "ltr_flags_upload", "ltr_apply_partition", "ltr_parse_projected",
-    "ltr_knn_diff", "ltr_knn_split_cloud", "ltr_knn_split_per_keyframe", "ltr_scanside_split", "ltr_scanside_stats", "ltr_icp_params_default", "ltr_icp_refine", "ltr_knn_diff_refined", "ltr_debug_pixel_index", "ltr_debug_scan_rimg", "ltr_debug_exact_knn_avg", "ltr_debug_nearest", "ltr_debug_fast_project", "ltr_debug_atan_sweep", "ltr_debug_margins", "ltr_debug_voxel_distributed", "ltr_reset_rimg_size", "ltr_last_pass_stats", "ltr_profile_get", "ltr_profile_reset", "ltr_timer_start", "ltr_timer_stop", "ltr_trace_dump",
+    "ltr_knn_diff", "ltr_knn_split_cloud", "ltr_knn_split_per_keyframe", "ltr_scanside_split", "ltr_scanside_stats", "ltr_icp_params_default", "ltr_icp_refine", "ltr_knn_diff_refined", "ltr_icp_refine_scanside", "ltr_scanside_split_refined", "ltr_debug_pixel_index", "ltr_debug_scan_rimg", "ltr_debug_exact_knn_avg", "ltr_debug_nearest", "ltr_debug_fast_project", "ltr_debug_atan_sweep", "ltr_debug_margins", "ltr_debug_voxel_distributed", "ltr_reset_rimg_size", "ltr_last_pass_stats", "ltr_profile_get", "ltr_profile_reset", "ltr_timer_start", "ltr_timer_stop", "ltr_trace_dump",
     "ltr_pinned_alloc", "ltr_pinned_free", "ltr_nccl_unique_id", "ltr_nccl_init", "ltr_nccl_split", "ltr_nccl_info", "ltr_nccl_destroy", "ltr_nccl_version", "ltr_nccl_allreduce_flags",
     "ltr_nccl_allgather_clouds", "ltr_nccl_exchange_clouds", "ltr_nccl_voxel_centroid_merged", "ltr_nccl_allgather_i64", "ltr_nccl_max_f64", "ltr_nccl_barrier", "ltr_stream_handle",
 ]
@@ -115,6 +115,8 @@ def lib():
     L.ltr_icp_params_default.restype = None
     L.ltr_icp_refine.argtypes = [vp, i32, i32, i32, i32, P(IcpParams), vp, vp, vp, vp]
     L.ltr_knn_diff_refined.argtypes = [vp, i32, i32, i32, i32, i32, f32, vp, vp, P(i32), P(i32)]
+    L.ltr_icp_refine_scanside.argtypes = [vp, i32, i32, i32, i32, P(IcpParams), vp, vp, vp, vp]
+    L.ltr_scanside_split_refined.argtypes = [vp, i32, i32, i32, i32, i32, i32, f32, vp, vp, P(i32), P(i32)]
     L.ltr_debug_pixel_index.argtypes = [vp, vp, i64, i32, i32, vp, vp, vp, vp, vp]
     L.ltr_debug_scan_rimg.argtypes = [vp, i32, i32, ctypes.c_float, vp]
     L.ltr_debug_exact_knn_avg.argtypes = [vp, i32, i32, i32, i32, vp, P(i64)]
@@ -407,6 +409,13 @@ class Context:
     def icp_refine(self, scans, poses, target_down, pose_offset=0, **params):
         """ltr_icp_refine: per keyframe (T (K, 4, 4) float32, fitness (K,) float64, iterations (K,) int32, exit reason (K,) int32).
         Keyword arguments override fields of ltr_icp_params (defaults: the reference's values), e.g. max_iterations=5."""
+        return self._icp(lib().ltr_icp_refine, scans, poses, target_down, pose_offset, params)
+
+    def icp_refine_scanside(self, scans, poses, target_down, pose_offset=0, **params):
+        """ltr_icp_refine_scanside: icp_refine with each scan moved to the global frame as scan-side removal moves it (lidar2base)."""
+        return self._icp(lib().ltr_icp_refine_scanside, scans, poses, target_down, pose_offset, params)
+
+    def _icp(self, fn, scans, poses, target_down, pose_offset, params):
         prm = IcpParams()
         lib().ltr_icp_params_default(ctypes.byref(prm))
         for key, v in params.items():
@@ -418,8 +427,8 @@ class Context:
         fit = np.empty(K, np.float64)
         it = np.empty(K, np.int32)
         ex = np.empty(K, np.int32)
-        self._ck(lib().ltr_icp_refine(self._h, scans, poses, pose_offset, target_down, ctypes.byref(prm), T.ctypes.data, fit.ctypes.data,
-                                      it.ctypes.data, ex.ctypes.data))
+        self._ck(fn(self._h, scans, poses, pose_offset, target_down, ctypes.byref(prm), T.ctypes.data, fit.ctypes.data, it.ctypes.data,
+                    ex.ctypes.data))
         return T, fit, it, ex
 
     def knn_diff_refined(self, scans, poses, target, k, thr, T, accepted, pose_offset=0):
@@ -430,6 +439,18 @@ class Context:
         a, b = ctypes.c_int32(), ctypes.c_int32()
         self._ck(lib().ltr_knn_diff_refined(self._h, scans, poses, pose_offset, target, k, thr, Tf.ctypes.data, acc.ctypes.data,
                                             ctypes.byref(a), ctypes.byref(b)))
+        return a.value, b.value
+
+    def scanside_split_refined(self, scans, poses, map_, criterion, k, thr, T, accepted, pose_offset=0):
+        """(static, dynamic) scan sets of ltr_scanside_split_refined: keyframes with accepted[k] are moved by T[k] (float32 4x4) first.
+        T or accepted None passes NULL."""
+        K = self.scanset_info(scans)[0]
+        Tf = None if T is None else np.ascontiguousarray(T, np.float32).reshape(K * 16)
+        acc = None if accepted is None else np.ascontiguousarray(accepted, np.uint8).reshape(K)
+        a, b = ctypes.c_int32(), ctypes.c_int32()
+        self._ck(lib().ltr_scanside_split_refined(self._h, scans, poses, pose_offset, map_, criterion, k, thr,
+                                                  None if Tf is None else Tf.ctypes.data, None if acc is None else acc.ctypes.data,
+                                                  ctypes.byref(a), ctypes.byref(b)))
         return a.value, b.value
 
     def scanside_stats(self):

@@ -369,14 +369,26 @@ int Removerter::removeHighDynamicPoints() {
 // Multi-GPU: every rank splits the keyframes of scan_sess it holds (its own block, poses included) and needs no collective: after
 // removeHighDynamicPoints every rank holds both sessions' static maps -- replicated over all ranks, or in session-split mode its own
 // session's map from Step 1 and the other one from the exchange above.
-int Removerter::scansideRemovalForEachScan(Session& map_sess, Session& scan_sess, int criterion) {
+int Removerter::scansideRemovalForEachScan(Session& map_sess, Session& scan_sess, int criterion, bool isFineRegistration) {
     StageTimer t(*this, "scanside");
+    scan_sess.scanside_icp_.clear();
     if (!owns(scan_sess)) return LTR_OK;
     if (map_sess.map_global_curr_static_.get() < 0) return fail(LTR_ERR_INVALID, "scansideRemovalForEachScan: no static map of the " + map_sess.sess_type_ + " session (run Steps 1-2 first)");
     if (scan_sess.keyframe_scans_.get() < 0) return fail(LTR_ERR_INVALID, "scansideRemovalForEachScan: no keyframe scans of the " + scan_sess.sess_type_ + " session");
     ltr_scanset st, dy;
-    CK(ltr_scanside_split(ctx, scan_sess.keyframe_scans_.get(), scan_sess.keyframe_poses_.get(), 0, map_sess.map_global_curr_static_.get(), criterion,
-                          P.num_nn_points_within, P.dist_nn_points_within, &st, &dy));   // :1302-1309
+    if (!isFineRegistration) {
+        CK(ltr_scanside_split(ctx, scan_sess.keyframe_scans_.get(), scan_sess.keyframe_poses_.get(), 0, map_sess.map_global_curr_static_.get(), criterion,
+                              P.num_nn_points_within, P.dist_nn_points_within, &st, &dy));   // :1302-1309
+    } else {
+        // :1263-1268 / :1325-1331 set up the ICP of Session.cpp:396-402 against the map session's map; :978 keeps the registered scan iff
+        // getFitnessScore() < 1.0.  A rejected keyframe is split unregistered (the live rule of Session.cpp:571-579, DESIGN.md §5.4).  The
+        // registration reaches scanside_icp_ only with the split that used it: a failed call leaves no stats behind.
+        IcpStats reg;
+        CK(registerKeyframes(scan_sess, scan_sess.keyframe_scans_.get(), map_sess.map_global_curr_static_.get(), ltr_icp_refine_scanside, &reg));
+        CK(ltr_scanside_split_refined(ctx, scan_sess.keyframe_scans_.get(), scan_sess.keyframe_poses_.get(), 0, map_sess.map_global_curr_static_.get(),
+                                      criterion, P.num_nn_points_within, P.dist_nn_points_within, reg.T16.data(), reg.accepted.data(), &st, &dy));
+        scan_sess.scanside_icp_ = std::move(reg);
+    }
     scan_sess.scans_static_ = ScanSetOwner(ctx, st);
     scan_sess.scans_dynamic_ = ScanSetOwner(ctx, dy);
     return LTR_OK;
@@ -396,30 +408,34 @@ int Removerter::parseStaticScansViaProjection() {
     return LTR_OK;
 }
 
+int Removerter::registerKeyframes(Session& s, ltr_scanset scans, ltr_cloud target_map, decltype(&ltr_icp_refine) icp, IcpStats* out) {
+    int32_t K = 0;
+    int64_t npts = 0;
+    CK(ltr_scanset_info(ctx, scans, &K, &npts));
+    out->resize((size_t)K);
+    ltr_cloud tgt;
+    CK(ltr_voxel_centroid(ctx, target_map, 0.4f, &tgt));   // Session.cpp:400
+    CloudOwner tgt_owner(ctx, tgt);
+    CK(icp(ctx, scans, s.keyframe_poses_.get(), 0, tgt, nullptr, out->T16.data(), out->fitness.data(), out->iterations.data(), out->exit.data()));
+    for (int32_t k = 0; k < K; ++k) out->accepted[(size_t)k] = out->fitness[(size_t)k] < 1.0 ? 1 : 0;   // Session.cpp:571
+    return LTR_OK;
+}
+
 int Removerter::extractLowDynPointsViaKnnDiff(Session& s, ltr_cloud target_map) {
     ltr_scanset co, di;
-    s.clear_icp_stats();
+    s.icp_.clear();
     if (!useICPrefinement_) {
         // Session.cpp:395-402 (0.4 m downsample + ICP target) only feed the refinement, which the reference switches off (Session.cpp:551)
         CK(ltr_knn_diff(ctx, s.keyframe_scans_static_projected_.get(), s.keyframe_poses_.get(), 0, target_map, P.num_nn_points_within, P.dist_nn_points_within, &co, &di));
     } else {
         // Session.cpp:394-402: the ICP target is the other session's map at 0.4 m; partitionLowDynamicPointsOfScanByKnn (:549-584) registers
         // every keyframe to it and keeps the registered scan iff getFitnessScore() < 1.0.  Multi-GPU: this rank's keyframe block against
-        // its replica of the target map, no collective.
-        int32_t K = 0;
-        int64_t npts = 0;
-        CK(ltr_scanset_info(ctx, s.keyframe_scans_static_projected_.get(), &K, &npts));
-        s.icp_T16_.resize((size_t)K * 16); s.icp_fitness_.resize((size_t)K); s.icp_iterations_.resize((size_t)K); s.icp_exit_.resize((size_t)K);
-        s.icp_accepted_.resize((size_t)K);
-        ltr_cloud tgt;
-        CK(ltr_voxel_centroid(ctx, target_map, 0.4f, &tgt));   // Session.cpp:400
-        CloudOwner tgt_owner(ctx, tgt);
-        CK(ltr_icp_refine(ctx, s.keyframe_scans_static_projected_.get(), s.keyframe_poses_.get(), 0, tgt, nullptr, s.icp_T16_.data(), s.icp_fitness_.data(),
-                          s.icp_iterations_.data(), s.icp_exit_.data()));
-        tgt_owner.reset();
-        for (int32_t k = 0; k < K; ++k) s.icp_accepted_[(size_t)k] = s.icp_fitness_[(size_t)k] < 1.0 ? 1 : 0;   // Session.cpp:571
+        // its replica of the target map, no collective.  As in scansideRemovalForEachScan, the stats reach s.icp_ only with the diff.
+        IcpStats reg;
+        CK(registerKeyframes(s, s.keyframe_scans_static_projected_.get(), target_map, ltr_icp_refine, &reg));
         CK(ltr_knn_diff_refined(ctx, s.keyframe_scans_static_projected_.get(), s.keyframe_poses_.get(), 0, target_map, P.num_nn_points_within,
-                                P.dist_nn_points_within, s.icp_T16_.data(), s.icp_accepted_.data(), &co, &di));
+                                P.dist_nn_points_within, reg.T16.data(), reg.accepted.data(), &co, &di));
+        s.icp_ = std::move(reg);
     }
     s.scans_knn_coexist_ = ScanSetOwner(ctx, co);
     s.scans_knn_diff_ = ScanSetOwner(ctx, di);
@@ -631,7 +647,8 @@ int Removerter::run_step3() {
 int Removerter::reset_to_step0() {
     CK(ltr_scan_images_release(ctx, 0));   // their storage stays for the next step's sets
     for (Session* s : {&central_sess_, &query_sess_}) {
-        s->clear_icp_stats();   // Step 2's results
+        s->icp_.clear();   // Step 2's results
+        s->scanside_icp_.clear();
         auto it = saved.find("OriginalNoisy" + s->sess_type_ + "MapGlobal");
         if (!owns(*s)) {   // session-split: everything held of the other session was derived after Step 0
             for (auto& kv : s->cloud_names()) kv.second->reset();
@@ -670,7 +687,8 @@ int Removerter::cascade_promote_updated() {
     for (Session* s : {&central_sess_, &query_sess_}) {
         for (auto& kv : s->cloud_names()) kv.second->reset();
         for (auto& kv : s->scanset_names()) kv.second->reset();
-        s->clear_icp_stats();
+        s->icp_.clear();
+        s->scanside_icp_.clear();
     }
     saved.clear();
     query_sess_.keyframe_poses_.reset();
@@ -806,6 +824,7 @@ int Removerter::rollback(int i) {
 // ---------------------------------------------------------------------------------------------------------------
 using ltremovert_b200::Removerter;
 using ltremovert_b200::Session;
+using ltremovert_b200::IcpStats;
 
 struct ltrh_removerter { Removerter* R; };
 static thread_local std::string g_err;
@@ -898,6 +917,14 @@ int ltrh_scanside_removal(ltrh_removerter* r, int32_t map_sess, int32_t scan_ses
     return R.scansideRemovalForEachScan(map_sess == 0 ? R.central_sess_ : R.query_sess_, scan_sess == 0 ? R.central_sess_ : R.query_sess_, criterion);
 }
 
+int ltrh_scanside_removal_registered(ltrh_removerter* r, int32_t map_sess, int32_t scan_sess, int32_t criterion) {
+    if (!r || (map_sess != 0 && map_sess != 1) || (scan_sess != 0 && scan_sess != 1)) return LTR_ERR_INVALID;
+    Removerter& R = *r->R;
+    R.err.clear();
+    return R.scansideRemovalForEachScan(map_sess == 0 ? R.central_sess_ : R.query_sess_, scan_sess == 0 ? R.central_sess_ : R.query_sess_, criterion,
+                                        true);
+}
+
 int ltrh_set_icp_refinement(ltrh_removerter* r, int32_t on) {
     if (!r) return LTR_ERR_INVALID;
     r->R->useICPrefinement_ = on != 0;
@@ -916,21 +943,33 @@ int ltrh_set_map_ball(ltrh_removerter* r, float radius) {
     return LTR_OK;
 }
 
+static int copy_icp_stats(const IcpStats& S, int32_t capacity, int32_t* K_out, float* T16, double* fitness, int32_t* iterations,
+                          int32_t* exit_reason, uint8_t* accepted) {
+    const int32_t K = (int32_t)S.fitness.size();
+    *K_out = K;
+    if (capacity < K) return LTR_OK;   // a size query
+    for (int32_t k = 0; k < K; ++k) {
+        if (T16) for (int j = 0; j < 16; ++j) T16[16 * (size_t)k + j] = S.T16[16 * (size_t)k + j];
+        if (fitness) fitness[k] = S.fitness[(size_t)k];
+        if (iterations) iterations[k] = S.iterations[(size_t)k];
+        if (exit_reason) exit_reason[k] = S.exit[(size_t)k];
+        if (accepted) accepted[k] = S.accepted[(size_t)k];
+    }
+    return LTR_OK;
+}
+
 int ltrh_icp_stats(ltrh_removerter* r, int32_t sess, int32_t capacity, int32_t* K_out, float* T16, double* fitness, int32_t* iterations,
                    int32_t* exit_reason, uint8_t* accepted) {
     if (!r || (sess != 0 && sess != 1) || !K_out) return LTR_ERR_INVALID;
     const Session& S = sess == 0 ? r->R->central_sess_ : r->R->query_sess_;
-    const int32_t K = (int32_t)S.icp_fitness_.size();
-    *K_out = K;
-    if (capacity < K) return LTR_OK;   // a size query
-    for (int32_t k = 0; k < K; ++k) {
-        if (T16) for (int j = 0; j < 16; ++j) T16[16 * (size_t)k + j] = S.icp_T16_[16 * (size_t)k + j];
-        if (fitness) fitness[k] = S.icp_fitness_[(size_t)k];
-        if (iterations) iterations[k] = S.icp_iterations_[(size_t)k];
-        if (exit_reason) exit_reason[k] = S.icp_exit_[(size_t)k];
-        if (accepted) accepted[k] = S.icp_accepted_[(size_t)k];
-    }
-    return LTR_OK;
+    return copy_icp_stats(S.icp_, capacity, K_out, T16, fitness, iterations, exit_reason, accepted);
+}
+
+int ltrh_scanside_icp_stats(ltrh_removerter* r, int32_t sess, int32_t capacity, int32_t* K_out, float* T16, double* fitness, int32_t* iterations,
+                            int32_t* exit_reason, uint8_t* accepted) {
+    if (!r || (sess != 0 && sess != 1) || !K_out) return LTR_ERR_INVALID;
+    const Session& S = sess == 0 ? r->R->central_sess_ : r->R->query_sess_;
+    return copy_icp_stats(S.scanside_icp_, capacity, K_out, T16, fitness, iterations, exit_reason, accepted);
 }
 
 int ltrh_stage(ltrh_removerter* r, const char* name) {

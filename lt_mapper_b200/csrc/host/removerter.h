@@ -25,6 +25,17 @@ struct PassLog { std::string what; int64_t n_map, n_dynamic, n_static_after, n_d
 
 class Removerter;
 
+// Per-keyframe results of one registration of a session's keyframes on this rank (ltr_icp_refine / ltr_icp_refine_scanside): the final
+// float 4x4 (16 per keyframe), fitness, iterations, exit reason and the accept flag (fitness < 1.0)
+struct IcpStats {
+    std::vector<float> T16;
+    std::vector<double> fitness;
+    std::vector<int32_t> iterations, exit;
+    std::vector<uint8_t> accepted;
+    void resize(size_t K) { T16.resize(K * 16); fitness.resize(K); iterations.resize(K); exit.resize(K); accepted.resize(K); }
+    void clear() { resize(0); }
+};
+
 class Session {
 public:
     static constexpr float kReprojectionAlpha = 3.0f;  // Session.h:13
@@ -43,11 +54,9 @@ public:
     // ltrh_rollback, per keyframe of this rank
     ScanSetOwner composed_pd_, composed_nd_, keyframe_scans_restored_;
     // ICP refinement of the last extractLowDynPointsViaKnnDiff with useICPrefinement_ on (ltr_icp_refine), per keyframe of this rank
-    std::vector<float> icp_T16_;
-    std::vector<double> icp_fitness_;
-    std::vector<int32_t> icp_iterations_, icp_exit_;
-    std::vector<uint8_t> icp_accepted_;
-    void clear_icp_stats() { icp_T16_.clear(); icp_fitness_.clear(); icp_iterations_.clear(); icp_exit_.clear(); icp_accepted_.clear(); }
+    IcpStats icp_;
+    // fine registration of the last scansideRemovalForEachScan of this session's scans with isFineRegistration (ltr_icp_refine_scanside)
+    IcpStats scanside_icp_;
     // maps (Session.h:67-87)
     CloudOwner map_global_orig_, map_global_curr_, map_global_curr_static_, map_global_curr_dynamic_;
     CloudOwner map_global_updated_, map_global_updated_strong_;
@@ -83,8 +92,10 @@ public:
     int parseLDScansViaProjection();                                           // :1564-1577
     int updateScansScanwise();                                                 // :1540-1548 -> Session.cpp:362-380
     // :1253-1310 (commented out in the reference): scan_sess.scans_{static,dynamic}_ <- removeDynamicPointsOfScanByKnn (:1019-1123) of
-    // every keyframe of scan_sess this rank holds, against map_sess.map_global_curr_static_; criterion = ltr_scanside_criterion
-    int scansideRemovalForEachScan(Session& map_sess, Session& scan_sess, int criterion);
+    // every keyframe of scan_sess this rank holds, against map_sess.map_global_curr_static_; criterion = ltr_scanside_criterion.
+    // isFineRegistration (:1295-1297): each keyframe is first registered to that map at 0.4 m (removeDynamicPointsOfScanByKnnBtnSession,
+    // :950-1017) and split registered when its fitness is below 1.0; scan_sess.scanside_icp_ holds the registration.
+    int scansideRemovalForEachScan(Session& map_sess, Session& scan_sess, int criterion, bool isFineRegistration = false);
     int run_step0();
     int run_step12();
     int run_step3();
@@ -99,6 +110,9 @@ public:
     // ---- Session methods (Session.cpp) ----
     int parseScansViaProjection(Session& s, ltr_cloud map, ScanSetOwner* vec_to_store);    // Session.cpp:348-360
     int extractLowDynPointsViaKnnDiff(Session& s, ltr_cloud target_map);                   // Session.cpp:393-427, 549-584
+    // every keyframe of `scans` (poses of s) registered by `icp` (ltr_icp_refine or ltr_icp_refine_scanside) to target_map at 0.4 m with
+    // the reference's parameters (Session.cpp:396-402); accepted iff fitness < 1.0 (Session.cpp:571)
+    int registerKeyframes(Session& s, ltr_scanset scans, ltr_cloud target_map, decltype(&ltr_icp_refine) icp, IcpStats* out);
     int extractHighDynPointsViaKnnDiff(Session& s, ltr_cloud target_map);                  // Session.cpp:487-504
     int constructGlobalNDMap(Session& s);                                                  // Session.cpp:430-435
     int constructGlobalPDMap(Session& s);                                                  // Session.cpp:437-445

@@ -9,6 +9,8 @@
 // fixes the arithmetic; the device equals the CPU restatement tests/_icp_oracle.py bit for bit (DESIGN.md §5.2).  For keyframe k of the
 // scan set (pose index pose_offset + k):
 //  1. scan_global = local2global(scan_k, pose, base2lidar) exactly as ltr_knn_diff moves it (the reference's choice of extrinsic);
+//     ltr_icp_refine_scanside instead moves it as ltr_scanside_split does, local2global(scan_k, pose, lidar2base) (utility.cpp:160-168,
+//     the scan-side registration of Removerter.cpp:950-1017); with the identity extrinsic the two agree bit for bit.
 //     src = octreeDownsampling(scan_global, source_leaf) (ltr_voxel_centroid_per_keyframe); tgt = the caller's 0.4 m target.
 //  2. Correspondences (CorrespondenceEstimation::determineCorrespondences): the partner of each working source point is its nearest tgt
 //     point by L2_Simple in f32 (((dx*dx) + dy*dy) + dz*dz, no FMA), the LOWEST tgt index on ties; pairs with (double)d2 > max_dist^2 are
@@ -330,9 +332,7 @@ __global__ void __launch_bounds__(256) nearest_debug_kernel(Levels T, PtrView q,
 
 using namespace ltr;
 
-extern "C" {
-
-void ltr_icp_params_default(ltr_icp_params* p) {
+extern "C" void ltr_icp_params_default(ltr_icp_params* p) {
     if (!p) return;
     p->max_correspondence_distance = 150.0;   // Session.cpp:396
     p->max_iterations = 100;                  // :397
@@ -343,10 +343,13 @@ void ltr_icp_params_default(ltr_icp_params* p) {
     p->source_leaf = 0.4f;                    // Session.cpp:558-559
 }
 
-int ltr_icp_refine(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_offset, ltr_cloud target_h, const ltr_icp_params* prm,
-                   float* T16_out, double* fitness_out, int32_t* iterations_out, int32_t* exit_out) {
-    ApiTrace tr__(ctx, "ltr_icp_refine");
-    if (!ctx) return LTR_ERR_INVALID;
+namespace ltr {
+namespace {
+
+// ltr_icp_refine (scanside = false: scan_global as ltr_knn_diff moves it, base2lidar then the pose) and ltr_icp_refine_scanside
+// (scanside = true: as ltr_scanside_split moves it, lidar2base then the pose); everything after step 1 is the same.
+int icp_refine(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_offset, ltr_cloud target_h, const ltr_icp_params* prm,
+               bool scanside, float* T16_out, double* fitness_out, int32_t* iterations_out, int32_t* exit_out) {
     ltr_icp_params P;
     ltr_icp_params_default(&P);
     if (prm) P = *prm;
@@ -378,9 +381,9 @@ int ltr_icp_refine(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t
         ScanSetOwner g_glob;
         LTR_TRY(scanset_new(ctx, scans.h_off, &g_glob));
         const DevCloud g = ctx->scansets[g_glob.get()].pts;
-        // scan_global as ltr_knn_diff moves it: base2lidar, then the pose
-        LTR_TRY(scans_to_global(ctx, scans, 0, scans.pts.n, poses.d + (size_t)pose_offset * 24, ctx->ext_identity ? nullptr : ctx->d_ext, g.x(),
-                                g.y(), g.z(), g.i()));
+        // scan_global as the partition that follows moves it: base2lidar (kNN diff) or lidar2base (scan-side removal), then the pose
+        const double* ext = ctx->ext_identity ? nullptr : ctx->d_ext + (scanside ? 12 : 0);
+        LTR_TRY(scans_to_global(ctx, scans, 0, scans.pts.n, poses.d + (size_t)pose_offset * 24, ext, g.x(), g.y(), g.z(), g.i()));
         {
             float mn[3], mx[3];
             LTR_TRY(finite_extent(ctx, g, "scan", mn, mx));
@@ -438,6 +441,25 @@ int ltr_icp_refine(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t
     if (iterations_out) std::copy(hit.begin(), hit.end(), iterations_out);
     if (exit_out) std::copy(hex.begin(), hex.end(), exit_out);
     return LTR_OK;
+}
+
+}  // namespace
+}  // namespace ltr
+
+extern "C" {
+
+int ltr_icp_refine(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_offset, ltr_cloud target_h, const ltr_icp_params* prm,
+                   float* T16_out, double* fitness_out, int32_t* iterations_out, int32_t* exit_out) {
+    ApiTrace tr__(ctx, "ltr_icp_refine");
+    if (!ctx) return LTR_ERR_INVALID;
+    return icp_refine(ctx, scans_h, poses_h, pose_offset, target_h, prm, false, T16_out, fitness_out, iterations_out, exit_out);
+}
+
+int ltr_icp_refine_scanside(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_offset, ltr_cloud target_h,
+                            const ltr_icp_params* prm, float* T16_out, double* fitness_out, int32_t* iterations_out, int32_t* exit_out) {
+    ApiTrace tr__(ctx, "ltr_icp_refine_scanside");
+    if (!ctx) return LTR_ERR_INVALID;
+    return icp_refine(ctx, scans_h, poses_h, pose_offset, target_h, prm, true, T16_out, fitness_out, iterations_out, exit_out);
 }
 
 int ltr_knn_diff_refined(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_offset, ltr_cloud target_h, int32_t k, float thr,

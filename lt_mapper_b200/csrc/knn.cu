@@ -92,11 +92,7 @@ __global__ void __launch_bounds__(128, 12) knn_scan_label_kernel(PtrView scans, 
     const int kf = find_kf(off, K, i);
     float x = scans.x[i], y = scans.y[i], z = scans.z[i];
     scan_to_global(poses + (size_t)kf * 24 + 12, ext, order, &x, &y, &z);
-    if (T16 && accept[kf]) {
-        const float* m = T16 + 16 * (size_t)kf;
-        const float nx = frow(m, x, y, z), ny = frow(m + 4, x, y, z), nz = frow(m + 8, x, y, z);
-        x = nx; y = ny; z = nz;
-    }
+    refine_point(T16, accept, kf, &x, &y, &z);
     gx[i] = x; gy[i] = y; gz[i] = z;
     label[i] = knn_label_dispatch(t, s_t, x, y, z, k, thr);
 }
@@ -204,10 +200,7 @@ int knn_diff(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_
         if (T16) {
             dT = (float*)((char*)p + b_g);
             dacc = (uint8_t*)p + b_g + b_T;
-            std::vector<uint8_t> acc((size_t)K);
-            for (int j = 0; j < K; ++j) acc[j] = accepted[j] ? 1 : 0;
-            LTR_CUDA(ctx, cudaMemcpyAsync(dT, T16, (size_t)K * 64, cudaMemcpyHostToDevice, ctx->stream));
-            LTR_CUDA(ctx, cudaMemcpyAsync(dacc, acc.data(), (size_t)K, cudaMemcpyHostToDevice, ctx->stream));
+            LTR_TRY(upload_refinement(ctx, K, T16, accepted, dT, dacc));
         }
         knn_scan_label_kernel<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(view(scans.pts), scans.d_off, K, poses.d + (size_t)pose_offset * 24,
             ctx->ext_identity ? nullptr : ctx->d_ext, ctx->cfg.transform_order, dT, dacc, t, k, thr, split.flags, gx, gy, gz);

@@ -234,9 +234,12 @@ int segment_counts(ltr_ctx* ctx, const uint8_t* flags, const DevScanSet& s, std:
 int split_scanset_by_flag(ltr_ctx* ctx, const DevScanSet& in, const uint8_t* flags, ltr_scanset* out_unflagged, ltr_scanset* out_flagged);
 
 // The points [base, base + n) of `scans` in the global frame (scan_to_global, ref_math.cuh), written to o*[i - base]; keyframe k's pose
-// rows are poses + 24 k + 12, ext is the extrinsic applied first (null: the identity).  oi (optional) receives the intensity.
+// rows are poses + 24 k + 12, ext is the extrinsic applied first (null: the identity).  oi (optional) receives the intensity.  With the
+// device tables T16 / accept (K x 16 floats, K bytes; null: none) the points of keyframe k are then moved by refine_point.
 int scans_to_global(ltr_ctx* ctx, const DevScanSet& scans, int64_t base, int64_t n, const double* poses, const double* ext, float* ox,
-                    float* oy, float* oz, float* oi);
+                    float* oy, float* oz, float* oi, const float* T16 = nullptr, const uint8_t* accept = nullptr);
+// The host tables of a refined split (K transforms of 16 floats, K accept flags) to the device: dT (K x 64 B) and dacc (K bytes, 0 / 1).
+int upload_refinement(ltr_ctx* ctx, int K, const float* T16, const uint8_t* accepted, float* dT, uint8_t* dacc);
 
 // The end of a scan-set split (ltr_knn_diff, ltr_scanside_split).  The caller sets flags[i] (1: second part) for every point and hands
 // over the points' global coordinates, all at once or a keyframe range at a time; relocalise() moves them back to their keyframes'

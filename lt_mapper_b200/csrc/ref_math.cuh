@@ -171,6 +171,15 @@ LTR_DEV void scan_to_global(const double* __restrict__ pose, const double* __res
 // ((m0 x + m1 y) + m2 z) + m3 in f32, m = one row of a row-major float 4x4 (PCL's Matrix4f applied to a point)
 LTR_DEV float frow(const float* m, float x, float y, float z) { return fa(fa(fa(fm(m[0], x), fm(m[1], y)), fm(m[2], z)), m[3]); }
 
+// The registration of ltr_knn_diff_refined and ltr_scanside_split_refined (Session.cpp:565): a global point of keyframe kf moved by the
+// float 4x4 T16 + 16 kf with frow when accept[kf] != 0.  T16 == null: no refinement, the point stays.
+LTR_DEV void refine_point(const float* __restrict__ T16, const uint8_t* __restrict__ accept, int kf, float* x, float* y, float* z) {
+    if (!T16 || !accept[kf]) return;
+    const float* m = T16 + 16 * (size_t)kf;
+    const float nx = frow(m, *x, *y, *z), ny = frow(m + 4, *x, *y, *z), nz = frow(m + 8, *x, *y, *z);
+    *x = nx; *y = ny; *z = nz;
+}
+
 // FLANN L2_Simple<float> squared distance: ((dx*dx) + dy*dy) + dz*dz with dx = query - point
 LTR_DEV float l2_simple(float qx, float qy, float qz, float px, float py, float pz) {
     const float dx = fs(qx, px), dy = fs(qy, py), dz = fs(qz, pz);

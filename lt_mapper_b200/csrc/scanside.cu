@@ -24,6 +24,8 @@
 // only as far as some query needs them.  Beside that the call holds one flag byte per point and a relocalised copy of the scans
 // (16 B/point) for the final order-preserving compaction, as ltr_knn_diff does.  All of it comes from the context's caching allocator and
 // is returned before the call ends.
+// ltr_scanside_split_refined (the fine registration between sessions, Removerter.cpp:950-1017; DESIGN.md §5.4) is the same body with a
+// per-keyframe transform table on the device (64 B + 1 B per keyframe), applied in the chunk's global-coordinate step.
 #include "ltr_internal.cuh"
 #include "ref_math.cuh"
 #include "device_util.cuh"
@@ -231,17 +233,11 @@ __global__ void __launch_bounds__(256) scanside_diff_kernel(const float* __restr
     flag[t] = (fabsf(fs(avg_scan[t], avg_map[t])) < thr) ? 0 : 1;
 }
 
-}  // namespace
-}  // namespace ltr
-
-using namespace ltr;
-
-extern "C" {
-
-int ltr_scanside_split(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_offset, ltr_cloud map_h, int32_t criterion,
-                       int32_t k, float thr, ltr_scanset* out_static, ltr_scanset* out_dynamic) {
-    ApiTrace tr__(ctx, "ltr_scanside_split");
-    if (!ctx) return LTR_ERR_INVALID;
+// ltr_scanside_split (refined = false, T16 = accepted = null) and ltr_scanside_split_refined: with refined, the global points of keyframe
+// k with accepted[k] != 0 are moved by T16 + 16 k in the chunk's global-coordinate step, before the finite check, both searches and the
+// relocalisation; K > 0 keyframes without T16 or accepted are LTR_ERR_INVALID.
+int scanside_split(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_offset, ltr_cloud map_h, int32_t criterion, int32_t k,
+                   float thr, bool refined, const float* T16, const uint8_t* accepted, ltr_scanset* out_static, ltr_scanset* out_dynamic) {
     DevScanSet* sp;
     DevPoses* pp;
     DevCloud* mp;
@@ -253,6 +249,7 @@ int ltr_scanside_split(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int
     if (!(thr > 0.0f)) return fail(ctx, LTR_ERR_INVALID, "threshold must be positive");
     LTR_TRY(check_pose_range(ctx, *sp, *pp, pose_offset));
     if (mp->n < 1) return fail(ctx, LTR_ERR_UNSUPPORTED, "empty map (PCL's nearestKSearch asserts on an empty tree)");
+    if (refined && sp->K > 0 && (!T16 || !accepted)) return fail(ctx, LTR_ERR_INVALID, "null transforms or accept mask");
     const DevScanSet scans = *sp;
     const DevPoses poses = *pp;
     const DevCloud map = *mp;
@@ -272,9 +269,18 @@ int ltr_scanside_split(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int
         const int64_t ccap = round_cap(max_chunk);
         void* work = nullptr;
         ScratchGuard g_work(ctx, &work);
-        // chunk global coordinates (a DevCloud layout, for minmax_xyz) | avg_map | avg_scan | two lists | counter | chunk offsets
+        // chunk global coordinates (a DevCloud layout, for minmax_xyz) | avg_map | avg_scan | two lists | counter | chunk offsets |
+        // refinement transforms | accept flags
         const size_t b_g = (size_t)ccap * 16, b_f = (size_t)ccap * 4, b_off = ((size_t)kMaxSegments + 1) * 8;
-        LTR_TRY(dev_alloc(ctx, &work, b_g + 4 * b_f + 256 + b_off));
+        const size_t b_T = refined ? ((size_t)scans.K * 64 + 255) / 256 * 256 : 0, b_acc = refined ? (size_t)scans.K : 0;
+        LTR_TRY(dev_alloc(ctx, &work, b_g + 4 * b_f + 256 + b_off + b_T + b_acc));
+        float* dT = nullptr;
+        uint8_t* dacc = nullptr;
+        if (refined) {
+            dT = (float*)((char*)work + b_g + 4 * b_f + 256 + b_off);
+            dacc = (uint8_t*)dT + b_T;
+            LTR_TRY(upload_refinement(ctx, scans.K, T16, accepted, dT, dacc));
+        }
         DevCloud g;
         g.base = (float*)work; g.cap = ccap;
         float* avg_map = (float*)((char*)work + b_g);
@@ -294,8 +300,9 @@ int ltr_scanside_split(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int
             const int64_t base = scans.h_off[kf0], m = scans.h_off[kf1] - base;
             ctx->scanside_stats[3]++;
             if (m == 0) continue;
-            // local2global with lidar2base (file header)
-            LTR_TRY(scans_to_global(ctx, scans, base, m, pose0, ctx->ext_identity ? nullptr : ctx->d_ext + 12, g.x(), g.y(), g.z(), nullptr));
+            // local2global with lidar2base (file header), then an accepted keyframe's registration
+            LTR_TRY(scans_to_global(ctx, scans, base, m, pose0, ctx->ext_identity ? nullptr : ctx->d_ext + 12, g.x(), g.y(), g.z(), nullptr, dT,
+                                    dacc));
             g.n = m;
             float mn[3], mx[3];
             char where[48];
@@ -326,6 +333,28 @@ int ltr_scanside_split(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int
         g_work.release();
     }
     return split.finish(out_static, out_dynamic);
+}
+
+}  // namespace
+}  // namespace ltr
+
+using namespace ltr;
+
+extern "C" {
+
+int ltr_scanside_split(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_offset, ltr_cloud map_h, int32_t criterion,
+                       int32_t k, float thr, ltr_scanset* out_static, ltr_scanset* out_dynamic) {
+    ApiTrace tr__(ctx, "ltr_scanside_split");
+    if (!ctx) return LTR_ERR_INVALID;
+    return scanside_split(ctx, scans_h, poses_h, pose_offset, map_h, criterion, k, thr, false, nullptr, nullptr, out_static, out_dynamic);
+}
+
+int ltr_scanside_split_refined(ltr_ctx* ctx, ltr_scanset scans_h, ltr_poses poses_h, int32_t pose_offset, ltr_cloud map_h, int32_t criterion,
+                               int32_t k, float thr, const float* T16, const uint8_t* accepted, ltr_scanset* out_static,
+                               ltr_scanset* out_dynamic) {
+    ApiTrace tr__(ctx, "ltr_scanside_split_refined");
+    if (!ctx) return LTR_ERR_INVALID;
+    return scanside_split(ctx, scans_h, poses_h, pose_offset, map_h, criterion, k, thr, true, T16, accepted, out_static, out_dynamic);
 }
 
 int ltr_scanside_stats(ltr_ctx* ctx, int64_t* stats4) {

@@ -946,13 +946,15 @@ static int voxel_distributed_simulated(ltr_ctx* ctx, int G, const ltr_cloud* loc
 __global__ void __launch_bounds__(256) scans_to_global_kernel(PtrView in, const int64_t* __restrict__ off, int K, int64_t base, int64_t n,
                                                               const double* __restrict__ poses, const double* __restrict__ ext, int order,
                                                               float* __restrict__ ox, float* __restrict__ oy, float* __restrict__ oz,
-                                                              float* __restrict__ oi) {
+                                                              float* __restrict__ oi, const float* __restrict__ T16,
+                                                              const uint8_t* __restrict__ accept) {
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= n) return;
     const int64_t i = base + t;
     const int k = find_kf(off, K, i);
     float x = in.x[i], y = in.y[i], z = in.z[i];
     scan_to_global(poses + (size_t)k * 24 + 12, ext, order, &x, &y, &z);
+    refine_point(T16, accept, k, &x, &y, &z);
     ox[t] = x; oy[t] = y; oz[t] = z;
     if (oi) oi[t] = in.i[i];
 }
@@ -969,11 +971,19 @@ __global__ void __launch_bounds__(256) global_to_scans_kernel(const float* __res
 }
 
 int scans_to_global(ltr_ctx* ctx, const DevScanSet& scans, int64_t base, int64_t n, const double* poses, const double* ext, float* ox,
-                    float* oy, float* oz, float* oi) {
+                    float* oy, float* oz, float* oi, const float* T16, const uint8_t* accept) {
     if (n == 0) return LTR_OK;
     scans_to_global_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(view(scans.pts), scans.d_off, scans.K, base, n, poses, ext,
-                                                                                ctx->cfg.transform_order, ox, oy, oz, oi);
+                                                                                ctx->cfg.transform_order, ox, oy, oz, oi, T16, accept);
     LTR_LAUNCH_CHECK(ctx);
+    return LTR_OK;
+}
+
+int upload_refinement(ltr_ctx* ctx, int K, const float* T16, const uint8_t* accepted, float* dT, uint8_t* dacc) {
+    std::vector<uint8_t> acc((size_t)K);
+    for (int j = 0; j < K; ++j) acc[j] = accepted[j] ? 1 : 0;
+    LTR_CUDA(ctx, cudaMemcpyAsync(dT, T16, (size_t)K * 64, cudaMemcpyHostToDevice, ctx->stream));
+    LTR_CUDA(ctx, cudaMemcpyAsync(dacc, acc.data(), (size_t)K, cudaMemcpyHostToDevice, ctx->stream));
     return LTR_OK;
 }
 

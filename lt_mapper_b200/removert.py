@@ -30,7 +30,7 @@ class Params(ctypes.Structure):
 
 
 HOST_EXPORTS = ["ltrh_params_default", "ltrh_create", "ltrh_destroy", "ltrh_last_error", "ltrh_context", "ltrh_comm_init_nccl", "ltrh_owns_session", "ltrh_invert_poses",
-                "ltrh_load_session", "ltrh_load_session_raw", "ltrh_run_step0", "ltrh_run_step12", "ltrh_run_step3", "ltrh_reset_to_step0", "ltrh_cascade_promote_updated", "ltrh_set_delta_maps", "ltrh_delta_load", "ltrh_delta_count", "ltrh_compose_changes", "ltrh_rollback", "ltrh_scanside_removal", "ltrh_set_icp_refinement", "ltrh_set_adaptive_threshold", "ltrh_set_map_ball", "ltrh_icp_stats", "ltrh_stage", "ltrh_cloud",
+                "ltrh_load_session", "ltrh_load_session_raw", "ltrh_run_step0", "ltrh_run_step12", "ltrh_run_step3", "ltrh_reset_to_step0", "ltrh_cascade_promote_updated", "ltrh_set_delta_maps", "ltrh_delta_load", "ltrh_delta_count", "ltrh_compose_changes", "ltrh_rollback", "ltrh_scanside_removal", "ltrh_scanside_removal_registered", "ltrh_set_icp_refinement", "ltrh_set_adaptive_threshold", "ltrh_set_map_ball", "ltrh_icp_stats", "ltrh_scanside_icp_stats", "ltrh_stage", "ltrh_cloud",
                 "ltrh_scanset", "ltrh_timing", "ltrh_log_count", "ltrh_log_get", "ltrh_io_last_error", "ltrh_io_read_pcd", "ltrh_io_write_pcd",
                 "ltrh_io_read_poses", "ltrh_io_parse_keyframes", "ltrh_io_parse_keyframes_in_roi", "ltrh_io_voxel_grid", "ltrh_io_voxel_grid_scans", "ltrh_io_yaml_get"]
 
@@ -68,10 +68,12 @@ def host_lib():
     L.ltrh_compose_changes.argtypes = [vp, i32, i32]
     L.ltrh_rollback.argtypes = [vp, i32]
     L.ltrh_scanside_removal.argtypes = [vp, i32, i32, i32]
+    L.ltrh_scanside_removal_registered.argtypes = [vp, i32, i32, i32]
     L.ltrh_set_icp_refinement.argtypes = [vp, i32]
     L.ltrh_set_adaptive_threshold.argtypes = [vp, ctypes.c_float]
     L.ltrh_set_map_ball.argtypes = [vp, ctypes.c_float]
     L.ltrh_icp_stats.argtypes = [vp, i32, i32, P(i32), vp, vp, vp, vp, vp]
+    L.ltrh_scanside_icp_stats.argtypes = [vp, i32, i32, P(i32), vp, vp, vp, vp, vp]
     L.ltrh_stage.argtypes = [vp, ctypes.c_char_p]
     L.ltrh_cloud.argtypes = [vp, ctypes.c_char_p, i32, P(i32)]
     L.ltrh_scanset.argtypes = [vp, ctypes.c_char_p, i32, P(i32)]
@@ -241,6 +243,11 @@ class Removerter:
         """scansideRemovalForEachScan (ltrh_scanside_removal): fills the scan sets "scans_static_" / "scans_dynamic_" of scan_sess."""
         self._ck(host_lib().ltrh_scanside_removal(self._h, map_sess, scan_sess, criterion))
 
+    def scanside_removal_registered(self, map_sess, scan_sess, criterion=0):
+        """scansideRemovalForEachScan with isFineRegistration (ltrh_scanside_removal_registered): every keyframe of scan_sess is registered
+        to map_sess's static map at 0.4 m first; fills "scans_static_" / "scans_dynamic_" of scan_sess and scanside_icp_stats(scan_sess)."""
+        self._ck(host_lib().ltrh_scanside_removal_registered(self._h, map_sess, scan_sess, criterion))
+
     def set_icp_refinement(self, on=True):
         """Session::partitionLowDynamicPointsOfScanByKnn's ICP refinement for later Step 2 runs (ltrh_set_icp_refinement; off by default)."""
         self._ck(host_lib().ltrh_set_icp_refinement(self._h, 1 if on else 0))
@@ -258,14 +265,21 @@ class Removerter:
     def icp_stats(self, sess):
         """This rank's refinement of session `sess` in the last Step 2 (ltrh_icp_stats): dict of per-keyframe arrays T (K, 4, 4) float32,
         fitness, iterations, exit (ltr_icp_exit) and accepted (bool); K = 0 when the step ran without refinement."""
+        return self._icp_stats(host_lib().ltrh_icp_stats, sess)
+
+    def scanside_icp_stats(self, sess):
+        """The same for the registration of the last scan-side removal of session `sess`'s scans (ltrh_scanside_icp_stats); K = 0 when
+        it ran without registration."""
+        return self._icp_stats(host_lib().ltrh_scanside_icp_stats, sess)
+
+    def _icp_stats(self, fn, sess):
         K = ctypes.c_int32()
-        self._ck(host_lib().ltrh_icp_stats(self._h, sess, 0, ctypes.byref(K), None, None, None, None, None))
+        self._ck(fn(self._h, sess, 0, ctypes.byref(K), None, None, None, None, None))
         n = K.value
         T = np.empty((n, 4, 4), np.float32); fit = np.empty(n, np.float64); it = np.empty(n, np.int32); ex = np.empty(n, np.int32)
         acc = np.empty(n, np.uint8)
         if n:
-            self._ck(host_lib().ltrh_icp_stats(self._h, sess, n, ctypes.byref(K), T.ctypes.data, fit.ctypes.data, it.ctypes.data, ex.ctypes.data,
-                                               acc.ctypes.data))
+            self._ck(fn(self._h, sess, n, ctypes.byref(K), T.ctypes.data, fit.ctypes.data, it.ctypes.data, ex.ctypes.data, acc.ctypes.data))
         return {"T": T, "fitness": fit, "iterations": it, "exit": ex, "accepted": acc.astype(bool)}
 
     def stage(self, name):
